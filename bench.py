@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- the GAN training step of the reference's hot path on B200, one JSON line per run.
+"""bench.py -- the GAN training step of the reference's hot path on H100, one JSON line per run.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|stock|reference]
-                    [--config dcgan|wgan_gp|pix2pix|cyclegan]
+                    [--config dcgan|wgan_gp|pix2pix|cyclegan] [--dump-outputs DIR]
 
 Default: BASELINE configs[1] -- DCGAN 64x64, batch 128 per GPU, the full G+D step of dcgan.py:146-183, images/sec.
 N > 1 is launched by torchrun (one rank per GPU, NCCL, weak scaling).  Rank 0 prints ONE JSON line.
@@ -17,8 +17,11 @@ Keys of the line (DESIGN.md section 5):
   e2e            the same step driven from pinned HOST buffers: H2D of the inputs every step, D2H of the losses
   gpu_reference  (N = 1, --impl ours) the stock arm measured in the same process on the same GPU
   roofline       the time-dominant kernel group of the step timed alone with CUDA events against its bound, plus the
-                 tcgen05 conv kernels against the TF32 peak and the whole step in reference-form FLOPs
+                 wgmma conv kernels against the TF32 peak and the whole step in reference-form FLOPs
   cpu_baseline   the oracle restatement of the reference step on the host cores (N = 1 only)
+
+--dump-outputs DIR writes what the last timed step computed (its losses and the parameters it updated, see
+dump_outputs) as .npy files, so that two builds can be compared output for output on identical seeded inputs.
 """
 import argparse
 import json
@@ -61,6 +64,8 @@ def parse_args():
     ap.add_argument("--no-gpu-reference", action="store_true")
     ap.add_argument("--no-roofline", action="store_true")
     ap.add_argument("--no-graph", action="store_true", help="eager step loop (debugging)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step to DIR/<name>.npy")
     a = ap.parse_args()
     if a.steps is None:
         a.steps = {"dcgan": 50, "wgan_gp": 200, "pix2pix": 20, "cyclegan": 10}[a.config]
@@ -120,8 +125,8 @@ def measured_peaks():
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(path):
         d = json.load(open(path))
-        return d.get("hbm_gbs", 6650.0), d.get("bf16_tflops", 1590.0), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, 1590.0, "fallback (B200_PROFILING.md)"
+        return d.get("hbm_gbs", 3350.0), d.get("bf16_tflops", 989.0), "measured (MEASURED_PEAKS.json)"
+    return 3350.0, 989.0, "H100 SXM data sheet (700 W; dense)"
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -246,7 +251,7 @@ def dcgan_kernel_groups(torch, batch, hbm_peak, tf32_peak, iters=20):
                         ("dgrad", lambda: ops.conv_dgrad(g, dy, pd, ALGO_TC)),
                         ("wgrad", lambda: ops.conv_wgrad(g, x, dy, tuple(w.shape), False, ALGO_TC))):
             ms = _event_time(torch, fn, iters)
-            out.append({"kernel": f"{name} {pas} (tcgen05 TF32, Upsample x2 folded)", "bound": "tensor", "ms": ms,
+            out.append({"kernel": f"{name} {pas} (wgmma TF32, Upsample x2 folded)", "bound": "tensor", "ms": ms,
                         "achieved": flops / ms / 1e9, "peak": tf32_peak, "unit": "TFLOP/s", "frac": flops / ms / 1e9 / tf32_peak,
                         "algorithmic_mbytes": nbytes / 1e6, "executed_gflop": flops / 1e9, "per_step": 1})
 
@@ -265,7 +270,7 @@ def dcgan_kernel_groups(torch, batch, hbm_peak, tf32_peak, iters=20):
         gimg = torch.randn(batch, 1, img, img, device="cuda")
         ms = _event_time(torch, lambda: ops.tail_fprop(d, a, ss, w3, b3), iters)
         nb = a.numel() * 4 + gimg.numel() * 4
-        out.append({"kernel": "G tail fprop: BN+LReLU+Conv 64->1+Tanh (tcgen05 on transformed tiles)", "bound": "hbm",
+        out.append({"kernel": "G tail fprop: BN+LReLU+Conv 64->1+Tanh (wgmma on transformed tiles)", "bound": "hbm",
                     "ms": ms, "achieved": nb / ms / 1e6, "peak": hbm_peak, "unit": "GB/s", "frac": nb / ms / 1e6 / hbm_peak,
                     "algorithmic_mbytes": nb / 1e6, "per_step": 1})
         ms = _event_time(torch, lambda: ops.tail_bwd(d, a, mr, ss, w3, gimg, True, True, True), iters)
@@ -342,6 +347,7 @@ def build_job(torch, config, stock, dev, world, rank):
             gl, dl, _ = train.dcgan_step(g, d, og, od, imgs, z, loss, valid, fake, rg, rd)
             return torch.stack([gl, dl])
         pools = [images(1), [torch.randn(B, LATENT, generator=gen).pin_memory() for _ in range(pool_n)]]
+        nets = [("generator", g), ("discriminator", d)]
     elif config == "wgan_gp":
         g = zoo.WGANGPGenerator((1, img, img), nn=ns).to(dev)
         d = zoo.WGANGPDiscriminator((1, img, img), nn=ns).to(dev)
@@ -354,6 +360,7 @@ def build_job(torch, config, stock, dev, world, rank):
             return torch.stack([dl, gp])
         pools = [images(1), [torch.randn(B, LATENT, generator=gen).pin_memory() for _ in range(pool_n)],
                  [torch.rand(B, 1, 1, 1, generator=gen).pin_memory() for _ in range(pool_n)]]
+        nets = [("discriminator", d)]
     elif config == "pix2pix":
         g, d = zoo.GeneratorUNet(nn=ns).to(dev), zoo.Pix2PixDiscriminator(nn=ns).to(dev)
         g.apply(zoo.weights_init_normal)
@@ -365,6 +372,7 @@ def build_job(torch, config, stock, dev, world, rank):
             lg, ld = train.pix2pix_step(g, d, og, od, a, b, reduce_g=rg, reduce_d=rd)
             return torch.stack([lg, ld])
         pools = [images(3), images(3)]
+        nets = [("generator", g), ("discriminator", d)]
     else:
         shape = (3, img, img)
         nets = [zoo.GeneratorResNet(shape, 9, nn=ns), zoo.GeneratorResNet(shape, 9, nn=ns),
@@ -382,12 +390,29 @@ def build_job(torch, config, stock, dev, world, rank):
             lg, ld = train.cyclegan_step(*nets, og, oa, ob, a, b, None, None, reduce_g=rg, reduce_d_a=ra, reduce_d_b=rb)
             return torch.stack([lg, ld])
         pools = [images(3), images(3)]
-    return step, pools, 8
+        named = list(zip(("generator_ab", "generator_ba", "discriminator_a", "discriminator_b"), nets))
+        return step, pools, 8, named
+    return step, pools, 8, nets
 
 
-def time_job(torch, dist, args, stock, dev, world, rank, local, steps, warmup, clocks=False):
+def dump_outputs(torch, path, losses, nets, cap=2_000_000):
+    """Writes what the last timed step computed: the losses it returned (losses.npy, float64) and the parameters it
+    updated (<net>_params.npy, float32, all of them flattened in parameters() order; a network with more than `cap`
+    values is sampled at fixed seeded positions), at most 8 MB per network."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    np.save(os.path.join(path, "losses.npy"), losses.detach().double().cpu().numpy())
+    for name, net in nets:
+        flat = torch.cat([p_.detach().reshape(-1) for p_ in net.parameters()]).float().cpu()
+        if flat.numel() > cap:
+            idx = torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(0))[:cap].sort().values
+            flat = flat[idx]
+        np.save(os.path.join(path, f"{name}_params.npy"), flat.numpy())
+
+
+def time_job(torch, dist, args, stock, dev, world, rank, local, steps, warmup, clocks=False, dump_dir=None):
     from b200gan import _lib, train
-    step, pools, d2h = build_job(torch, args.config, stock, dev, world, rank)
+    step, pools, d2h, nets = build_job(torch, args.config, stock, dev, world, rank)
     pool_n = len(pools[0])
     dev_pools = [[t.to(dev) for t in p] for p in pools]
     torch.manual_seed(99 + rank)  # dropout streams differ per rank
@@ -430,6 +455,8 @@ def time_job(torch, dist, args, stock, dev, world, rank, local, steps, warmup, c
     clk = sampler.stop() if (sampler and rank == 0) else None
     ms = e0.elapsed_time(e1)
     losses = out.tolist()
+    if dump_dir and rank == 0:
+        dump_outputs(torch, dump_dir, out, nets)
     # e2e: host buffers in, losses out, every step
     for i in range(3):
         runner(*[p[i % pool_n] for p in pools])
@@ -449,7 +476,7 @@ def time_job(torch, dist, args, stock, dev, world, rank, local, steps, warmup, c
     h2d = sum(p[0].numel() * 4 for p in pools)
     res = dict(ms_per_step=ms / steps, ms_per_step_e2e=ms_e2e / steps, losses=losses, clocks=clk, h2d=h2d, d2h=d2h,
                calls_per_step=calls_per_step, graph_error=graph_error)
-    del runner, step
+    del runner, step, nets
     return res
 
 
@@ -495,13 +522,14 @@ def run_gpu(args):
                    "e2e_ms_per_step": r["ms_per_step_e2e"]}
         torch.cuda.empty_cache()
     set_stock_flags(stock)
-    res = time_job(torch, dist, args, stock, dev, world, rank, local, args.steps, args.warmup, clocks=True)
+    res = time_job(torch, dist, args, stock, dev, world, rank, local, args.steps, args.warmup, clocks=True,
+                   dump_dir=args.dump_outputs)
     if rank != 0:
         _finish(world)
         return
 
     hbm_peak, bf16_peak, peak_src = measured_peaks()
-    tf32_peak = bf16_peak / 2.0  # kind::tf32 issues at half the kind::f16 rate (guide: 1.13 vs 2.25 PF nominal)
+    tf32_peak = bf16_peak / 2.0  # dense TF32 issues at half the BF16 rate (H100 SXM data sheet: 495 vs 989 TFLOP/s)
     step_ms = res["ms_per_step"]
     roofline = None
     if not stock and not args.no_roofline and args.config == "dcgan":
@@ -509,19 +537,14 @@ def run_gpu(args):
         for g_ in groups:
             g_["share_of_step"] = g_["ms"] * g_["per_step"] / step_ms
         dom = max(groups, key=lambda g_: g_["share_of_step"])
-        # dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed `ncu --set full` capture of the same
-        # kernels (profiles/r2_ncu_full_tail_kernels_c3.txt; the kernels' traffic is set by the algorithm, not the timing)
-        ncu_traffic = {"G tail fprop": 145.4e6, "G tail backward": 141.6e6 + 218.7e6}
-        dom_traffic = next((v for k_, v in ncu_traffic.items() if dom["kernel"].startswith(k_)), None)
         tc = [g_ for g_ in groups if g_["bound"] == "tensor"]
         roofline = {"kernel": dom["kernel"], "bound": dom["bound"], "achieved": dom["achieved"], "peak": dom["peak"],
                     "unit": dom["unit"], "frac": dom["frac"], "ms_per_launch": dom["ms"],
-                    "share_of_step": dom["share_of_step"], "traffic": dom_traffic,
-                    "traffic_source": "profiles/r2_ncu_full_tail_kernels_c3.txt (bytes per launch)" if dom_traffic else None,
+                    "share_of_step": dom["share_of_step"], "traffic": None,
                     "peak_source": peak_src + ("; TF32 = bf16/2" if dom["bound"] == "tensor" else ""),
                     "step_tensor_fraction_reference_form": cfg["gflop"] / step_ms / tf32_peak,
                     "step_gflop_reference_form": cfg["gflop"],
-                    "tcgen05_kernels_exec_tflops": {g_["kernel"]: round(g_["achieved"], 1) for g_ in tc},
+                    "wgmma_kernels_exec_tflops": {g_["kernel"]: round(g_["achieved"], 1) for g_ in tc},
                     "cublas_tf32_gemm_8192_tflops": cublas_tf32_tflops(torch),
                     "groups": groups}
     elif not stock:
@@ -546,7 +569,7 @@ def run_gpu(args):
         "config": {"workload": cfg["workload"], "global_batch": B * world, "parallelism": f"dp{world}",
                    "cuda_graph": not args.no_graph and res["graph_error"] is None,
                    "cuda_graph_error": res["graph_error"],
-                   "l2": "per-step working set of activations exceeds the 126 MB L2; a pool of distinct input batches; "
+                   "l2": "per-step working set of activations exceeds the 50 MB L2; a pool of distinct input batches; "
                          "no explicit flush",
                    "algo": "stock" if stock else b200gan.Config.algo},
         "e2e": {"value": B * world / res["ms_per_step_e2e"] * 1e3, "unit": cfg["unit"], "h2d_bytes_per_step": res["h2d"],

@@ -1,5 +1,5 @@
 /*
- * b200gan.h -- C ABI of libb200gan.so: the sm_100a implementation of the
+ * b200gan.h -- C ABI of libb200gan.so: the sm_90a implementation of the
  * Generator/Discriminator hot path of eriklindernoren/PyTorch-GAN.
  *
  * The reference has no FFI of its own: its operator boundary is the torch.nn.Module
@@ -35,7 +35,7 @@ enum {
   B200GAN_E_UNSUPPORTED = -1, /* geometry not supported by the requested algorithm */
   B200GAN_E_BAD_ARG = -2,     /* null pointer, misalignment, inconsistent sizes */
   B200GAN_E_CUDA = -3,        /* a CUDA runtime/driver call failed */
-  B200GAN_E_ARCH = -4         /* device is not sm_100 */
+  B200GAN_E_ARCH = -4         /* device is not sm_90 */
 };
 
 /* activation fused into an epilogue / applied by a norm kernel */
@@ -43,9 +43,9 @@ enum { B200GAN_ACT_NONE = 0, B200GAN_ACT_LRELU = 1, B200GAN_ACT_RELU = 2, B200GA
        B200GAN_ACT_SIGMOID = 4 };
 
 /* algorithm selector for the convolution entry points */
-enum { B200GAN_ALGO_AUTO = 0, /* tcgen05 when the geometry qualifies, else SIMT */
+enum { B200GAN_ALGO_AUTO = 0, /* wgmma TF32 when the geometry qualifies, else SIMT */
        B200GAN_ALGO_SIMT = 1, /* fp32 FFMA implicit GEMM (any geometry) */
-       B200GAN_ALGO_TC = 2 }; /* tcgen05 TF32 implicit GEMM (error if unsupported) */
+       B200GAN_ALGO_TC = 2 }; /* wgmma TF32 implicit GEMM (error if unsupported) */
 
 /* padding mode of the (virtual) padded input */
 enum { B200GAN_PAD_ZERO = 0, B200GAN_PAD_REFLECT = 1 };
@@ -54,7 +54,7 @@ enum { B200GAN_PAD_ZERO = 0, B200GAN_PAD_REFLECT = 1 };
 enum {
   B200GAN_PACK_SIMT_FPROP = 0, /* [R][S][Cin][Cout]   : conv fprop / convT dgrad, SIMT        */
   B200GAN_PACK_SIMT_DGRAD = 1, /* [R][S][Cout][Cin]   : conv dgrad / convT fprop, SIMT        */
-  B200GAN_PACK_TC_FPROP = 2,   /* [R*S][Cout][Cin]    tf32-rounded, K-major, tcgen05 fprop    */
+  B200GAN_PACK_TC_FPROP = 2,   /* [R*S][Cout][Cin]    tf32-rounded, K-major, wgmma fprop      */
   B200GAN_PACK_TC_DGRAD = 3,   /* [R*S][Cin][Cout]    tf32-rounded, taps flipped, dgrad       */
   B200GAN_PACK_TC_FPROP_UP2 = 4, /* [4 phases][4 taps][Cout][Cin]: 3x3 s1 p1 conv folded with a
                                     preceding nearest x2 upsample into four 2x2 phase filters  */
@@ -96,13 +96,13 @@ typedef struct b200gan_epilogue {
   const float *chan_scale; /* [N][K] Dropout2d keep-mask / (1-p)  (dcgan.py:77) or NULL    */
   double *stats;           /* [2][G] or NULL                                               */
   int32_t stats_per_sample;
-  int32_t round_tf32;      /* store y rounded to TF32 (RN) so that a following tcgen05 conv
+  int32_t round_tf32;      /* store y rounded to TF32 (RN) so that a following wgmma conv
                               consumes exactly-representable operands                      */
 } b200gan_epilogue;
 
 int b200gan_version(void);
 const char *b200gan_last_error(void);
-/* 0 if the current device is sm_100 and the tcgen05/TMA paths can run, else B200GAN_E_ARCH */
+/* 0 if the current device is sm_90 and the wgmma/TMA paths can run, else B200GAN_E_ARCH */
 int b200gan_check_device(void);
 
 /* ---- weights ------------------------------------------------------------------------ */
@@ -211,7 +211,7 @@ typedef struct b200gan_tail_desc {
 } b200gan_tail_desc;
 int b200gan_tail_supported(const b200gan_tail_desc *d);
 /* out[N][H][W][K] = act_out(conv3x3(act_mid(a * scale + shift), w) + bias); w: the Conv2d parameter [K][C][3][3].
- * The convolution runs on tcgen05 (kind::tf32). */
+ * The convolution runs on wgmma (TF32). */
 int b200gan_tail_fprop(const b200gan_tail_desc *d, const float *a, const float *scale_shift, const float *w,
                        const float *bias, float *out, void *stream);
 /* Backward of the same composite given g = d(loss)/d(conv output before act_out) [N][H][W][K]:
@@ -234,7 +234,7 @@ int b200gan_upsample2x_fwd(const float *x, float *y, int32_t N, int32_t H, int32
 int b200gan_upsample2x_bwd(const float *dy, float *dx, int32_t N, int32_t H, int32_t W, int32_t C,
                            void *stream);
 /* Constant-zero or reflection padding and its gradient (crop / fold), NHWC. */
-/* round_tf32: store RN-rounded TF32 values (the padded copy feeds a tcgen05 conv) */
+/* round_tf32: store RN-rounded TF32 values (the padded copy feeds a wgmma conv) */
 int b200gan_pad2d_fwd(const float *x, float *y, int32_t N, int32_t H, int32_t W, int32_t C,
                       int32_t pad_t, int32_t pad_l, int32_t pad_b, int32_t pad_r, int32_t mode,
                       int32_t round_tf32, void *stream);

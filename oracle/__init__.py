@@ -7,6 +7,6 @@ this package, and only as the checker or the timed CPU baseline -- never from th
 
 Pinning: the reference holds no tests or golden vectors (SURVEY.md section 8c), so this oracle is
 pinned against outputs of the reference itself: oracle/make_golden.py imports/executes the
-reference's own Python from /root/reference in the build container, asserts that the restatement
+reference's own Python from a checkout of the reference (no GPU needed), asserts that the restatement
 reproduces it bit-for-bit on CPU, and commits small fixtures under tests/golden/.
 """

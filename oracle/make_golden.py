@@ -1,8 +1,8 @@
 """Pin the oracle against the reference itself and write the golden fixtures.
 
-Run in the build container (needs /root/reference; the GPU box never runs this):
+Needs a checkout of the reference (no GPU), its path in B200GAN_REFERENCE:
 
-    python oracle/make_golden.py
+    B200GAN_REFERENCE=/path/to/PyTorch-GAN python oracle/make_golden.py
 
 For each model family it (1) executes the reference's own Python (runpy for the flat scripts,
 import for models.py files) under fixed seeds, (2) builds the oracle restatement under the same
@@ -22,7 +22,9 @@ import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-REF = os.environ.get("B200GAN_REFERENCE", "/root/reference")
+REF = os.environ.get("B200GAN_REFERENCE")
+if __name__ == "__main__" and not REF:
+    sys.exit("oracle/make_golden.py: set B200GAN_REFERENCE to a checkout of eriklindernoren/PyTorch-GAN")
 GOLD = os.path.join(ROOT, "tests", "golden")
 sys.path.insert(0, ROOT)
 

@@ -1,4 +1,4 @@
-"""b200gan -- B200-native Generator/Discriminator training hot path behind PyTorch-GAN's own
+"""b200gan -- H100-native (sm_90a) Generator/Discriminator training hot path behind PyTorch-GAN's own
 torch.nn.Module API.  See DESIGN.md / INTEGRATION.md at the repository root."""
 from . import _lib
 from .ops import Config

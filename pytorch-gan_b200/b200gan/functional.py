@@ -27,8 +27,8 @@ class ConvSpec:
     act: int = ACT_NONE
     slope: float = 0.0
     stats: Optional[bool] = None  # None: no fused statistics; False: per channel (BN); True: per sample (IN)
-    rtf_out: bool = False         # round the output to TF32 (it feeds a tcgen05 conv)
-    rtf_dz: bool = False          # round the epilogue-backward output (feeds tcgen05 dgrad/wgrad)
+    rtf_out: bool = False         # round the output to TF32 (it feeds a wgmma conv)
+    rtf_dz: bool = False          # round the epilogue-backward output (feeds wgmma dgrad/wgrad)
 
 
 @dataclass(frozen=True)
@@ -103,7 +103,7 @@ def _pow2ceil(v):
 
 
 def _tc_tile_is_one_image(g, spec):
-    """True when a 128-pixel tile of the tcgen05 fprop never spans two images, the condition for fusing
+    """True when a 128-pixel tile of the wgmma fprop never spans two images, the condition for fusing
     per-sample (InstanceNorm) sums into its epilogue (mirrors the tile choice in conv_tc.cu:run_tc)."""
     if spec.up == 2:
         ho, wo = g.H, g.W                 # per-phase grid of the upsample fold

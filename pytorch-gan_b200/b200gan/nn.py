@@ -84,7 +84,7 @@ def _tc_like(conv, up, full=False):
                 and conv.out_channels % 64 == 0)
     if conv.stride[0] in (1, 2) and conv.in_channels % 32 == 0 and conv.out_channels % 32 == 0:
         return True
-    # fewer than 32 output channels (cyclegan/models.py:82: Conv2d(64, 3, 7)): the FORWARD runs on tcgen05 (weight rows
+    # fewer than 32 output channels (cyclegan/models.py:82: Conv2d(64, 3, 7)): the FORWARD runs on wgmma (weight rows
     # zero-padded to 32 by TMA), the gradients on the fp32 kernels
     return (full is False and not isinstance(conv, _T["ConvTranspose2d"]) and conv.stride[0] == 1
             and conv.in_channels % 32 == 0 and conv.out_channels < 32)

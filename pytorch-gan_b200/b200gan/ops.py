@@ -17,7 +17,7 @@ CL = torch.channels_last
 
 
 class Config:
-    """Global switches. `algo`: 'auto' (tcgen05 where the geometry qualifies) or 'simt'."""
+    """Global switches. `algo`: 'auto' (wgmma TF32 where the geometry qualifies) or 'simt'."""
     algo = os.environ.get("B200GAN_ALGO", "auto")
     weight_cache = True
     # a fused Sequential fed an NCHW-contiguous tensor returns an NCHW-contiguous tensor (what a script may .view,

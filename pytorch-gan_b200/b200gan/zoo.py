@@ -1,8 +1,8 @@
 """The model families of the hot path, built from an `nn` namespace (b200gan.nn by default).
 
-These restate the architectures of the reference scripts so that bench.py / smoke() can run on a
-box where /root/reference does not exist; with the launcher (launch.py) the reference's own
-classes are used unmodified instead.  Citations: implementations/<name>/...
+These restate the architectures of the reference scripts so that bench.py / smoke() can run without
+a checkout of the reference; with the launcher (launch.py) the reference's own classes are used
+unmodified instead.  Citations: implementations/<name>/...
 """
 import types
 

@@ -1,9 +1,9 @@
-"""Build libb200gan.so (sm_100a only) in-tree with nvcc.  No torch headers, no -lcuda.
+"""Build libb200gan.so (sm_90a only) in-tree with nvcc.  No torch headers, no -lcuda.
 
     python pytorch-gan_b200/build.py [--force] [--verbose]
 
 The resulting shared library sits next to the Python package
-(pytorch-gan_b200/b200gan/libb200gan.so), is git-ignored and travels to the GPU box with gpurun.
+(pytorch-gan_b200/b200gan/libb200gan.so) and is git-ignored.
 """
 import argparse
 import concurrent.futures as cf
@@ -18,7 +18,7 @@ OUT = os.path.join(HERE, "b200gan", "libb200gan.so")
 OBJ = os.path.join(HERE, "build")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
     "-DB200GAN_BUILD",
 ]
@@ -46,7 +46,7 @@ def build(force=False, verbose=False):
         return OUT
     if not os.path.exists(NVCC):
         if os.path.exists(OUT):
-            return OUT  # GPU box without a toolchain mismatch: use the shipped library
+            return OUT  # no toolchain: use the library built earlier
         raise RuntimeError("nvcc not found and no prebuilt libb200gan.so")
 
     def compile_one(src):
@@ -66,7 +66,7 @@ def build(force=False, verbose=False):
             if verbose:
                 sys.stderr.write(f"== {src}\n{r.stderr}\n")
             objs.append(obj)
-    link = [NVCC, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", OUT, *objs, "-lcudart"]
+    link = [NVCC, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", OUT, *objs, "-lcudart"]
     r = subprocess.run(link, capture_output=True, text=True)
     if r.returncode != 0:
         sys.stderr.write(r.stdout + r.stderr)

@@ -1,4 +1,4 @@
-// common.cuh -- shared host/device helpers of libb200gan (sm_100a only).
+// common.cuh -- shared host/device helpers of libb200gan (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -40,6 +40,10 @@ void set_error(const char *fmt, ...);
 static inline cudaStream_t as_stream(void *s) { return reinterpret_cast<cudaStream_t>(s); }
 static inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
+
+// SMs of the current device (queried once per device ordinal): grid sizes, split counts and the tile-width choices are
+// planned for it.  Host-only planning queries without a usable device assume the 132 SMs of an H100 SXM.
+int num_sms();
 
 // geometry checks shared by every conv entry point (fills nothing; validates P/Q)
 int validate_geom(const b200gan_conv_geom *g);

@@ -1,7 +1,8 @@
 // conv_api.cu -- C-ABI entry points for convolution: validation, weight packing, and the
-// choice between the tcgen05 TF32 kernels (conv_tc.cu / wgrad_tc.cu) and the fp32 SIMT kernels
+// choice between the wgmma TF32 kernels (conv_tc.cu / wgrad_tc.cu) and the fp32 SIMT kernels
 // (conv_simt.cu).  See include/b200gan.h for the contract and the reference call sites.
 #include "common.cuh"
+#include <atomic>
 #include <mutex>
 #include <string.h>
 #include <stdlib.h>
@@ -51,6 +52,23 @@ void set_error(const char *fmt, ...) {
   va_start(ap, fmt);
   vsnprintf(g_err, sizeof(g_err), fmt, ap);
   va_end(ap);
+}
+
+int num_sms() {
+  static std::atomic<int> cache[64];
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) {
+    cudaGetLastError();
+    return 132;
+  }
+  int v = cache[dev].load(std::memory_order_relaxed);
+  if (v > 0) return v;
+  if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) {
+    cudaGetLastError();
+    return 132;
+  }
+  cache[dev].store(v, std::memory_order_relaxed);
+  return v;
 }
 
 int validate_geom(const b200gan_conv_geom *g) {
@@ -321,8 +339,8 @@ extern "C" int b200gan_check_device(void) {
   B2_CUDA(cudaGetDevice(&dev));
   cudaDeviceProp p;
   B2_CUDA(cudaGetDeviceProperties(&p, dev));
-  if (p.major != 10) {
-    set_error("device %s is sm_%d%d; libb200gan is built for sm_100a only", p.name, p.major, p.minor);
+  if (p.major != 9 || p.minor != 0) {
+    set_error("device %s is sm_%d%d; libb200gan is built for sm_90a only", p.name, p.major, p.minor);
     return B200GAN_E_ARCH;
   }
   return B200GAN_OK;
@@ -388,7 +406,7 @@ extern "C" int b200gan_conv2d_fprop(const b200gan_conv_geom *g, const b200gan_ep
   B2_CHECK_ARG(algo != B200GAN_ALGO_AUTO, "conv2d_fprop: the packed layout fixes the algorithm; pass SIMT or TC");
   cudaStream_t st = as_stream(stream);
   if (algo == B200GAN_ALGO_TC) {
-    if (!tc_supported(g, 0)) B2_UNSUPPORTED("conv2d_fprop: geometry not supported by the tcgen05 path");
+    if (!tc_supported(g, 0)) B2_UNSUPPORTED("conv2d_fprop: geometry not supported by the tensor-core path");
     return tc_fprop(g, ep, x, packed, y, st);
   }
   int rc;
@@ -431,7 +449,7 @@ extern "C" int b200gan_conv2d_dgrad(const b200gan_conv_geom *g, const float *dy,
   B2_CHECK_ARG(algo != B200GAN_ALGO_AUTO, "conv2d_dgrad: pass SIMT or TC explicitly");
   cudaStream_t st = as_stream(stream);
   if (algo == B200GAN_ALGO_TC) {
-    if (!tc_supported(g, 1)) B2_UNSUPPORTED("conv2d_dgrad: geometry not supported by the tcgen05 path");
+    if (!tc_supported(g, 1)) B2_UNSUPPORTED("conv2d_dgrad: geometry not supported by the tensor-core path");
     return tc_dgrad(g, dy, packed, dx, st);
   }
   if (g->transposed) {
@@ -502,7 +520,7 @@ extern "C" int b200gan_conv2d_wgrad(const b200gan_conv_geom *g, const float *x, 
   int a = resolve_algo(g, 2, algo);
   int rc;
   if (a == B200GAN_ALGO_TC) {
-    if (!tc_supported(g, 2)) B2_UNSUPPORTED("conv2d_wgrad: geometry not supported by the tcgen05 path");
+    if (!tc_supported(g, 2)) B2_UNSUPPORTED("conv2d_wgrad: geometry not supported by the tensor-core path");
     rc = tc_wgrad(g, x, dy, dw, workspace, st);
   } else if (fewk_ok(g, 2)) {
     // K <= 4 output channels, stride 1 (the image / patch output layers): lanes = input channels

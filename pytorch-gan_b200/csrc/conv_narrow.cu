@@ -93,7 +93,7 @@ int narrow_wgrad(int N, int H, int W, int Cg, int P, int Q, int Cd, int R, int S
   if (M == 0) return B200GAN_OK;
   const int DT = (Cd % 4 == 0) ? 4 : 1;
   const int64_t nout = (int64_t)R * S * Cg * (Cd / DT);
-  // ~150k threads in total (half of what 148 SMs hold), at least 64 pixels per thread
+  // ~150k threads in total (half of what the SMs hold), at least 64 pixels per thread
   int64_t splits = ceil_div64(150000, nout);
   if (splits > ceil_div64(M, 64)) splits = ceil_div64(M, 64);
   if (splits < 1) splits = 1;

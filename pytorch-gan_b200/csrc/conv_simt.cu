@@ -3,7 +3,7 @@
 // These kernels serve (1) the HBM-bound layers with tiny channel counts where tensor cores
 // cannot be fed (DCGAN discriminator 1->16->32->64->128 k3 s2, dcgan.py:77-88; the 64->1
 // output conv dcgan.py:62; pix2pix/cyclegan C=3 edge layers) and (2) every other geometry as
-// the always-correct fp32 path that the tcgen05 kernels are validated against on the GPU.
+// the always-correct fp32 path that the wgmma kernels are validated against on the GPU.
 //
 // One gather function maps an output pixel + filter tap to the stored input pixel, covering
 // stride, zero / reflection padding (cyclegan/models.py:27,49), a folded nearest x2 upsample
@@ -807,7 +807,7 @@ int simt_gather_gemm(int N, int H, int W, int C, int P, int Q, int K, int R, int
     const int L = C >= 128 ? 32 : (C >= 64 ? 16 : (C >= 32 ? 8 : 4));
     const int64_t ngroups = (int64_t)N * H * ((W + 3) / 4);
     int64_t blocks = ceil_div64(ngroups, 8 * (32 / L));
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > num_sms() * 16) blocks = num_sms() * 16;
 #define LAUNCH_SK(LL, KK_) conv3x3s1_smallk_kernel<LL, KK_><<<(unsigned)blocks, 256, wbytes, st>>>(x, wp, y, e, N, H, W, C, dir)
 #define LAUNCH_SK_L(KK_) \
   do { if (L == 32) LAUNCH_SK(32, KK_); else if (L == 16) LAUNCH_SK(16, KK_); else if (L == 8) LAUNCH_SK(8, KK_); else LAUNCH_SK(4, KK_); } while (0)
@@ -819,7 +819,7 @@ int simt_gather_gemm(int N, int H, int W, int C, int P, int Q, int K, int R, int
   }
   if (s3 && C <= 4 && K % 8 == 0 && wbytes <= 48 * 1024) {
     int64_t blocks = ceil_div64(M * (K / 8), 256);
-    if (blocks > 148 * 32) blocks = 148 * 32;
+    if (blocks > num_sms() * 32) blocks = num_sms() * 32;
     if (C == 1) conv3x3s1_smallc_kernel<1><<<(unsigned)blocks, 256, wbytes, st>>>(x, wp, y, e, N, H, W, K, dir);
     else if (C == 2) conv3x3s1_smallc_kernel<2><<<(unsigned)blocks, 256, wbytes, st>>>(x, wp, y, e, N, H, W, K, dir);
     else if (C == 3) conv3x3s1_smallc_kernel<3><<<(unsigned)blocks, 256, wbytes, st>>>(x, wp, y, e, N, H, W, K, dir);
@@ -829,7 +829,7 @@ int simt_gather_gemm(int N, int H, int W, int C, int P, int Q, int K, int R, int
   }
   if (K <= 4 && C % 4 == 0 && C >= 16 && wbytes <= 48 * 1024 && aligned) {
     // few output channels: lanes over channels (float4), several pixels in flight per lane group
-    const int64_t blocks_max = 148 * 8;
+    const int64_t blocks_max = num_sms() * 8;
     if (C >= 128) {
       int64_t blocks = ceil_div64(M, 8 * 1 * 4);
       if (blocks > blocks_max) blocks = blocks_max;
@@ -849,11 +849,11 @@ int simt_gather_gemm(int N, int H, int W, int C, int P, int Q, int K, int R, int
     }
   } else if (K <= 4 && C >= 32 && wbytes <= 48 * 1024) {
     int64_t blocks = ceil_div64(M, 8);
-    if (blocks > 148 * 64) blocks = 148 * 64;
+    if (blocks > num_sms() * 64) blocks = num_sms() * 64;
     conv_gather_smallk_kernel<4><<<(unsigned)blocks, 256, wbytes, st>>>(g, e, x, wp, y, K);
   } else if (C <= 8 && K % 4 == 0 && K >= 8 && wbytes <= 48 * 1024 && aligned) {
     int64_t blocks = ceil_div64(M * (K / 4), 256);
-    if (blocks > 148 * 32) blocks = 148 * 32;
+    if (blocks > num_sms() * 32) blocks = num_sms() * 32;
     conv_smallc_kernel<<<(unsigned)blocks, 256, wbytes, st>>>(g, e, x, wp, y, K);
   } else {
     if (mode == 1 && stride > 1 && stride <= 4) {
@@ -884,7 +884,7 @@ int simt_wgrad(int N, int H, int W, int Cg, int P, int Q, int Cd, int R, int S, 
   if (Cd == 1 && R == 3 && S == 3 && stride == 1 && pad_t == 1 && pad_l == 1 && up == 1 && pad_mode == B200GAN_PAD_ZERO &&
       P == H && Q == W && Cg % 4 == 0 && Cg >= 16 && Cg <= 128 && ((uintptr_t)xg % 16 == 0)) {
     const int L = Cg >= 128 ? 32 : (Cg >= 64 ? 16 : (Cg >= 32 ? 8 : 4));
-    int64_t blocks = 148 * 4;
+    int64_t blocks = num_sms() * 4;
     int64_t ppb = ceil_div64(M, blocks);
     if (ppb < 256) ppb = 256;
     blocks = ceil_div64(M, ppb);
@@ -897,7 +897,7 @@ int simt_wgrad(int N, int H, int W, int Cg, int P, int Q, int Cd, int R, int S, 
   }
   if (Cd <= 4) {
     int yb = ceil_div(Ktot, 256);
-    int64_t xb = (148 * 8) / yb;
+    int64_t xb = (num_sms() * 8) / yb;
     if (xb < 1) xb = 1;
     int64_t m_per_block = ceil_div64(M, xb);
     if (m_per_block < 64) m_per_block = 64;
@@ -907,7 +907,7 @@ int simt_wgrad(int N, int H, int W, int Cg, int P, int Q, int Cd, int R, int S, 
     return B200GAN_OK;
   }
   int tiles = ceil_div(Ktot, FBM) * ceil_div(Cd, FBN);
-  int64_t splits = (148 * 4 + tiles - 1) / tiles;
+  int64_t splits = (num_sms() * 4 + tiles - 1) / tiles;
   int64_t max_splits = ceil_div64(M, 128);
   if (splits > max_splits) splits = max_splits;
   if (splits < 1) splits = 1;
@@ -923,7 +923,7 @@ int simt_wgrad(int N, int H, int W, int Cg, int P, int Q, int Cd, int R, int S, 
 int simt_colsum(const float *x, float *out, int64_t M, int C, cudaStream_t st) {
   B2_CUDA(cudaMemsetAsync(out, 0, (size_t)C * sizeof(float), st));
   if (M == 0) return B200GAN_OK;
-  int64_t yb = 148 * 8 / ceil_div(C, 32);
+  int64_t yb = num_sms() * 8 / ceil_div(C, 32);
   if (yb < 1) yb = 1;
   int64_t rows = ceil_div64(M, yb);
   if (rows < 64) rows = 64;

@@ -1,26 +1,27 @@
-// conv_tc.cu -- tcgen05 TF32 implicit-GEMM convolution (fprop and dgrad) for sm_100a.
+// conv_tc.cu -- wgmma TF32 implicit-GEMM convolution (fprop and dgrad) for sm_90a.
 //
 // Hot path of the reference: the big Generator convolutions
 //   Upsample(x2) -> Conv2d(128,128,3,1,1)   dcgan.py:54-55
 //   Upsample(x2) -> Conv2d(128, 64,3,1,1)   dcgan.py:58-59
 // and every other stride-1 convolution with >= 32 input channels (cyclegan/models.py:28,32,75).
 //
-// Formulation.  y[m][k] = sum_taps sum_c A_tap[m][c] * B_tap[k][c], m = output pixel, accumulated in
-// TMEM by tcgen05.mma (kind::tf32, M = 128, N = BN).  No im2col buffer ever exists: the A tile of a
-// tap is a rank-5 TMA box {32 channels, BW, 1, BH, BNn} of the NHWC activation tensor shifted by the
-// tap offset; TMA zero-fills out-of-bounds coordinates, which *is* the zero padding.  The box lands
-// in shared memory as 128 rows x 128 B with the 128-byte swizzle -- exactly the K-major UMMA operand
-// layout.  B tiles come from the packed weight matrix [tap][Cout][Cin] (tf32-rounded at pack time).
+// Formulation.  y[m][k] = sum_taps sum_c A_tap[m][c] * B_tap[k][c], m = output pixel, accumulated in registers by
+// wgmma (TF32, M = 64 per warpgroup, N = BN).  No im2col buffer ever exists: the A tile of a tap is a rank-5 TMA box
+// {32 channels, BW, 1, BH, BNn} of the NHWC activation tensor shifted by the tap offset; TMA zero-fills out-of-bounds
+// coordinates, which *is* the zero padding.  The box lands in shared memory as 128 rows x 128 B with the 128-byte
+// swizzle -- exactly the K-major wgmma operand layout.  B tiles come from the packed weight matrix [tap][Cout][Cin]
+// (tf32-rounded at pack time).
 //
 // A nearest x2 upsample in front of a 3x3 conv is folded into four 2x2 "phase" convolutions on the
 // low-resolution input (B200GAN_PACK_TC_*_UP2): the 4x larger upsampled tensor is never written and
 // 2.25x fewer MACs are executed.  The data gradient of that composite runs through the same kernel:
 // 16 taps over a rank-5 phase view {2K, Q/2, 2, P/2, N} of dy.
 //
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = TMEM allocator + MMA issuer (one elected
-// thread), warps 2-5 = epilogue (tcgen05.ld -> bias / activation / Dropout2d scale / BatchNorm
-// partial sums -> global).  smem ring of STAGES x (A 16 KB + B BN*128 B), full/empty mbarriers;
-// two CTAs are resident per SM so one CTA's epilogue overlaps the other's main loop.
+// Warp roles (384 threads): warpgroup 0 = TMA producer (one thread), warpgroups 1-2 = consumers, each issuing the
+// wgmma of one 64-pixel half of the 128-pixel tile.  smem ring of STAGES x (A 16 KB + B BN*128 B), full/empty
+// mbarriers.  Epilogue: the consumers write their accumulators into the 128B-swizzled staging tile (the idle pipeline
+// buffers), then each thread takes one pixel row of a 32-channel chunk (bias / activation / Dropout2d scale /
+// BatchNorm partial sums) and one thread issues the TMA bulk tensor stores.
 #include "tc_common.cuh"
 #include <mutex>
 #include <stdlib.h>
@@ -42,7 +43,7 @@ PFN_encodeTiled get_encode_tiled() {
 }
 
 int make_tmap_f32(CUtensorMap *map, const void *base, int rank, const uint64_t *dims, const uint64_t *strides_bytes,
-                  const uint32_t *box, int atom32) {
+                  const uint32_t *box) {
   PFN_encodeTiled enc = get_encode_tiled();
   if (!enc) {
     set_error("cuTensorMapEncodeTiled entry point not available");
@@ -57,7 +58,7 @@ int make_tmap_f32(CUtensorMap *map, const void *base, int rank, const uint64_t *
   }
   for (int i = 0; i < rank - 1; ++i) gs[i] = strides_bytes[i];
   CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, (cuuint32_t)rank, const_cast<void *>(base), gd, gs, bx, es,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, atom32 ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
@@ -76,7 +77,7 @@ constexpr int TC_BM = 128;
 constexpr int TC_BK = 32;  // fp32 elements = 128 bytes = one swizzle row
 constexpr int TC_A_BYTES = TC_BM * TC_BK * 4;
 constexpr int TC_MAX_TAPS = 52;
-constexpr int TC_THREADS = 192;
+constexpr int TC_THREADS = 384;  // producer warpgroup + two consumer warpgroups
 
 struct TcTap {
   int16_t dc;  // channel base offset in the A view (selects the w-parity half of a phase view)
@@ -130,25 +131,87 @@ __device__ __forceinline__ float warp_colsum32(float (&v)[32], int lane) {
   return v[0];  // sum over the 32 lanes of column `lane`
 }
 
-// CL = 2: launched as clusters of two CTAs along x (two neighbouring pixel tiles of the same output-channel tile).  Both
-// need the same weight (B) box every iteration: each CTA fetches HALF of it and multicasts it into both shared memories, so
-// the weights cross L2 -> SM once per pair (at BN = 256 the per-CTA re-fetch of B was 2/3 of the 906 MB a 256->256 residual
-// conv pulls through L2, and L2 -> SM bandwidth, ~10 TB/s, is what the kernel ran at).  A stage is free again only when BOTH
-// CTAs' MMAs on it have retired: the MMA warps commit to the empty barrier of both CTAs (count 2).
-template <int BN, int STAGES, int CL = 1>
-__global__ void __launch_bounds__(TC_THREADS, 2)
+__device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+
+// 32 channels of pixel row m of a staging chunk (128B-swizzled, 128 rows x 128 B)
+__device__ __forceinline__ void ld_row32(const uint8_t *chunk, int m, float (&v)[32]) {
+  const uint8_t *row = chunk + m * 128;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const float4 t = *reinterpret_cast<const float4 *>(row + ((j ^ (m & 7)) << 4));
+    v[4 * j] = t.x; v[4 * j + 1] = t.y; v[4 * j + 2] = t.z; v[4 * j + 3] = t.w;
+  }
+}
+__device__ __forceinline__ void st_row32(uint8_t *chunk, int m, const float (&v)[32]) {
+  uint8_t *row = chunk + m * 128;
+#pragma unroll
+  for (int j = 0; j < 8; ++j)
+    *reinterpret_cast<float4 *>(row + ((j ^ (m & 7)) << 4)) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+}
+
+// bias, activation, Dropout2d scale and TF32 rounding of 32 output channels of one pixel.  Every option is tested ONCE
+// per chunk, never per element: a switch inside the unrolled element loop becomes 32 indirect branches.
+__device__ __forceinline__ void epilogue_chunk(float (&v)[32], const float *bias, int narrow_k, int act, float slope,
+                                               const float *cs, int rtf) {
+  if (bias && narrow_k) {
+#pragma unroll
+    for (int j = 0; j < 32; ++j)
+      if (j < narrow_k) v[j] += __ldg(bias + j);
+  } else if (bias) {
+    const float4 *b4 = reinterpret_cast<const float4 *>(bias);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      float4 b = __ldg(b4 + j);
+      v[4 * j] += b.x; v[4 * j + 1] += b.y; v[4 * j + 2] += b.z; v[4 * j + 3] += b.w;
+    }
+  }
+  if (act == B200GAN_ACT_LRELU) {
+#pragma unroll
+    for (int j = 0; j < 32; ++j) v[j] = v[j] > 0.f ? v[j] : v[j] * slope;
+  } else if (act == B200GAN_ACT_RELU) {
+#pragma unroll
+    for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
+  } else if (act == B200GAN_ACT_TANH) {
+#pragma unroll
+    for (int j = 0; j < 32; ++j) v[j] = tanhf(v[j]);
+  } else if (act == B200GAN_ACT_SIGMOID) {
+#pragma unroll
+    for (int j = 0; j < 32; ++j) v[j] = 1.f / (1.f + __expf(-v[j]));
+  }
+  if (cs) {
+    const float4 *s4 = reinterpret_cast<const float4 *>(cs);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      float4 b = __ldg(s4 + j);
+      v[4 * j] *= b.x; v[4 * j + 1] *= b.y; v[4 * j + 2] *= b.z; v[4 * j + 3] *= b.w;
+    }
+  }
+  if (rtf) {
+#pragma unroll
+    for (int j = 0; j < 32; ++j) v[j] = round_tf32(v[j]);
+  }
+}
+
+// shared-memory budget of conv_tc_kernel: the ring, reused as the staging tile of all BN channels after the last MMA
+template <int BN, int STAGES>
+struct TcSmem {
+  static constexpr int STAGE_BYTES = TC_A_BYTES + BN * TC_BK * 4;
+  static constexpr int RING = STAGES * STAGE_BYTES;
+  static constexpr int STAGING = (BN / 32) * TC_A_BYTES;
+  static constexpr int MAIN = RING > STAGING ? RING : STAGING;
+  static constexpr int TOTAL = MAIN + 1024 + 256 + 4 * BN * 2 * 4;  // + alignment slack, barriers, statistics
+};
+
+template <int BN, int STAGES>
+__global__ void __launch_bounds__(TC_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-               const __grid_constant__ CUtensorMap tmY, const __grid_constant__ TcParams p,
-               const __grid_constant__ CUtensorMap tmBh) {
-  constexpr int B_BYTES = BN * TC_BK * 4;
-  constexpr int STAGE_BYTES = TC_A_BYTES + B_BYTES;
+               const __grid_constant__ CUtensorMap tmY, const __grid_constant__ TcParams p) {
+  using L = TcSmem<BN, STAGES>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t *full = reinterpret_cast<uint64_t *>(smem + STAGES * STAGE_BYTES);
+  uint64_t *full = reinterpret_cast<uint64_t *>(smem + L::MAIN);
   uint64_t *empty = full + STAGES;
-  uint64_t *tmem_full = empty + STAGES;
-  uint32_t *tmem_ptr = reinterpret_cast<uint32_t *>(tmem_full + 1);
-  float *red = reinterpret_cast<float *>(tmem_ptr + 2);  // [4][BN][2]
+  float *red = reinterpret_cast<float *>(smem + L::MAIN + 256);  // [4][BN][2]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int ph = blockIdx.z / p.ksplit, ks = blockIdx.z % p.ksplit;
@@ -166,29 +229,18 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const int it0 = (int)((long long)iters_all * ks / p.ksplit), it1 = (int)((long long)iters_all * (ks + 1) / p.ksplit);
   const int iters = it1 - it0;   // >= 1: the host never asks for more splits than iterations
 
-  if (threadIdx.x == 0) TC_TRACE(0);
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
+    TC_TRACE(0);
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     tma_prefetch_desc(&tmY);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], CL);
+      mbar_init(&empty[s], 2);  // one arrival per consumer warpgroup
     }
-    mbar_init(tmem_full, 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<BN>(tmem_ptr);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  uint32_t crank = 0;
-  if (CL == 2) {
-    crank = cluster_ctarank();
-    cluster_sync_all();   // the peer's barriers exist before anything is multicast at them
-  }
-  const uint32_t tmem = *tmem_ptr;
-  if (threadIdx.x == 0) TC_TRACE(1);
 
   if (warp == 0) {
     if (lane == 0) {
@@ -198,17 +250,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       int tap = it0 / p.kchunks, kc = it0 % p.kchunks;
       for (int it = 0; it < iters; ++it) {
         mbar_wait(&empty[stage], phase ^ 1);
-        uint8_t *sa = smem + stage * STAGE_BYTES;
+        uint8_t *sa = smem + stage * L::STAGE_BYTES;
         uint8_t *sb = sa + TC_A_BYTES;
         const TcTap tp = p.taps[tap0 + tap];
         if (it < 16) TC_TRACE(2 + it);
-        mbar_arrive_expect_tx(&full[stage], STAGE_BYTES);
+        mbar_arrive_expect_tx(&full[stage], L::STAGE_BYTES);
         tma_load_5d(sa, &tmA, &full[stage], tp.dc + kc * TC_BK, w0 + tp.dw, tp.da, h0 + tp.dh, n0);
-        if (CL == 2)   // rows [crank * BN/2, +BN/2) of the B box, into both CTAs
-          tma_load_3d_mc(sb + crank * (B_BYTES / 2), &tmBh, &full[stage], kc * TC_BK, ntile * BN + (int)crank * (BN / 2), tp.bt,
-                         (uint16_t)3);
-        else
-          tma_load_3d(sb, &tmB, &full[stage], kc * TC_BK, ntile * BN, tp.bt);
+        tma_load_3d(sb, &tmB, &full[stage], kc * TC_BK, ntile * BN, tp.bt);
         if (++kc == p.kchunks) {
           kc = 0;
           ++tap;
@@ -219,156 +267,96 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ===== MMA issuer =====
-      constexpr uint32_t idesc = umma_idesc_tf32(TC_BM, BN, 0, 0);
-      int stage = 0;
+  } else if (warp >= 4) {
+    const int ct = threadIdx.x - 128;
+    const int half = ct >> 7;  // consumer warpgroup: MMA rows [64 * half, +64) of the tile
+    {
+      // ===== MMA: the previous stage is released once the wgmma group issued after it has been waited for =====
+      float acc[BN / 2];  // the first MMA overwrites it (scale_d = 0)
+      int stage = 0, prev = 0;
       uint32_t phase = 0;
       for (int it = 0; it < iters; ++it) {
         mbar_wait(&full[stage], phase);
-        tc_fence_after();
-        if (it < 16) TC_TRACE(20 + it);
-        const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
-        const uint32_t sb = sa + TC_A_BYTES;
+        if (ct == 0 && it < 16) TC_TRACE(20 + it);
+        const uint32_t sa = smem_u32(smem + stage * L::STAGE_BYTES) + half * (TC_A_BYTES / 2);
+        const uint32_t sb = smem_u32(smem + stage * L::STAGE_BYTES + TC_A_BYTES);
+        wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < TC_BK / 8; ++k) {
-          uint64_t da = umma_desc_sw128(sa + k * 32, 16, 1024);
-          uint64_t db = umma_desc_sw128(sb + k * 32, 16, 1024);
-          umma_tf32(tmem, da, db, idesc, (it > 0 || k > 0) ? 1u : 0u);
-        }
-        if (CL == 2) umma_commit_mc(&empty[stage], (uint16_t)3);   // ... in both CTAs of the pair
-        else umma_commit(&empty[stage]);  // smem slot reusable once these MMAs retire
+        for (int k = 0; k < TC_BK / 8; ++k)
+          wgmma_tf32<BN>(acc, gmma_desc_sw128(sa + k * 32), gmma_desc_sw128(sb + k * 32), (it > 0 || k > 0) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (it > 0 && (ct & 127) == 0) mbar_arrive(&empty[prev]);
+        prev = stage;
         if (++stage == STAGES) {
           stage = 0;
           phase ^= 1;
         }
       }
-      umma_commit(tmem_full);  // accumulator complete
+      wgmma_wait<0>();
+      wgmma_fence_regs<BN / 2>(acc);
+      consumers_sync();  // every MMA of both halves has retired: the ring is free for the staging tile
+      store_acc_sw128<BN>(smem, acc, half * 64);
     }
-  } else {
-    // ===== epilogue: warps 2..5 own TMEM lane quarters (warp & 3) =====
-    // TMEM -> registers -> (bias, activation, Dropout2d scale, TF32 rounding, BN partial sums) -> shared memory in
-    // the 128B-swizzled box layout -> TMA bulk tensor store.  The pipeline buffers are free once tmem_full fired
-    // (every MMA has retired), so the staging tile reuses them: chunk c (32 channels) at smem + c * 16 KB.
-    const int q = warp & 3;
-    const int m = q * 32 + lane;
+    consumers_sync();
+    // ===== epilogue: thread <-> pixel row m of the tile, the two warpgroups take alternate 32-channel chunks =====
+    const int q = (ct >> 5) & 3;
+    const int m = ct & 127;
     const int lw = m & (BW - 1);
     const int lh = (m >> p.bw_log2) & (BH - 1);
     const int ln = m >> (p.bw_log2 + p.bh_log2);
     const int ow = w0 + lw, oh = h0 + lh, on = n0 + ln;
     const bool valid = (ow < p.Wo) && (oh < p.Ho) && (on < p.N);
-    const float *cs = p.chan_scale ? p.chan_scale + (int64_t)on * p.ldk + ntile * BN : nullptr;
-    const int act = p.act, rtf = p.rtf;
-    const float slope = p.slope;
+    const float *cs = p.chan_scale && valid ? p.chan_scale + (int64_t)on * p.ldk + ntile * BN : nullptr;
     const bool partial = p.ksplit > 1;  // raw partial sums: no bias / activation / statistics (the host checked)
-    mbar_wait(tmem_full, 0);
-    tc_fence_after();
-    if (threadIdx.x == 64) TC_TRACE(40);
-    // The staging tile is written 128 output channels (four 16 KB chunks) at a time: BN = 256 takes two rounds through
-    // the same four buffers, the second one after the first round's TMA stores have finished reading shared memory.
-    constexpr int ROUND = BN < 128 ? BN : 128;
+    if (ct == 0) TC_TRACE(40);
 #pragma unroll 1
-    for (int c0 = 0; c0 < BN; c0 += ROUND) {
-      if (c0 > 0) {
-        if (threadIdx.x == 64) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-      }
-#pragma unroll 1
-      for (int c = c0; c < c0 + ROUND; c += 32) {
-        float v[32];
-        if (threadIdx.x == 64) TC_TRACE(48 + ((c >> 5) & 3) * 3);
-        tmem_ld_32x32(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)c, v);
-        if (threadIdx.x == 64) TC_TRACE(49 + ((c >> 5) & 3) * 3);
-        // every option is tested ONCE per chunk, never per element: a switch inside the unrolled element loop
-        // becomes 32 indirect branches into a 50 KB body and costs ~200 cycles each (measured: 6.5k cycles/chunk)
-        if (p.bias && p.narrow_k) {
+    for (int c = half * 32; c < BN; c += 64) {
+      float v[32];
+      uint8_t *chunk = smem + (c >> 5) * TC_A_BYTES;
+      ld_row32(chunk, m, v);
+      epilogue_chunk(v, p.bias ? p.bias + (p.narrow_k ? 0 : ntile * BN + c) : nullptr, p.narrow_k, p.act, p.slope,
+                     cs ? cs + c : nullptr, p.rtf);
+      if (p.narrow_k) {
+        // fewer than 32 real output channels: one pixel's channels are 4..124 contiguous bytes, written directly
+        if (valid) {
+          float *dst = p.y + ((int64_t)(on * p.Ho + oh) * p.Wo + ow) * p.narrow_k;
 #pragma unroll
           for (int j = 0; j < 32; ++j)
-            if (j < p.narrow_k) v[j] += __ldg(p.bias + j);
-        } else if (p.bias) {
-          const float4 *b4 = reinterpret_cast<const float4 *>(p.bias + ntile * BN + c);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            float4 b = __ldg(b4 + j);
-            v[4 * j] += b.x; v[4 * j + 1] += b.y; v[4 * j + 2] += b.z; v[4 * j + 3] += b.w;
-          }
+            if (j < p.narrow_k) dst[j] = v[j];
         }
-        if (act == B200GAN_ACT_LRELU) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = v[j] > 0.f ? v[j] : v[j] * slope;
-        } else if (act == B200GAN_ACT_RELU) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-        } else if (act == B200GAN_ACT_TANH) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = tanhf(v[j]);
-        } else if (act == B200GAN_ACT_SIGMOID) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = 1.f / (1.f + __expf(-v[j]));
-        }
-        if (cs && valid) {
-          const float4 *s4 = reinterpret_cast<const float4 *>(cs + c);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            float4 b = __ldg(s4 + j);
-            v[4 * j] *= b.x; v[4 * j + 1] *= b.y; v[4 * j + 2] *= b.z; v[4 * j + 3] *= b.w;
-          }
-        }
-        if (rtf) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = round_tf32(v[j]);
-        }
-        if (p.narrow_k) {
-          // fewer than 32 real output channels: one pixel's channels are 4..124 contiguous bytes, written directly
-          if (valid) {
-            float *dst = p.y + ((int64_t)(on * p.Ho + oh) * p.Wo + ow) * p.narrow_k;
-#pragma unroll
-            for (int j = 0; j < 32; ++j)
-              if (j < p.narrow_k) dst[j] = v[j];
-          }
-        } else {
-          uint8_t *row = smem + (((c - c0) >> 5)) * TC_A_BYTES + m * 128;
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            *reinterpret_cast<float4 *>(row + ((j ^ (m & 7)) << 4)) =
-                make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-        }
-        if (threadIdx.x == 64) TC_TRACE(50 + ((c >> 5) & 3) * 3);
-        if (p.stats) {
-          float s2[32];
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            v[j] = valid ? v[j] : 0.f;
-            s2[j] = v[j] * v[j];
-          }
-          float cs1 = warp_colsum32(v, lane);
-          float cs2 = warp_colsum32(s2, lane);
-          red[(q * BN + c + lane) * 2 + 0] = cs1;
-          red[(q * BN + c + lane) * 2 + 1] = cs2;
-        }
+      } else {
+        st_row32(chunk, m, v);
       }
-      if (threadIdx.x == 64) TC_TRACE(43);
-      fence_proxy_async();  // generic-proxy smem writes -> visible to the async (TMA) proxy
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (threadIdx.x == 64 && !p.narrow_k) {
-        TC_TRACE(44);
-#pragma unroll 1
-        for (int c = c0; c < c0 + ROUND; c += 32) {
-          if (partial)
-            tma_reduce_add_5d(&tmY, smem + ((c - c0) >> 5) * TC_A_BYTES, p.out_dc[ph] + ntile * BN + c, w0, p.out_da[ph], h0,
-                              n0);
-          else
-            tma_store_5d(&tmY, smem + ((c - c0) >> 5) * TC_A_BYTES, p.out_dc[ph] + ntile * BN + c, w0, p.out_da[ph], h0, n0);
+      if (p.stats) {
+        float s2[32];
+#pragma unroll
+        for (int j = 0; j < 32; ++j) {
+          v[j] = valid ? v[j] : 0.f;
+          s2[j] = v[j] * v[j];
         }
-        TC_TRACE(45);
-        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+        float cs1 = warp_colsum32(v, lane);
+        float cs2 = warp_colsum32(s2, lane);
+        red[(q * BN + c + lane) * 2 + 0] = cs1;
+        red[(q * BN + c + lane) * 2 + 1] = cs2;
       }
     }
-    if (threadIdx.x == 64) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+    fence_proxy_async();  // generic-proxy smem writes -> visible to the async (TMA) proxy
+    consumers_sync();
+    if (ct == 0 && !p.narrow_k) {
+      TC_TRACE(44);
+#pragma unroll 1
+      for (int c = 0; c < BN; c += 32) {
+        if (partial)
+          tma_reduce_add_5d(&tmY, smem + (c >> 5) * TC_A_BYTES, p.out_dc[ph] + ntile * BN + c, w0, p.out_da[ph], h0, n0);
+        else
+          tma_store_5d(&tmY, smem + (c >> 5) * TC_A_BYTES, p.out_dc[ph] + ntile * BN + c, w0, p.out_da[ph], h0, n0);
+      }
+      tma_store_commit_and_wait_read();
+      TC_TRACE(45);
+    }
     if (p.stats) {
-      asm volatile("bar.sync 1, 128;" ::: "memory");  // every warp's partial sums are in `red`
-      for (int e = threadIdx.x - 64; e < BN; e += 128) {
+      for (int e = ct; e < BN; e += 256) {
         float a = 0.f, b = 0.f;
 #pragma unroll
         for (int qq = 0; qq < 4; ++qq) {
@@ -381,30 +369,23 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
     }
   }
-  if (threadIdx.x == 64) TC_TRACE(41);
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tmem_dealloc<BN>(tmem);
-  }
-  if (CL == 2) cluster_sync_all();   // no CTA leaves while its peer may still signal its barriers
-  if (threadIdx.x == 0) TC_TRACE(42);
+  if (threadIdx.x == 128) TC_TRACE(42);
 }
 
 // ---- all-phase kernel for the folded Upsample(2x)+Conv3x3 forward -------------------------------------------
 // The four output phases of the fold read 2x2 windows of the SAME nine shifted input tiles (dh, dw in {-1,0,1}).  The
 // per-phase kernel above fetches 16 A boxes per k-chunk; this one fetches the 9 distinct ones once and feeds each to
-// every phase that uses it (1, 2 or 4 of the four TMEM accumulators; the centre shift is fetched twice so that a stage
-// holds at most two B boxes and three stages fit): operand ingest per MMA drops from 24 KB to 18 KB,
-// which is what bounds the per-phase kernel (DESIGN.md section 4).  BN = 64: 4 accumulators x 64 columns = 256 TMEM
-// columns, two CTAs per SM still fit (512 columns, 2 x 97 KB of shared memory).
+// every phase that uses it (1, 2 or 4 of the four register accumulators; the centre shift is fetched twice so that a
+// stage holds at most two B boxes): operand ingest per MMA drops from 24 KB to 18 KB.  BN = 64: four accumulators of
+// 64 x 64 per consumer warpgroup = 128 registers per thread.
 constexpr int MP_BN = 64;
-constexpr int MP_STAGES = 3;
+constexpr int MP_STAGES = 6;
 constexpr int MP_B_BYTES = MP_BN * TC_BK * 4;
 constexpr int MP_MAX_USES = 2;  // B boxes per stage; the centre shift (used by all four phases) takes two stages
 constexpr int MP_STEPS = 10;
 constexpr int MP_STAGE_BYTES = TC_A_BYTES + MP_MAX_USES * MP_B_BYTES;
+constexpr int MP_MAIN = MP_STAGES * MP_STAGE_BYTES;  // >= the four 32 KB staging buffers of the epilogue
+static_assert(MP_MAIN >= 4 * 2 * TC_A_BYTES, "all-phase staging buffers");
 
 struct MpStep {
   int8_t dw, dh, nb, pad_;
@@ -412,8 +393,47 @@ struct MpStep {
   int8_t bt[MP_MAX_USES];   // tap block of each use in the packed weight matrix
 };
 
+// The fixed step schedule: shifts (dh, dw) in row-major order, one stage per shift (the centre shift, read by all four
+// phases, takes two); phase (a,b) reads shift (dh,dw) through its tap (dr,ds) = (dh-a+1, dw-b+1) when both are in {0,1}.
+// A compile-time table, so that the consumers pick each MMA's accumulator statically.
+struct MpSchedule {
+  MpStep s[MP_STEPS];
+  int n;
+};
+__host__ __device__ constexpr MpSchedule mp_schedule() {
+  MpSchedule r{};
+  for (int dh = -1; dh <= 1; ++dh)
+    for (int dw = -1; dw <= 1; ++dw) {
+      int cur = -1;
+      for (int a = 0; a < 2; ++a)
+        for (int b = 0; b < 2; ++b) {
+          const int dr = dh - a + 1, ds = dw - b + 1;
+          if (dr < 0 || dr > 1 || ds < 0 || ds > 1) continue;
+          if (cur < 0 || r.s[cur].nb == MP_MAX_USES) {
+            cur = r.n++;
+            r.s[cur].dw = (int8_t)dw;
+            r.s[cur].dh = (int8_t)dh;
+          }
+          const int ph = a * 2 + b;
+          r.s[cur].acc[r.s[cur].nb] = (int8_t)ph;
+          r.s[cur].bt[r.s[cur].nb] = (int8_t)(ph * 4 + dr * 2 + ds);
+          ++r.s[cur].nb;
+        }
+    }
+  return r;
+}
+static_assert(mp_schedule().n == MP_STEPS, "all-phase step schedule");
+// true when use U of step S is the first MMA into its accumulator (it overwrites: scale_d = 0 on its first k-chunk)
+__host__ __device__ constexpr bool mp_first_use(int S, int U) {
+  const MpSchedule r = mp_schedule();
+  for (int s = 0; s <= S; ++s)
+    for (int u = 0; u < r.s[s].nb && (s < S || u < U); ++u)
+      if (r.s[s].acc[u] == r.s[S].acc[U]) return false;
+  return true;
+}
+
 struct MpParams {
-  MpStep steps[MP_STEPS];
+  MpStep steps[MP_STEPS];  // = mp_schedule() (the producer's copy)
   int32_t kout_total, kchunks, bw_log2, bh_log2, tiles_w, tiles_h, N, Ho, Wo;
   int32_t out_dc[4], out_da[4];
   int32_t ldk;
@@ -426,17 +446,60 @@ struct MpParams {
   long long *trace;  // bring-up: per-CTA clock64 timeline (64 slots per CTA) or nullptr
 };
 
-__global__ void __launch_bounds__(TC_THREADS, 2)
+// use U of step S: four K8 slices of one B box into the accumulator of its phase
+template <int S, int U>
+__device__ __forceinline__ void mp_mma_use(float *acc0, float *acc1, float *acc2, float *acc3, uint32_t sa, uint32_t sb,
+                                           bool first_chunk) {
+  constexpr int A = mp_schedule().s[S].acc[U];
+  constexpr bool fresh = mp_first_use(S, U);
+#pragma unroll
+  for (int k = 0; k < TC_BK / 8; ++k) {
+    const uint64_t da = gmma_desc_sw128(sa + k * 32), db = gmma_desc_sw128(sb + k * 32);
+    const uint32_t scale_d = (fresh && first_chunk && k == 0) ? 0u : 1u;
+    if constexpr (A == 0) wgmma_tf32<MP_BN>(acc0, da, db, scale_d);
+    else if constexpr (A == 1) wgmma_tf32<MP_BN>(acc1, da, db, scale_d);
+    else if constexpr (A == 2) wgmma_tf32<MP_BN>(acc2, da, db, scale_d);
+    else wgmma_tf32<MP_BN>(acc3, da, db, scale_d);
+  }
+}
+
+// consumer side of steps S.. : every k-chunk of step S is one stage of the ring; the previous stage is released once the
+// wgmma group issued after it has been waited for
+template <int S>
+__device__ __forceinline__ void mp_consume(float *acc0, float *acc1, float *acc2, float *acc3, uint8_t *smem, uint64_t *full,
+                                           uint64_t *empty, int kchunks, int half, bool leader, int &stage, uint32_t &phase,
+                                           int &prev, int &it) {
+  constexpr int NB = mp_schedule().s[S].nb;
+#pragma unroll 1
+  for (int kc = 0; kc < kchunks; ++kc, ++it) {
+    mbar_wait(&full[stage], phase);
+    const uint32_t base = smem_u32(smem + stage * MP_STAGE_BYTES);
+    const uint32_t sa = base + half * (TC_A_BYTES / 2);
+    wgmma_fence();
+    mp_mma_use<S, 0>(acc0, acc1, acc2, acc3, sa, base + TC_A_BYTES, kc == 0);
+    if constexpr (NB > 1) mp_mma_use<S, 1>(acc0, acc1, acc2, acc3, sa, base + TC_A_BYTES + MP_B_BYTES, kc == 0);
+    wgmma_commit();
+    wgmma_wait<1>();
+    if (it > 0 && leader) mbar_arrive(&empty[prev]);
+    prev = stage;
+    if (++stage == MP_STAGES) {
+      stage = 0;
+      phase ^= 1;
+    }
+  }
+  if constexpr (S + 1 < MP_STEPS)
+    mp_consume<S + 1>(acc0, acc1, acc2, acc3, smem, full, empty, kchunks, half, leader, stage, phase, prev, it);
+}
+
+__global__ void __launch_bounds__(TC_THREADS, 1)
 conv_tc_up2_allphase_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                             const __grid_constant__ CUtensorMap tmY, const __grid_constant__ MpParams p) {
   constexpr int BN = MP_BN;
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t *full = reinterpret_cast<uint64_t *>(smem + MP_STAGES * MP_STAGE_BYTES);
+  uint64_t *full = reinterpret_cast<uint64_t *>(smem + MP_MAIN);
   uint64_t *empty = full + MP_STAGES;
-  uint64_t *tmem_full = empty + MP_STAGES;
-  uint32_t *tmem_ptr = reinterpret_cast<uint32_t *>(tmem_full + 1);
-  float *red = reinterpret_cast<float *>(tmem_ptr + 2);  // [4][BN][2]
+  float *red = reinterpret_cast<float *>(smem + MP_MAIN + 256);  // [4][BN][2]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int ntile = blockIdx.y;
@@ -449,25 +512,19 @@ conv_tc_up2_allphase_kernel(const __grid_constant__ CUtensorMap tmA, const __gri
   const int w0 = tw << p.bw_log2, h0 = th << p.bh_log2;
   const int n0 = tn * (TC_BM >> (p.bw_log2 + p.bh_log2));
   const int iters = MP_STEPS * p.kchunks;
-  if (threadIdx.x == 0) TC_TRACE(0);
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
+    TC_TRACE(0);
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     tma_prefetch_desc(&tmY);
     for (int s = 0; s < MP_STAGES; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
+      mbar_init(&empty[s], 2);
     }
-    mbar_init(tmem_full, 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<4 * BN>(tmem_ptr);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_ptr;
-  if (threadIdx.x == 0) TC_TRACE(1);
 
   if (warp == 0) {
     if (lane == 0) {
@@ -479,7 +536,6 @@ conv_tc_up2_allphase_kernel(const __grid_constant__ CUtensorMap tmA, const __gri
         uint8_t *sa = smem + stage * MP_STAGE_BYTES;
         const MpStep sp = p.steps[step];
         if (it < 16) TC_TRACE(2 + it);
-        if (it == iters - 1) TC_TRACE(18);
         mbar_arrive_expect_tx(&full[stage], TC_A_BYTES + sp.nb * MP_B_BYTES);
         tma_load_5d(sa, &tmA, &full[stage], kc * TC_BK, w0 + sp.dw, 0, h0 + sp.dh, n0);
 #pragma unroll 1
@@ -496,170 +552,92 @@ conv_tc_up2_allphase_kernel(const __grid_constant__ CUtensorMap tmA, const __gri
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ===== MMA issuer: one A box feeds every phase that reads this shift =====
-      constexpr uint32_t idesc = umma_idesc_tf32(TC_BM, BN, 0, 0);
-      int stage = 0, step = 0, kc = 0;
-      uint32_t phase = 0, touched = 0;
-      for (int it = 0; it < iters; ++it) {
-        mbar_wait(&full[stage], phase);
-        tc_fence_after();
-        if (it < 16) TC_TRACE(20 + it);
-        if (it == iters - 1) TC_TRACE(36);
-        const MpStep sp = p.steps[step];
-        const uint32_t sa = smem_u32(smem + stage * MP_STAGE_BYTES);
-#pragma unroll 1
-        for (int u = 0; u < sp.nb; ++u) {
-          const uint32_t sb = sa + TC_A_BYTES + u * MP_B_BYTES;
-          const uint32_t acc = (uint32_t)sp.acc[u];
-          const uint32_t fresh = ((touched >> acc) & 1u) ^ 1u;
-#pragma unroll
-          for (int k = 0; k < TC_BK / 8; ++k) {
-            uint64_t da = umma_desc_sw128(sa + k * 32, 16, 1024);
-            uint64_t db = umma_desc_sw128(sb + k * 32, 16, 1024);
-            umma_tf32(tmem + acc * BN, da, db, idesc, (fresh && k == 0) ? 0u : 1u);
-          }
-          touched |= 1u << acc;
-        }
-        umma_commit(&empty[stage]);
-        if (++kc == p.kchunks) {
-          kc = 0;
-          ++step;
-        }
-        if (++stage == MP_STAGES) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-      umma_commit(tmem_full);
+  } else if (warp >= 4) {
+    const int ct = threadIdx.x - 128;
+    const int half = ct >> 7;
+    // ===== MMA: one A box feeds every phase that reads this shift =====
+    float acc0[BN / 2], acc1[BN / 2], acc2[BN / 2], acc3[BN / 2];  // each phase's first MMA overwrites (scale_d = 0)
+    {
+      int stage = 0, prev = 0, it = 0;
+      uint32_t phase = 0;
+      mp_consume<0>(acc0, acc1, acc2, acc3, smem, full, empty, p.kchunks, half, (ct & 127) == 0, stage, phase, prev, it);
+      wgmma_wait<0>();
+      wgmma_fence_regs<BN / 2>(acc0);
+      wgmma_fence_regs<BN / 2>(acc1);
+      wgmma_fence_regs<BN / 2>(acc2);
+      wgmma_fence_regs<BN / 2>(acc3);
     }
-  } else {
-    // ===== epilogue: one accumulator (= output phase) at a time through three 32 KB staging buffers, so the TMA
-    // store of phase j overlaps the TMEM read-out of phase j+1 =====
-    const int q = warp & 3;
-    const int m = q * 32 + lane;
+    consumers_sync();  // every MMA has retired: the ring is free for the staging buffers
+    // ===== epilogue: all four accumulators (= output phases) go to their own 32 KB staging buffer first, so that no
+    // accumulator is live during the element-wise work; then phase by phase, the TMA store of phase j overlapping the
+    // epilogue of phase j+1; warpgroup `half` takes channels [32 * half, +32) =====
+    store_acc_sw128<BN>(smem + 0 * (2 * TC_A_BYTES), acc0, half * 64);
+    store_acc_sw128<BN>(smem + 1 * (2 * TC_A_BYTES), acc1, half * 64);
+    store_acc_sw128<BN>(smem + 2 * (2 * TC_A_BYTES), acc2, half * 64);
+    store_acc_sw128<BN>(smem + 3 * (2 * TC_A_BYTES), acc3, half * 64);
+    consumers_sync();
+    const int q = (ct >> 5) & 3;
+    const int m = ct & 127;
+    const int c = half * 32;
     const int lw = m & (BW - 1);
     const int lh = (m >> p.bw_log2) & (BH - 1);
     const int ln = m >> (p.bw_log2 + p.bh_log2);
     const int ow = w0 + lw, oh = h0 + lh, on = n0 + ln;
     const bool valid = (ow < p.Wo) && (oh < p.Ho) && (on < p.N);
-    const float *cs = p.chan_scale ? p.chan_scale + (int64_t)on * p.ldk + ntile * BN : nullptr;
-    const int act = p.act, rtf = p.rtf;
-    const float slope = p.slope;
-    float st1[BN / 32], st2[BN / 32];
-#pragma unroll
-    for (int i = 0; i < BN / 32; ++i) st1[i] = st2[i] = 0.f;
-    mbar_wait(tmem_full, 0);
-    tc_fence_after();
-    if (threadIdx.x == 64) TC_TRACE(40);
+    const float *cs = p.chan_scale && valid ? p.chan_scale + (int64_t)on * p.ldk + ntile * BN + c : nullptr;
+    const float *bias = p.bias ? p.bias + ntile * BN + c : nullptr;
+    float st1 = 0.f, st2 = 0.f;
+    if (ct == 0) TC_TRACE(40);
 #pragma unroll 1
     for (int j = 0; j < 4; ++j) {
-      uint8_t *buf = smem + (j % 3) * (2 * TC_A_BYTES);
-      if (j == 3) {  // buffer 0 is reused: its store must have finished reading shared memory
-        if (threadIdx.x == 64) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-        asm volatile("bar.sync 1, 128;" ::: "memory");
+      uint8_t *buf = smem + j * (2 * TC_A_BYTES);
+      float v[32];
+      uint8_t *chunk = buf + half * TC_A_BYTES;
+      ld_row32(chunk, m, v);
+      epilogue_chunk(v, bias, 0, p.act, p.slope, cs, p.rtf);
+      st_row32(chunk, m, v);
+      if (p.stats) {
+        float s2[32];
+#pragma unroll
+        for (int e = 0; e < 32; ++e) {
+          v[e] = valid ? v[e] : 0.f;
+          s2[e] = v[e] * v[e];
+        }
+        st1 += warp_colsum32(v, lane);
+        st2 += warp_colsum32(s2, lane);
       }
-      if (threadIdx.x == 64) TC_TRACE(48 + 3 * j);
-#pragma unroll
-      for (int c = 0; c < BN; c += 32) {
-        float v[32];
-        tmem_ld_32x32(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(j * BN + c), v);
-        if (p.bias) {
-          const float4 *b4 = reinterpret_cast<const float4 *>(p.bias + ntile * BN + c);
-#pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            float4 b = __ldg(b4 + e);
-            v[4 * e] += b.x; v[4 * e + 1] += b.y; v[4 * e + 2] += b.z; v[4 * e + 3] += b.w;
-          }
-        }
-        if (act == B200GAN_ACT_LRELU) {
-#pragma unroll
-          for (int e = 0; e < 32; ++e) v[e] = v[e] > 0.f ? v[e] : v[e] * slope;
-        } else if (act == B200GAN_ACT_RELU) {
-#pragma unroll
-          for (int e = 0; e < 32; ++e) v[e] = fmaxf(v[e], 0.f);
-        } else if (act == B200GAN_ACT_TANH) {
-#pragma unroll
-          for (int e = 0; e < 32; ++e) v[e] = tanhf(v[e]);
-        } else if (act == B200GAN_ACT_SIGMOID) {
-#pragma unroll
-          for (int e = 0; e < 32; ++e) v[e] = 1.f / (1.f + __expf(-v[e]));
-        }
-        if (cs && valid) {
-          const float4 *s4 = reinterpret_cast<const float4 *>(cs + c);
-#pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            float4 b = __ldg(s4 + e);
-            v[4 * e] *= b.x; v[4 * e + 1] *= b.y; v[4 * e + 2] *= b.z; v[4 * e + 3] *= b.w;
-          }
-        }
-        if (rtf) {
-#pragma unroll
-          for (int e = 0; e < 32; ++e) v[e] = round_tf32(v[e]);
-        }
-        {
-          uint8_t *row = buf + (c >> 5) * TC_A_BYTES + m * 128;
-#pragma unroll
-          for (int e = 0; e < 8; ++e)
-            *reinterpret_cast<float4 *>(row + ((e ^ (m & 7)) << 4)) =
-                make_float4(v[4 * e], v[4 * e + 1], v[4 * e + 2], v[4 * e + 3]);
-        }
-        if (p.stats) {
-          float s2[32];
-#pragma unroll
-          for (int e = 0; e < 32; ++e) {
-            v[e] = valid ? v[e] : 0.f;
-            s2[e] = v[e] * v[e];
-          }
-          st1[c >> 5] += warp_colsum32(v, lane);
-          st2[c >> 5] += warp_colsum32(s2, lane);
-        }
-      }
-      if (threadIdx.x == 64) TC_TRACE(49 + 3 * j);
       fence_proxy_async();
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (threadIdx.x == 64) {
+      consumers_sync();
+      if (ct == 0) {
         TC_TRACE(50 + 3 * j);
 #pragma unroll
-        for (int c = 0; c < BN; c += 32)
-          tma_store_5d(&tmY, buf + (c >> 5) * TC_A_BYTES, p.out_dc[j] + ntile * BN + c, w0, p.out_da[j], h0, n0);
+        for (int cc = 0; cc < BN; cc += 32)
+          tma_store_5d(&tmY, buf + (cc >> 5) * TC_A_BYTES, p.out_dc[j] + ntile * BN + cc, w0, p.out_da[j], h0, n0);
         asm volatile("cp.async.bulk.commit_group;" ::: "memory");
       }
     }
-    if (threadIdx.x == 64) {
-      TC_TRACE(43);
+    if (ct == 0) {
       asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
       TC_TRACE(41);
     }
     if (p.stats) {
-#pragma unroll
-      for (int i = 0; i < BN / 32; ++i) {
-        red[(q * BN + i * 32 + lane) * 2 + 0] = st1[i];
-        red[(q * BN + i * 32 + lane) * 2 + 1] = st2[i];
-      }
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      const int e = threadIdx.x - 64;
-      if (e < BN) {
+      red[(q * BN + c + lane) * 2 + 0] = st1;
+      red[(q * BN + c + lane) * 2 + 1] = st2;
+      consumers_sync();
+      if (ct < BN) {
         float a = 0.f, b = 0.f;
 #pragma unroll
         for (int qq = 0; qq < 4; ++qq) {
-          a += red[(qq * BN + e) * 2 + 0];
-          b += red[(qq * BN + e) * 2 + 1];
+          a += red[(qq * BN + ct) * 2 + 0];
+          b += red[(qq * BN + ct) * 2 + 1];
         }
-        const int gidx = (p.stats_per_sample ? n0 * p.ldk : 0) + ntile * BN + e;
+        const int gidx = (p.stats_per_sample ? n0 * p.ldk : 0) + ntile * BN + ct;
         atomicAdd(p.stats + gidx, (double)a);
         atomicAdd(p.stats + p.stats_groups + gidx, (double)b);
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tmem_dealloc<4 * BN>(tmem);
-  }
-  if (threadIdx.x == 0) TC_TRACE(42);
+  if (threadIdx.x == 128) TC_TRACE(42);
 }
 
 // ---- host ----------------------------------------------------------------------------------------
@@ -671,35 +649,18 @@ static int ilog2_ceil(int v) {
 
 template <int BN, int STAGES>
 static int launch_tc(const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmY, const TcParams &p, dim3 grid,
-                     cudaStream_t st, const CUtensorMap *tmBh = nullptr) {
-  constexpr int SMEM = STAGES * (TC_A_BYTES + BN * TC_BK * 4) + 1024 + 256 + 4 * BN * 2 * 4;
-  if (tmBh) {   // clusters of two CTAs along x sharing the weight boxes (see conv_tc_kernel)
-    static std::atomic<uint64_t> attr_done2{0};
-    if (int e = ensure_dynamic_smem(conv_tc_kernel<BN, STAGES, 2>, SMEM, attr_done2)) return e;
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = grid;
-    cfg.blockDim = dim3(TC_THREADS);
-    cfg.dynamicSmemBytes = SMEM;
-    cfg.stream = st;
-    cudaLaunchAttribute attr;
-    attr.id = cudaLaunchAttributeClusterDimension;
-    attr.val.clusterDim.x = 2; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
-    cfg.attrs = &attr;
-    cfg.numAttrs = 1;
-    B2_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<BN, STAGES, 2>, tmA, tmB, tmY, p, *tmBh));
-    return B200GAN_OK;
-  }
+                     cudaStream_t st) {
+  constexpr int SMEM = TcSmem<BN, STAGES>::TOTAL;
   static std::atomic<uint64_t> attr_done{0};
-  if (int e = ensure_dynamic_smem(conv_tc_kernel<BN, STAGES, 1>, SMEM, attr_done)) return e;
-  conv_tc_kernel<BN, STAGES, 1><<<grid, TC_THREADS, SMEM, st>>>(tmA, tmB, tmY, p, tmB);
+  if (int e = ensure_dynamic_smem(conv_tc_kernel<BN, STAGES>, SMEM, attr_done)) return e;
+  conv_tc_kernel<BN, STAGES><<<grid, TC_THREADS, SMEM, st>>>(tmA, tmB, tmY, p);
   B2_LAUNCH_CHECK();
   return B200GAN_OK;
 }
 
 int tc_wgrad_supported(const b200gan_conv_geom *g);  // wgrad_tc.cu
 
-// Which passes of which geometries the tcgen05 path takes.
+// Which passes of which geometries the tensor-core path takes.
 //   gather form  (out[p] = sum_t in[stride*p + off_t] B_t): Conv2d fprop, ConvTranspose2d dgrad
 //   scatter form (out[h] = sum_{t | stride divides h+pad-t} in[(h+pad-t)/stride] B_t): Conv2d dgrad, ConvTranspose2d fprop
 // stride 2 is handled with parity views: the gathered tensor {2C, W/2, 2, H/2, N} for the gather form, the
@@ -771,11 +732,11 @@ static int run_tc(const float *in, int N, int Hi, int Wi, int Cc, bool phase_in,
   p.tiles_w = ceil_div(Wo, BW);
   p.tiles_h = ceil_div(Ho, BH);
   {
-    // 256-wide tiles (A 16 KB + B 32 KB per stage feed 4 x M128 N256 K8: operand ingest and tensor time balance) when
-    // the layer still gives every SM a CTA
+    // 256-wide tiles (A 16 KB + B 32 KB per stage feed 2 x 4 x M64 N256 K8: the 128-channel A box is fetched half as
+    // often per output channel) when the layer still gives every SM a CTA
     static const bool bn256 = !(getenv("B200GAN_TC_BN256") && atoi(getenv("B200GAN_TC_BN256")) == 0);
     const int64_t tiles = (int64_t)p.tiles_w * p.tiles_h * ceil_div(N, BNn) * nphase;
-    if (bn256 && Kout % 256 == 0 && tiles * (Kout / 256) >= 148) BN = 256;
+    if (bn256 && Kout % 256 == 0 && tiles * (Kout / 256) >= num_sms()) BN = 256;
   }
   p.N = N;
   p.Ho = Ho;
@@ -791,15 +752,15 @@ static int run_tc(const float *in, int N, int Hi, int Wi, int Cc, bool phase_in,
   p.stats_per_sample = ep ? ep->stats_per_sample : 0;
   p.stats_groups = p.stats_per_sample ? N * ldk : ldk;
   if (p.stats && p.stats_per_sample && BNn != 1)
-    B2_UNSUPPORTED("tcgen05 fprop: per-sample statistics need one image per tile (H*W >= 128 per phase)");
+    B2_UNSUPPORTED("tensor-core fprop: per-sample statistics need one image per tile (H*W >= 128 per phase)");
   p.act = ep ? ep->act : 0;
   p.slope = ep ? ep->slope : 0.f;
   p.rtf = ep ? ep->round_tf32 : 0;
   p.y = y;
   p.narrow_k = narrow_k;
   if (narrow_k) {
-    B2_CHECK_ARG(!phase_in && !phase_out && nphase == 1, "tcgen05 conv: narrow output only in the plain gather form");
-    B2_CHECK_ARG(!p.chan_scale, "tcgen05 conv: Dropout2d scale with fewer than 32 output channels");
+    B2_CHECK_ARG(!phase_in && !phase_out && nphase == 1, "tensor-core conv: narrow output only in the plain gather form");
+    B2_CHECK_ARG(!p.chan_scale, "tensor-core conv: Dropout2d scale with fewer than 32 output channels");
   }
   p.ksplit = 1;
   double *deferred_stats = nullptr;
@@ -817,8 +778,8 @@ static int run_tc(const float *in, int N, int Hi, int Wi, int Cc, bool phase_in,
       const int it = (tap_begin[z + 1] - tap_begin[z]) * p.kchunks;
       if (it < min_iters) min_iters = it;
     }
-    if (allow && plain && !narrow_k && ctas < 148 && min_iters >= 16) {
-      int ks = (int)((2 * 148 + ctas - 1) / ctas);
+    if (allow && plain && !narrow_k && ctas < num_sms() && min_iters >= 16) {
+      int ks = (int)((2 * num_sms() + ctas - 1) / ctas);
       if (ks > min_iters / 8) ks = min_iters / 8;
       if (ks > 32) ks = 32;
       if (ks >= 2) {
@@ -833,7 +794,7 @@ static int run_tc(const float *in, int N, int Hi, int Wi, int Cc, bool phase_in,
   p.trace = nullptr;
   if (const char *tv = getenv("B200GAN_TC_TRACE")) p.trace = reinterpret_cast<long long *>(strtoull(tv, nullptr, 0));
   B2_CHECK_ARG(((uintptr_t)in % 16 == 0) && ((uintptr_t)packedB % 16 == 0) && ((uintptr_t)y % 16 == 0),
-               "tcgen05 conv: pointers must be 16-byte aligned");
+               "tensor-core conv: pointers must be 16-byte aligned");
   if (p.ksplit > 1) {
     const int64_t out_elems = phase_out ? (int64_t)N * (2 * Ho) * (2 * Wo) * ldk : (int64_t)N * Ho * Wo * ldk;
     B2_CUDA(cudaMemsetAsync(y, 0, (size_t)out_elems * sizeof(float), st));
@@ -883,23 +844,11 @@ static int run_tc(const float *in, int N, int Hi, int Wi, int Cc, bool phase_in,
     if (int e = make_tmap_f32(&tmB, packedB, 3, dims, strides, box)) return e;
   }
   dim3 grid((unsigned)(p.tiles_w * p.tiles_h * ceil_div(N, BNn)), (unsigned)(Kout / BN), (unsigned)(nphase * p.ksplit));
-  // pairs of neighbouring pixel tiles share their weight boxes through a cluster multicast (wide tiles only: that is where
-  // the weights dominate the operand traffic)
-  CUtensorMap tmBh;
-  const CUtensorMap *pair = nullptr;
-  static const int cluster_mode = getenv("B200GAN_TC_CLUSTER") ? atoi(getenv("B200GAN_TC_CLUSTER")) : 0;
-  if (cluster_mode && !narrow_k && BN >= 128 && grid.x % 2 == 0 && grid.x >= 2) {
-    uint64_t dims[3] = {(uint64_t)Cc, (uint64_t)Kreal, (uint64_t)btaps};
-    uint64_t strides[2] = {(uint64_t)Cc * 4, (uint64_t)Kreal * Cc * 4};
-    uint32_t box[3] = {TC_BK, (uint32_t)(BN / 2), 1};
-    if (int e = make_tmap_f32(&tmBh, packedB, 3, dims, strides, box)) return e;
-    pair = &tmBh;
-  }
   int rc;
-  if (BN == 256) rc = launch_tc<256, 2>(tmA, tmB, tmY, p, grid, st, pair);
-  else if (BN == 128) rc = launch_tc<128, 3>(tmA, tmB, tmY, p, grid, st, pair);
-  else if (BN == 64) rc = launch_tc<64, 4>(tmA, tmB, tmY, p, grid, st);
-  else rc = launch_tc<32, 4>(tmA, tmB, tmY, p, grid, st);
+  if (BN == 256) rc = launch_tc<256, 4>(tmA, tmB, tmY, p, grid, st);
+  else if (BN == 128) rc = launch_tc<128, 6>(tmA, tmB, tmY, p, grid, st);
+  else if (BN == 64) rc = launch_tc<64, 8>(tmA, tmB, tmY, p, grid, st);
+  else rc = launch_tc<32, 8>(tmA, tmB, tmY, p, grid, st);
   if (rc == B200GAN_OK && deferred_stats) {
     b200gan_norm_desc nd;
     memset(&nd, 0, sizeof(nd));
@@ -918,27 +867,8 @@ static int run_up2_allphase(const float *x, int N, int H, int W, int C, const fl
                             const b200gan_epilogue *ep, float *y, cudaStream_t st) {
   MpParams p;
   memset(&p, 0, sizeof(p));
-  int ns = 0;
-  for (int dh = -1; dh <= 1; ++dh)
-    for (int dw = -1; dw <= 1; ++dw) {
-      // phase (a,b) reads shift (dh,dw) through its tap (dr,ds) = (dh-a+1, dw-b+1) when both are in {0,1}
-      MpStep *s = nullptr;
-      for (int a = 0; a < 2; ++a)
-        for (int b = 0; b < 2; ++b) {
-          const int dr = dh - a + 1, ds = dw - b + 1;
-          if (dr < 0 || dr > 1 || ds < 0 || ds > 1) continue;
-          if (!s || s->nb == MP_MAX_USES) {  // new stage (the centre shift needs two)
-            s = &p.steps[ns++];
-            s->dw = (int8_t)dw;
-            s->dh = (int8_t)dh;
-          }
-          const int ph = a * 2 + b;
-          s->acc[s->nb] = (int8_t)ph;
-          s->bt[s->nb] = (int8_t)(ph * 4 + dr * 2 + ds);
-          ++s->nb;
-        }
-    }
-  if (ns != MP_STEPS) B2_UNSUPPORTED("internal: all-phase step list");
+  constexpr MpSchedule sched = mp_schedule();
+  for (int i = 0; i < MP_STEPS; ++i) p.steps[i] = sched.s[i];
   p.kout_total = K;
   p.kchunks = C / TC_BK;
   int bwl = ilog2_ceil(W);
@@ -964,14 +894,14 @@ static int run_up2_allphase(const float *x, int N, int H, int W, int C, const fl
   p.stats_per_sample = ep ? ep->stats_per_sample : 0;
   p.stats_groups = p.stats_per_sample ? N * K : K;
   if (p.stats && p.stats_per_sample && BNn != 1)
-    B2_UNSUPPORTED("tcgen05 fprop: per-sample statistics need one image per tile (H*W >= 128 per phase)");
+    B2_UNSUPPORTED("tensor-core fprop: per-sample statistics need one image per tile (H*W >= 128 per phase)");
   p.act = ep ? ep->act : 0;
   p.slope = ep ? ep->slope : 0.f;
   p.rtf = ep ? ep->round_tf32 : 0;
   p.trace = nullptr;
   if (const char *tv = getenv("B200GAN_TC_TRACE")) p.trace = reinterpret_cast<long long *>(strtoull(tv, nullptr, 0));
   B2_CHECK_ARG(((uintptr_t)x % 16 == 0) && ((uintptr_t)packed % 16 == 0) && ((uintptr_t)y % 16 == 0),
-               "tcgen05 conv: pointers must be 16-byte aligned");
+               "tensor-core conv: pointers must be 16-byte aligned");
   CUtensorMap tmA, tmB, tmY;
   uint32_t box[5] = {TC_BK, (uint32_t)BW, 1, (uint32_t)BH, (uint32_t)BNn};
   {
@@ -991,7 +921,7 @@ static int run_up2_allphase(const float *x, int N, int H, int W, int C, const fl
     uint32_t bbox[2] = {TC_BK, (uint32_t)MP_BN};
     if (int e = make_tmap_f32(&tmB, packed, 2, dims, strides, bbox)) return e;
   }
-  constexpr int SMEM = MP_STAGES * MP_STAGE_BYTES + 1024 + 256 + 4 * MP_BN * 2 * 4;
+  constexpr int SMEM = MP_MAIN + 1024 + 256 + 4 * MP_BN * 2 * 4;
   static std::atomic<uint64_t> attr_done{0};
   if (int e = ensure_dynamic_smem(conv_tc_up2_allphase_kernel, SMEM, attr_done)) return e;
   dim3 grid((unsigned)(p.tiles_w * p.tiles_h * ceil_div(N, BNn)), (unsigned)(K / MP_BN), 1);

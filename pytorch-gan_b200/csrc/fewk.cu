@@ -642,7 +642,7 @@ int fewk_fprop(const b200gan_conv_geom *g, const b200gan_epilogue *ep, const flo
   p.slope = ep ? ep->slope : 0.f;
   const size_t smem = (size_t)g->R * g->S * g->K * g->C * sizeof(float);
   const int64_t ntiles = (int64_t)g->N * ceil_div(g->P, 8) * ceil_div(g->Q, p.G * FK_PX);
-  const int grid = (int)(ntiles < 148 * 4 ? ntiles : 148 * 4);
+  const int grid = (int)(ntiles < num_sms() * 4 ? ntiles : num_sms() * 4);
   if (fewk_fold_on(g)) {   // folded x2 upsample: parity-specific filters with 2..3 taps per dimension
     const int par = g->pad_l & 1;
     if (g->S == 3) return par ? fewk_fprop_up2_launch<3, 1>(p, g->K, grid, fewk_fold_smem<3>(g), st)
@@ -681,7 +681,7 @@ int fewk_dgrad(const b200gan_conv_geom *g, const float *dy, const float *packed,
   p.dy = dy; p.w = packed; p.dx = dx;
   const size_t smem = (size_t)g->R * g->S * g->K * g->C * sizeof(float);
   const int64_t ntiles = (int64_t)g->N * ceil_div(g->H, 8) * ceil_div(g->W, p.G * FK_PX);
-  const int grid = (int)(ntiles < 148 * 4 ? ntiles : 148 * 4);
+  const int grid = (int)(ntiles < num_sms() * 4 ? ntiles : num_sms() * 4);
   if (fewk_fold_on(g)) {
     if (g->S == 3) return fewk_dgrad_up2_launch<3>(p, g->K, grid, fewk_fold_smem<3>(g), st);
     return fewk_dgrad_up2_launch<4>(p, g->K, grid, fewk_fold_smem<4>(g), st);
@@ -695,9 +695,9 @@ int fewk_dgrad(const b200gan_conv_geom *g, const float *dy, const float *packed,
   return fewk_dgrad_launch<7, 1>(p, g->K, grid, smem, st);
 }
 
-constexpr int FK_WG_BLOCKS = 148 * 2;
+static int fk_wg_blocks() { return num_sms() * 2; }
 size_t fewk_wgrad_workspace_floats(const b200gan_conv_geom *g) {
-  return (size_t)FK_WG_BLOCKS * g->K * g->C * g->R * g->S;
+  return (size_t)fk_wg_blocks() * g->K * g->C * g->R * g->S;
 }
 
 template <int S>
@@ -705,13 +705,13 @@ static int fewk_wgrad_launch(const FewkP &p, int K, size_t smem, cudaStream_t st
   static std::atomic<uint64_t> d1{0}, d2{0}, d3{0}, d4{0};
   switch (K) {
     case 1: if (int e = ensure_dynamic_smem(fewk_wgrad_kernel<S, 1>, 160 * 1024, d1)) return e;
-            fewk_wgrad_kernel<S, 1><<<FK_WG_BLOCKS, 256, smem, st>>>(p); break;
+            fewk_wgrad_kernel<S, 1><<<fk_wg_blocks(), 256, smem, st>>>(p); break;
     case 2: if (int e = ensure_dynamic_smem(fewk_wgrad_kernel<S, 2>, 160 * 1024, d2)) return e;
-            fewk_wgrad_kernel<S, 2><<<FK_WG_BLOCKS, 256, smem, st>>>(p); break;
+            fewk_wgrad_kernel<S, 2><<<fk_wg_blocks(), 256, smem, st>>>(p); break;
     case 3: if (int e = ensure_dynamic_smem(fewk_wgrad_kernel<S, 3>, 160 * 1024, d3)) return e;
-            fewk_wgrad_kernel<S, 3><<<FK_WG_BLOCKS, 256, smem, st>>>(p); break;
+            fewk_wgrad_kernel<S, 3><<<fk_wg_blocks(), 256, smem, st>>>(p); break;
     default: if (int e = ensure_dynamic_smem(fewk_wgrad_kernel<S, 4>, 160 * 1024, d4)) return e;
-            fewk_wgrad_kernel<S, 4><<<FK_WG_BLOCKS, 256, smem, st>>>(p); break;
+            fewk_wgrad_kernel<S, 4><<<fk_wg_blocks(), 256, smem, st>>>(p); break;
   }
   B2_LAUNCH_CHECK();
   return B200GAN_OK;
@@ -732,18 +732,18 @@ int fewk_wgrad(const b200gan_conv_geom *g, const float *x, const float *dy, floa
   int rc;
   if (fewk_fold_on(g)) {
     const int par = g->pad_l & 1;
-    if (g->S == 3) rc = par ? fewk_wgrad_up2_launch<3, 1>(p, g->K, FK_WG_BLOCKS, fewk_fold_smem<3>(g), st)
-                            : fewk_wgrad_up2_launch<3, 0>(p, g->K, FK_WG_BLOCKS, fewk_fold_smem<3>(g), st);
-    else rc = par ? fewk_wgrad_up2_launch<4, 1>(p, g->K, FK_WG_BLOCKS, fewk_fold_smem<4>(g), st)
-                  : fewk_wgrad_up2_launch<4, 0>(p, g->K, FK_WG_BLOCKS, fewk_fold_smem<4>(g), st);
+    if (g->S == 3) rc = par ? fewk_wgrad_up2_launch<3, 1>(p, g->K, fk_wg_blocks(), fewk_fold_smem<3>(g), st)
+                            : fewk_wgrad_up2_launch<3, 0>(p, g->K, fk_wg_blocks(), fewk_fold_smem<3>(g), st);
+    else rc = par ? fewk_wgrad_up2_launch<4, 1>(p, g->K, fk_wg_blocks(), fewk_fold_smem<4>(g), st)
+                  : fewk_wgrad_up2_launch<4, 0>(p, g->K, fk_wg_blocks(), fewk_fold_smem<4>(g), st);
     if (rc) return rc;
-    return nb_wgrad_reduce(workspace, dw, dw_elems, FK_WG_BLOCKS, st);
+    return nb_wgrad_reduce(workspace, dw, dw_elems, fk_wg_blocks(), st);
   }
   if (g->S == 3) rc = fewk_wgrad_launch<3>(p, g->K, smem, st);
   else if (g->S == 4) rc = fewk_wgrad_launch<4>(p, g->K, smem, st);
   else rc = fewk_wgrad_launch<7>(p, g->K, smem, st);
   if (rc) return rc;
-  return nb_wgrad_reduce(workspace, dw, dw_elems, FK_WG_BLOCKS, st);
+  return nb_wgrad_reduce(workspace, dw, dw_elems, fk_wg_blocks(), st);
 }
 
 }  // namespace b200gan

@@ -346,7 +346,7 @@ adam_multi_kernel(const __grid_constant__ AdamTable tb, double lr, double b1, do
 
 static unsigned stream_blocks(int64_t n) {
   int64_t b = ceil_div64(n, 256);
-  if (b > 148 * 16) b = 148 * 16;
+  if (b > num_sms() * 16) b = num_sms() * 16;
   if (b < 1) b = 1;
   return (unsigned)b;
 }
@@ -496,7 +496,7 @@ extern "C" int b200gan_bias_grad(const float *dy, const float *y, const float *c
   cudaStream_t st = as_stream(stream);
   B2_CUDA(cudaMemsetAsync(db, 0, (size_t)K * sizeof(float), st));
   if (rows == 0) return B200GAN_OK;
-  int64_t yb = 148 * 8 / ceil_div(K, 32);
+  int64_t yb = num_sms() * 8 / ceil_div(K, 32);
   if (yb < 1) yb = 1;
   int64_t rpb = ceil_div64(rows, yb);
   if (rpb < 64) rpb = 64;

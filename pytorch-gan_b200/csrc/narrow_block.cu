@@ -281,7 +281,7 @@ struct NbFprop2 {
   NbTile t;
   int PR, PC, CP;   // patch rows, columns, channel pitch (C + 4: lanes = pixels 2 * CP floats apart stay 2-way conflicted at worst)
   int reflect;      // reflection padding (stand-alone use: cyclegan/models.py:49-50), chains are zero-padded
-  int rtf;          // store y rounded to TF32 (a tcgen05 conv consumes it next)
+  int rtf;          // store y rounded to TF32 (a wgmma conv consumes it next)
   int groups;       // statistics groups of the batch (NbBn::groups of the edges; 1 stand-alone)
 };
 // Forward: the patch (BatchNorm of the producer applied while staging) and this block's slice of the weights live in
@@ -1179,7 +1179,7 @@ static NbPlan nb_plan(int nout, int64_t wrow, int cin, int N, int Ho, int Wo, in
         const int64_t blocks = (int64_t)ceil_div(N, t.TN) * t.tiles_r * t.tiles_q * (nout / KB) * nclasses;
         double cost = (double)(PT + KT) / (double)(PT * KT);
         if (cost < 0.25) cost = 0.25;
-        cost /= (double)(blocks < 148 ? blocks : 148);
+        cost /= (double)(blocks < num_sms() ? blocks : num_sms());
         // staging (a third of a block's life, latency-bound) only overlaps with another block's FMAs when two blocks
         // are resident per SM and the grid is large enough to put two on every SM
         if (smem > 110 * 1024 || blocks < 256) cost *= 1.4;
@@ -1313,7 +1313,7 @@ extern "C" int b200gan_nb_fprop(const b200gan_conv_geom *g, const b200gan_nb_bn 
     return nb_fprop2_launch(g, p.in_bn, p.rm, p.rv, p.nbt, momentum, x, packed, bias, act, slope, chan_scale, y, out_stats,
                             0, 0, groups, st);
   // v1 (B200GAN_NB_V1=1): direct gathers from global memory
-  const int KT = (g->K % 8 == 0 && M * (g->K / 8) >= 148 * 512) ? 8 : 4;
+  const int KT = (g->K % 8 == 0 && M * (g->K / 8) >= num_sms() * 512) ? 8 : 4;
   p.Mpad = (int)(ceil_div64(M, 256) * 256);
   const unsigned blocks = (unsigned)((int64_t)(g->K / KT) * (p.Mpad / 256));
   if (KT == 8) nbk_fprop_kernel<8><<<blocks, 256, 0, st>>>(p);
@@ -1337,7 +1337,7 @@ extern "C" int b200gan_nb_dz(int32_t N, int64_t PQ, int32_t K, const float *g, c
   const int groups = p.out_bn.stats ? p.out_bn.groups : 1;
   B2_CHECK_ARG(N % groups == 0, "nb_dz: the batch must split evenly into the statistics groups");
   int64_t blocks = ceil_div64(p.rows / groups, rows_per_block * 4);
-  if (blocks > 148 * 4 / groups) blocks = 148 * 4 / groups;
+  if (blocks > num_sms() * 4 / groups) blocks = num_sms() * 4 / groups;
   if (blocks < 1) blocks = 1;
   nbk_dz_kernel<<<dim3((unsigned)blocks, (unsigned)groups), 256, 0, st>>>(p);
   B2_LAUNCH_CHECK();
@@ -1404,7 +1404,7 @@ static NbWgPlan nb_wgrad_plan(const b200gan_conv_geom *g) {
   while (w.TQ > 1 && tile_bytes(w.TN, w.TR, w.TQ) > 96 * 1024) w.TQ = (w.TQ + 1) / 2;
   w.smem = tile_bytes(w.TN, w.TR, w.TQ);
   const int ntiles = ceil_div(g->N, w.TN) * ceil_div(g->P, w.TR) * ceil_div(g->Q, w.TQ);
-  w.gx = (2 * 148) / w.nchunks;
+  w.gx = (2 * num_sms()) / w.nchunks;
   if (w.gx < 8) w.gx = 8;
   if (w.gx > ntiles) w.gx = ntiles;
   if (w.gx < 1) w.gx = 1;
@@ -1562,7 +1562,7 @@ extern "C" int b200gan_nb_dgrad(const b200gan_conv_geom *g, const float *dz, con
   if (!nb_v1()) return nb_dgrad2_launch(g, dz, packed, p.in_bn, a_prev, g_out, sums, st);
   const int64_t Mc = (int64_t)g->N * ceil_div(g->H, st_) * ceil_div(g->W, st_);  // class 0 is the largest
   p.Mpad = (int)(ceil_div64(Mc, 256) * 256);
-  const int KT = g->C % 8 == 0 ? ((Mc * (g->C / 8) * st_ * st_ >= 148 * 512) ? 8 : 4) : (g->C % 4 == 0 ? 4 : 1);
+  const int KT = g->C % 8 == 0 ? ((Mc * (g->C / 8) * st_ * st_ >= num_sms() * 512) ? 8 : 4) : (g->C % 4 == 0 ? 4 : 1);
   dim3 grid((unsigned)((int64_t)(g->C / KT) * (p.Mpad / 256)), 1, (unsigned)(st_ * st_));
   if (KT == 8) nbk_dgrad_kernel<8><<<grid, 256, 0, st>>>(p);
   else if (KT == 4) nbk_dgrad_kernel<4><<<grid, 256, 0, st>>>(p);
@@ -1573,7 +1573,7 @@ extern "C" int b200gan_nb_dgrad(const b200gan_conv_geom *g, const float *dz, con
 
 static int tail_grid(int64_t total, int C) {
   int64_t blocks = ceil_div64(total, 256 * 4);
-  if (blocks > 148 * 4) blocks = 148 * 4;
+  if (blocks > num_sms() * 4) blocks = num_sms() * 4;
   if (blocks < 1) blocks = 1;
   // total threads a multiple of C (C <= 128 divides 256 when it is a power of two; otherwise round the block count)
   while ((blocks * 256) % C != 0) ++blocks;

@@ -370,7 +370,7 @@ static dim3 fast_grid(const b200gan_norm_desc *d, int64_t &rows) {
   rows = d->per_sample ? (int64_t)d->HW : (int64_t)d->N * d->HW;
   const int ny = d->per_sample ? d->N : 1;
   const int rpb = 256 / (d->C / 4);
-  int64_t want = (148 * 8 + ny - 1) / ny;
+  int64_t want = (num_sms() * 8 + ny - 1) / ny;
   int64_t maxb = ceil_div64(rows, (int64_t)rpb * 4);
   if (want > maxb) want = maxb;
   if (want < 1) want = 1;
@@ -381,7 +381,7 @@ static void reduce_grid(const b200gan_norm_desc *d, dim3 &grid, int64_t &rows, i
   rows = d->per_sample ? (int64_t)d->HW : (int64_t)d->N * d->HW;
   int xb = ceil_div(d->C, 32);
   int zb = d->per_sample ? d->N : 1;
-  int64_t want = (148 * 8) / ((int64_t)xb * zb);
+  int64_t want = (num_sms() * 8) / ((int64_t)xb * zb);
   if (want < 1) want = 1;
   rpb = ceil_div64(rows, want);
   if (rpb < 32) rpb = 32;
@@ -449,7 +449,7 @@ extern "C" int b200gan_norm_apply(const b200gan_norm_desc *d, const float *x,
   bool vec = (d->C % 4 == 0) && (((uintptr_t)x | (uintptr_t)y) % 16 == 0);
   int64_t tv = vec ? total / 4 : total;
   int64_t blocks = ceil_div64(tv, 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > num_sms() * 16) blocks = num_sms() * 16;
   if (vec)
     norm_apply_kernel<4><<<(unsigned)blocks, 256, 0, as_stream(stream)>>>(
         x, scale_shift, y, tv, d->C, d->HW, G, d->per_sample, d->act, d->slope, d->round_tf32);
@@ -497,7 +497,7 @@ extern "C" int b200gan_norm_bwd(const b200gan_norm_desc *d, const float *dy, con
              (((uintptr_t)x | (uintptr_t)dy | (uintptr_t)dx | (uintptr_t)(y ? y : x)) % 16 == 0);
   int64_t tv = vec ? total / 4 : total;
   int64_t blocks = ceil_div64(tv, 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > num_sms() * 16) blocks = num_sms() * 16;
   float inv_count = (float)(1.0 / (d->per_sample ? (double)d->HW : (double)d->N * (double)d->HW));
   if (vec)
     norm_bwd_apply_kernel<4><<<(unsigned)blocks, 256, 0, st>>>(

@@ -8,11 +8,11 @@
 // write da), conv wgrad (read y): ~1.6 GB of HBM traffic.  Fused:
 //   tail_fprop_tc_kernel   reads a once (134 MB).  A tile of 128 pixels is loaded with coalesced 16-byte loads,
 //                          normalised + activated in registers, stored TF32-rounded into shared memory in the K-major
-//                          128B-swizzled UMMA layout, and multiplied on tcgen05 (M128 x N16 x K8, kind::tf32) with the
-//                          [taps x C] filter matrix: D[pixel][tap] in TMEM.  The epilogue warps read D back with
-//                          tcgen05.ld and scatter-add the nine tap partials into the band's output rows in shared
-//                          memory (the 3x3 stencil), then bias + Tanh + one coalesced store.  HBM-bound by design: the
-//                          SM does ~300 instructions per pixel.
+//                          128B-swizzled wgmma layout, and multiplied with wgmma (two warpgroups x M64 x N16/32 x K8,
+//                          TF32) by the [taps x C] filter matrix: D[pixel][tap] in registers.  Every thread writes its
+//                          accumulator fragment as tap partials into the band's rows in shared memory (the 3x3
+//                          stencil is gathered at the end), then bias + Tanh + one coalesced store.  HBM-bound by
+//                          design: the SM does ~300 instructions per pixel.
 //   tail_bwd_reduce_kernel reads a once: recomputes the conv's data gradient from the 2 MB output gradient (9 FMAs per
 //                          channel), applies the activation mask, accumulates the BatchNorm backward sums AND the conv's
 //                          weight gradient (y recomputed from a) in registers; lane <-> 4 channels, so there is no
@@ -39,20 +39,6 @@ struct TailP {
   int act_out;
 };
 
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, float *v) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-
 __device__ __forceinline__ float mid_act(float v, int act, float slope) {
   if (act == B200GAN_ACT_LRELU) return v > 0.f ? v : v * slope;
   if (act == B200GAN_ACT_RELU) return fmaxf(v, 0.f);
@@ -78,7 +64,7 @@ __device__ __forceinline__ float ld_shared_f32(uint32_t addr) {
 }
 
 // grid (bands per image, N); block 256.  C4 = C/4 float4 per pixel (8, 16 or 32), NB = MMA N (16: K = 1; 32: K <= 3).
-// Shared memory: A tile (KC x 16 KB, UMMA K-major SW128) | filter matrix B | mbarrier | T[(TH+2) rows][W][9K] tap
+// Shared memory: A tile (KC x 16 KB, wgmma K-major SW128) | filter matrix B | T[(TH+2) rows][W][9K] tap
 // partials of every input pixel of the band (+1 halo row each side).  No atomics: the 3x3 stencil is a gather over T at
 // the end of the band (shared-memory fp32 atomics are CAS loops on this architecture).
 template <int C4, int NB>
@@ -92,13 +78,10 @@ tail_fprop_tc_kernel(const __grid_constant__ TailP p) {
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t sA = (raw + 1023u) & ~1023u;   // shared-space byte addresses
   const uint32_t sB = sA + A_BYTES;
-  const uint32_t sBar = sB + KC * B_CHUNK;
-  const uint32_t sTmem = sBar + 8;
-  const uint32_t sT = sBar + 16;
-  uint64_t *mbar = reinterpret_cast<uint64_t *>(smem_raw + (sBar - raw));
-  uint32_t *tmem_ptr = reinterpret_cast<uint32_t *>(smem_raw + (sTmem - raw));
+  const uint32_t sT = sB + KC * B_CHUNK;
 
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int wg = tid >> 7;  // warpgroup: MMA rows (pixels) [64 * wg, +64) of the tile
   const int W = p.W, H = p.H, K = p.K;
   const int n = blockIdx.y;
   const int p0 = blockIdx.x * TL_TH;
@@ -106,14 +89,6 @@ tail_fprop_tc_kernel(const __grid_constant__ TailP p) {
   const int RT = 128 >> p.w_log2;           // image rows per 128-pixel tile
   const int K9 = 9 * K;
 
-  if (tid == 0) {
-    mbar_init(mbar, 1);
-    fence_barrier_init();
-  }
-  if (warp == 0) {
-    __syncwarp();
-    tmem_alloc<32>(tmem_ptr);
-  }
   // filter matrix B[row = k*9 + tap][c] (zero rows above 9K), TF32-rounded, K-major SW128
   for (int i = tid; i < NB * C4 * 4; i += TL_THREADS) {
     const int c = i % (C4 * 4), row = i / (C4 * 4);
@@ -136,12 +111,7 @@ tail_fprop_tc_kernel(const __grid_constant__ TailP p) {
   const int act_mid = p.act_mid;
   const float slope = p.slope;
   fence_proxy_async();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_ptr;
-  constexpr uint32_t idesc = umma_idesc_tf32(128, NB, 0, 0);
-  uint32_t parity = 0;
 
   // tiles of RT input rows starting at row p0 - 1; only those with a valid row that reaches the band are processed
   int t_lo = 0, t_hi = (TL_TH + 2) / RT;
@@ -179,45 +149,37 @@ tail_fprop_tc_kernel(const __grid_constant__ TailP p) {
       st_shared_v4(sA + kc * 16384 + m * 128 + ((j ^ (m & 7)) << 4), o);
     }
     fence_proxy_async();  // generic-proxy smem writes -> visible to the tensor core (async proxy)
-    tc_fence_before();    // the previous tile's tcgen05.ld are ordered before the barrier ...
     __syncthreads();
-    if (tid == 0) {
-      tc_fence_after();   // ... and the MMAs below after it
+    float d[NB / 2];
+    wgmma_fence();
 #pragma unroll
-      for (int kc = 0; kc < KC; ++kc)
+    for (int kc = 0; kc < KC; ++kc)
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const uint64_t da = umma_desc_sw128(sA + kc * 16384 + k * 32, 16, 1024);
-          const uint64_t db = umma_desc_sw128(sB + kc * B_CHUNK + k * 32, 16, 1024);
-          umma_tf32(tmem, da, db, idesc, (kc > 0 || k > 0) ? 1u : 0u);
-        }
-      umma_commit(mbar);
-    }
-    if (t + 1 < t_hi) load_tile(t + 1);  // in flight while the tensor core and the epilogue work on tile t
-    mbar_wait(mbar, parity);  // every thread: the MMAs have retired, sA may be overwritten, D is complete
-    parity ^= 1;
-    tc_fence_after();
-    if (warp < 4) {
-      // thread m <-> TMEM lane m <-> pixel m of the tile: D[m][k*9 + r*3 + s] is the (r,s) tap partial of that INPUT pixel
-      float d[NB];
-      const uint32_t taddr = tmem + ((uint32_t)(warp * 32) << 16);
-      if constexpr (NB == 16) {
-        tmem_ld_32x16(taddr, d);
-      } else {
-        tmem_ld_32x32(taddr, d);
-      }
-      const int m = tid;
+      for (int k = 0; k < 4; ++k)
+        wgmma_tf32<NB>(d, gmma_desc_sw128(sA + kc * 16384 + wg * 8192 + k * 32), gmma_desc_sw128(sB + kc * B_CHUNK + k * 32),
+                       (kc > 0 || k > 0) ? 1u : 0u);
+    wgmma_commit();
+    if (t + 1 < t_hi) load_tile(t + 1);  // in flight while the tensor core works on tile t
+    wgmma_wait<0>();
+    wgmma_fence_regs<NB / 2>(d);
+    // D[m][k*9 + r*3 + s] is the (r,s) tap partial of INPUT pixel m of the tile; this thread holds rows m0 and m0 + 8
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      const int m = wg * 64 + (warp & 3) * 16 + (lane >> 2) + hr * 8;
       const int h = r0 + (m >> p.w_log2), w = m & (W - 1);
       if (h >= 0 && h < H) {
         const uint32_t dst = sT + (uint32_t)(((h - (p0 - 1)) * W + w) * K9) * 4;
 #pragma unroll
-        for (int j = 0; j < NB; ++j)
-          if (j < K9) st_shared_f32(dst + j * 4, d[j]);
+        for (int j = 0; j < NB / 8; ++j)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int col = j * 8 + (lane & 3) * 2 + e;
+            if (col < K9) st_shared_f32(dst + col * 4, d[4 * j + 2 * hr + e]);
+          }
       }
     }
+    __syncthreads();  // both warpgroups' MMAs have retired: sA may be overwritten
   }
-  tc_fence_before();
-  __syncthreads();
   {
     // out[p][q][k] = act(bias[k] + sum_{r,s} T[p + r - 1][q + s - 1][k*9 + r*3 + s])
     float *dst = p.out + ((int64_t)(n * H + p0) * W) * K;
@@ -240,10 +202,6 @@ tail_fprop_tc_kernel(const __grid_constant__ TailP p) {
       dst[i] = apply_act(acc, act_out, 0.f);
     }
   }
-  if (warp == 0) {
-    __syncwarp();
-    tmem_dealloc<32>(tmem);
-  }
 }
 
 // ---- backward -------------------------------------------------------------------------------------------------
@@ -263,7 +221,7 @@ struct TailBwdP {
   int N, H, W, C, K;
   int act_mid;
   float slope;
-  int rtf;                   // round da to TF32 (it feeds the tcgen05 dgrad / wgrad of the preceding conv)
+  int rtf;                   // round da to TF32 (it feeds the tensor-core dgrad / wgrad of the preceding conv)
   int64_t px_per_block;
 };
 
@@ -596,7 +554,7 @@ static int ilog2_exact(int v) {
 
 template <int C4, int NB>
 static int launch_tail_fprop(const TailP &p, cudaStream_t st) {
-  const int smem = 1024 + (C4 / 8) * (16384 + NB * 128) + 16 + (TL_TH + 2) * p.W * 9 * p.K * 4;
+  const int smem = 1024 + (C4 / 8) * (16384 + NB * 128) + (TL_TH + 2) * p.W * 9 * p.K * 4;
   static std::atomic<uint64_t> done{0};
   B2_CHECK_ARG(smem <= 227 * 1024, "tail_fprop: W=%d K=%d C=%d needs %d bytes of shared memory", p.W, p.K, p.C, smem);
   if (int e = ensure_dynamic_smem(tail_fprop_tc_kernel<C4, NB>, 227 * 1024, done)) return e;
@@ -618,7 +576,7 @@ static int launch_tail_bwd(TailBwdP &p, cudaStream_t st) {
   if (int e = ensure_dynamic_smem(tail_bwd_apply_kernel<C4, KK>, smem_apply, done_a)) return e;
   const int per_sm = (KK == 1 && C4 <= 16) ? 2 : 1;
   // contiguous pixel ranges, a whole number of ring chunks each, one block per resident slot
-  int64_t per = ceil_div64(ceil_div64(total, (int64_t)148 * per_sm), RB_CHUNK) * RB_CHUNK;
+  int64_t per = ceil_div64(ceil_div64(total, (int64_t)num_sms() * per_sm), RB_CHUNK) * RB_CHUNK;
   p.px_per_block = per;
   const unsigned blocks = (unsigned)ceil_div64(total, per);
   tail_bwd_reduce_kernel<C4, KK><<<blocks, RB_THREADS, smem_reduce, st>>>(p);

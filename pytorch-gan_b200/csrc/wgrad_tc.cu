@@ -1,19 +1,19 @@
-// wgrad_tc.cu -- tcgen05 TF32 weight gradient of the stride-1 convolutions (sm_100a).
+// wgrad_tc.cu -- wgmma TF32 weight gradient of the stride-1 convolutions (sm_90a).
 //
 // dW[tap][k][c] = sum over output pixels o of  dy[o][k] * x[o + offset(tap)][c]
 // (reference: autograd of nn.Conv2d, dcgan.py:168,182 -> cudnnConvolutionBackwardFilter).
 //
-// As a GEMM the contraction runs over PIXELS, so both operands are "MN-major" in UMMA terms: a TMA
-// box {32 channels, BW, 1, BH, 1} (32 pixels) lands in shared memory as 32 rows x 128 B.  For TF32 the
-// tensor core accepts MN-major operands only in the SWIZZLE_128B_BASE32B layout (32-byte swizzle atoms,
-// 4-row period), which TMA writes with CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B; one 32-channel chunk per box,
-// chunks LBO bytes apart, 4-row groups SBO = 512 B apart.  The operand with a multiple of 128 channels is
-// A (M = 128), the other is B (N = 64/128).  Zero padding = TMA out-of-bounds fill on the shifted x box.
-// The upsample-folded convolution (dcgan.py:54-55,58-59) contributes 16 (phase, tap) jobs that read dy
-// through the phase view {2K, Q/2, 2, P/2, N}; a second kernel folds them back into the 3x3 filter.
+// As a GEMM the contraction runs over PIXELS, so both operands arrive "MN-major": a TMA box {32 channels, BW, 1, BH,
+// ipb} (32 pixels) lands in shared memory as 32 pixel rows x 128 B (128-byte swizzle).  wgmma takes TF32 operands only
+// K-major, so the consumer warpgroups transpose every stage into K-major 128B-swizzled tiles (channel rows of 32
+// pixels; double-buffered, so the transpose of stage i overlaps the MMAs of stage i-1).  The operand with a multiple of
+// 128 channels is A (M = 128: two warpgroups of 64 rows), the other is B (N = 32..256).  Zero padding = TMA
+// out-of-bounds fill on the shifted x box.  The upsample-folded convolution (dcgan.py:54-55,58-59) contributes 16
+// (phase, tap) jobs that read dy through the phase view {2K, Q/2, 2, P/2, N}; a second kernel folds them back into the
+// 3x3 filter.
 //
 // Parallelisation: grid = (pixel splits, jobs, M-tiles x N-tiles).  Every CTA accumulates its pixel range in
-// TMEM, stages the tile in shared memory and adds it into the job's [M'][N'] matrix with a TMA reduce-store
+// registers, stages the tile in shared memory and adds it into the job's [M'][N'] matrix with a TMA reduce-store
 // (cp.reduce.async.bulk.tensor ... .add: the fp32 additions happen at L2); wgrad_reduce_kernel then folds the
 // jobs into the parameter layout [K][C][R][S].
 #include "tc_common.cuh"
@@ -21,9 +21,10 @@
 
 namespace b200gan {
 
-// pixels (GEMM-K) per pipeline stage: 32 (4 KB boxes) or 64 (8 KB boxes: half as many TMA instructions per byte)
-constexpr int WG_THREADS = 192;
+constexpr int WG_THREADS = 384;  // producer warpgroup + two consumer warpgroups
 constexpr int WG_MAX_JOBS = 52;
+constexpr int WG_PIX = 32;       // pixels (GEMM-K) per pipeline stage
+constexpr int WG_CHUNK_BYTES = WG_PIX * 128;  // one 32-channel chunk of one stage
 
 // One job = one filter tap (or one (phase, tap) pair of the upsample fold).  "S" is the operand that is shifted by
 // the tap (x for Conv2d, dy for ConvTranspose2d), "D" the one that is read at the loop pixel.
@@ -45,23 +46,32 @@ struct WgParams {
   int32_t ldn;                    // N' total (row length of a partial matrix)
   int32_t mtotal;                 // M' total
   float *partial;                 // [job][M'][N'], zeroed by the host; splits accumulate with TMA reduce-add
-  uint32_t lbo, sbo;              // UMMA descriptor byte offsets (chunk stride, 8-row group stride)
 };
 
-template <int NB, int STAGES, int WG_PIX>
-__global__ void __launch_bounds__(WG_THREADS, 2)
+// shared memory: TMA ring | two K-major operand buffers; after the last MMA the front is the staging tile
+template <int NB, int STAGES>
+struct WgSmem {
+  static constexpr int A_BYTES = 4 * WG_CHUNK_BYTES;            // 128 channels
+  static constexpr int B_BYTES = (NB / 32) * WG_CHUNK_BYTES;
+  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+  static constexpr int RING = STAGES * STAGE_BYTES;
+  static constexpr int T_BYTES = 128 * 128 + NB * 128;          // A^T (128 rows) + B^T (NB rows), 32 pixels each
+  static constexpr int STAGING = (NB / 32) * 16384;
+  static constexpr int MAIN = RING + 2 * T_BYTES > STAGING ? RING + 2 * T_BYTES : STAGING;
+  static constexpr int TOTAL = MAIN + 1024 + 256;
+};
+
+__device__ __forceinline__ void wg_consumers_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+
+template <int NB, int STAGES>
+__global__ void __launch_bounds__(WG_THREADS, 1)
 wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmY,
                 const __grid_constant__ CUtensorMap tmP, const __grid_constant__ WgParams p) {
-  constexpr int WG_CHUNK_BYTES = WG_PIX * 128;           // one 32-channel chunk of one stage
-  constexpr int A_BYTES = 4 * WG_CHUNK_BYTES;            // 128 channels
-  constexpr int B_BYTES = (NB / 32) * WG_CHUNK_BYTES;
-  constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+  using L = WgSmem<NB, STAGES>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t *full = reinterpret_cast<uint64_t *>(smem + STAGES * STAGE_BYTES);
+  uint64_t *full = reinterpret_cast<uint64_t *>(smem + L::MAIN);
   uint64_t *empty = full + STAGES;
-  uint64_t *tmem_full = empty + STAGES;
-  uint32_t *tmem_ptr = reinterpret_cast<uint32_t *>(tmem_full + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int split = blockIdx.x, job = blockIdx.y;
@@ -71,21 +81,16 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
   if (t_end > p.tiles_total) t_end = p.tiles_total;
   const int iters = t_end - t_begin;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmX);
     tma_prefetch_desc(&tmY);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
+      mbar_init(&empty[s], 256);  // every consumer thread, once its transpose reads of the stage are done
     }
-    mbar_init(tmem_full, 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<NB>(tmem_ptr);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_ptr;
 
   if (warp == 0) {
     if (lane == 0) {
@@ -106,9 +111,9 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
         const int n = (t / p.tiles_h) * p.imgs_per_box;  // a box spans several images when H*W < WG_PIX
         const int w0 = tw << p.bw_log2, h0 = th << p.bh_log2;
         mbar_wait(&empty[stage], phase ^ 1);
-        uint8_t *sa = smem + stage * STAGE_BYTES;
-        uint8_t *sb = sa + A_BYTES;
-        mbar_arrive_expect_tx(&full[stage], STAGE_BYTES);
+        uint8_t *sa = smem + stage * L::STAGE_BYTES;
+        uint8_t *sb = sa + L::A_BYTES;
+        mbar_arrive_expect_tx(&full[stage], L::STAGE_BYTES);
 #pragma unroll
         for (int c = 0; c < 4; ++c)
           tma_load_5d(sa + c * WG_CHUNK_BYTES, mapA, &full[stage], a_dc + (mt * 4 + c) * 32, w0 + a_dw, a_da,
@@ -123,76 +128,57 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_tf32(128, NB, 1, 1);  // both operands MN-major
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int it = 0; it < iters; ++it) {
-        mbar_wait(&full[stage], phase);
-        tc_fence_after();
-        const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
-        const uint32_t sb = sa + A_BYTES;
+  } else if (warp >= 4 && iters > 0) {
+    const int ct = threadIdx.x - 128;
+    const int half = ct >> 7;           // MMA rows [64 * half, +64) of the 128 x NB tile
+    const int tp = ct & 31, tq = ct >> 5;  // transpose: pixel row tp, 16-byte column tq (4 channels) of every chunk
+    float acc[NB / 2];                  // the first MMA overwrites it (scale_d = 0)
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int it = 0; it < iters; ++it) {
+      uint8_t *ta = smem + L::RING + (it & 1) * L::T_BYTES;  // A^T: 128 rows x 128 B, then B^T: NB rows x 128 B
+      mbar_wait(&full[stage], phase);
+      wg_consumers_sync();  // both warpgroups' MMAs of iteration it-2 (which read this buffer) have retired
+      const uint8_t *src = smem + stage * L::STAGE_BYTES;
 #pragma unroll
-        for (int k = 0; k < WG_PIX / 8; ++k) {
-          // K step = 8 pixel rows = two 4-row swizzle atoms (SBO = 512 B apart); channel chunks LBO = 4096 B apart
-          uint64_t da = umma_desc_sw128(sa + k * 1024, p.lbo, p.sbo, 1);
-          uint64_t db = umma_desc_sw128(sb + k * 1024, p.lbo, p.sbo, 1);
-          umma_tf32(tmem, da, db, idesc, (it > 0 || k > 0) ? 1u : 0u);
-        }
-        umma_commit(&empty[stage]);
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1;
+      for (int c = 0; c < 4 + NB / 32; ++c) {
+        const float4 v = *reinterpret_cast<const float4 *>(src + c * WG_CHUNK_BYTES + tp * 128 + ((tq ^ (tp & 7)) << 4));
+        const float e[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const int r = c * 32 + tq * 4 + i;  // A rows 0..127, then B rows
+          *reinterpret_cast<float *>(ta + r * 128 + (((tp >> 2) ^ (r & 7)) << 4) + (tp & 3) * 4) = e[i];
         }
       }
-      umma_commit(tmem_full);
-    }
-  } else {
-    // TMEM -> registers -> 128B-swizzled staging tile in the (now idle) pipeline buffers -> TMA store of the
-    // partial tile into partial[split][job][m'][n'] (a 2-D tensor map over [rows][ldn]).
-    const int q = warp & 3;
-    const int m = q * 32 + lane;  // row of the 128 x NB tile
-    if (iters > 0) {
-      mbar_wait(tmem_full, 0);
-      tc_fence_after();
-    }
-    // The staging tile reuses the pipeline buffers, which hold at most 128 columns x 128 rows (NB = 256 with two stages:
-    // 96 KB): rounds of 128 columns, each stored before the next one overwrites the staging area.
-    constexpr int ROUND = NB < 128 ? NB : 128;
-    const int row0 = job * p.mtotal + mt * 128;
-#pragma unroll 1
-    for (int r0 = 0; r0 < NB; r0 += ROUND) {
-#pragma unroll 1
-      for (int c = r0; c < r0 + ROUND; c += 32) {
-        float v[32];
-        if (iters > 0) {
-          tmem_ld_32x32(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)c, v);
-        } else {
+      mbar_arrive(&empty[stage]);
+      fence_proxy_async();  // generic-proxy smem writes -> visible to wgmma
+      wg_consumers_sync();
+      const uint32_t sa = smem_u32(ta) + half * 8192, sb = smem_u32(ta) + 128 * 128;
+      wgmma_fence();
 #pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = 0.f;
-        }
-        uint8_t *row = smem + ((c - r0) >> 5) * 16384 + m * 128;
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-          *reinterpret_cast<float4 *>(row + ((j ^ (m & 7)) << 4)) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+      for (int k = 0; k < WG_PIX / 8; ++k)
+        wgmma_tf32<NB>(acc, gmma_desc_sw128(sa + k * 32), gmma_desc_sw128(sb + k * 32), (it > 0 || k > 0) ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (++stage == STAGES) {
+        stage = 0;
+        phase ^= 1;
       }
-      fence_proxy_async();
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (threadIdx.x == 64 && iters > 0) {
-        // all pixel splits of a job accumulate into the same [job][M'][N'] tile: TMA reduce-add (fp32 add at L2)
-#pragma unroll 1
-        for (int c = r0; c < r0 + ROUND; c += 32) tma_reduce_add_2d(&tmP, smem + ((c - r0) >> 5) * 16384, nt * NB + c, row0);
-        tma_store_commit_and_wait_read();
-      }
-      if (NB > ROUND) asm volatile("bar.sync 1, 128;" ::: "memory");   // the staging area is read before it is reused
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tmem_dealloc<NB>(tmem);
+    wgmma_wait<0>();
+    wgmma_fence_regs<NB / 2>(acc);
+    wg_consumers_sync();  // every MMA has retired: ring and operand buffers are free for the staging tile
+    // registers -> 128B-swizzled staging tile -> TMA reduce-add of the partial tile into partial[job][m'][n']
+    store_acc_sw128<NB>(smem, acc, half * 64);
+    fence_proxy_async();
+    wg_consumers_sync();
+    if (ct == 0) {
+      // all pixel splits of a job accumulate into the same [job][M'][N'] tile: TMA reduce-add (fp32 add at L2)
+      const int row0 = job * p.mtotal + mt * 128;
+#pragma unroll 1
+      for (int c = 0; c < NB; c += 32) tma_reduce_add_2d(&tmP, smem + (c >> 5) * 16384, nt * NB + c, row0);
+      tma_store_commit_and_wait_read();
+    }
   }
 }
 
@@ -299,17 +285,7 @@ struct WgPlan {
   int s_is_a, NB, mtiles, ntiles, mtotal, ldn, njobs, bwl, bhl, tiles_w, tiles_h, tiles_total, nsplits, tps, Ho, Wo;
   int sch, dch;  // channels of the shifted / dense operand
   int ipb;
-  int pix;       // pixels per stage (32 or 64)
 };
-
-static int wg_pix_pref() {
-  static const int v = [] {
-    const char *e = getenv("B200GAN_WG_PIX");
-    const int x = e ? atoi(e) : 64;
-    return x == 32 ? 32 : 64;
-  }();
-  return v;
-}
 
 static bool wg_plan(const b200gan_conv_geom *g, WgPlan &pl) {
   if (g->pad_mode != B200GAN_PAD_ZERO || g->N < 1) return false;
@@ -333,9 +309,8 @@ static bool wg_plan(const b200gan_conv_geom *g, WgPlan &pl) {
   else return false;
   const int mch = pl.s_is_a ? pl.sch : pl.dch, nch = pl.s_is_a ? pl.dch : pl.sch;
   pl.NB = nch % 128 == 0 ? 128 : (nch % 64 == 0 ? 64 : 32);
-  // 128 x 256 output tiles: the 128-channel operand is re-read half as often.  The kernel is L2 -> SM bound (a 256 -> 256
-  // 3x3 layer pulls 9 jobs x 4 tiles x 33 MB = 1.2 GB through L2 in 132 us with 128 x 128 tiles).
-  // measured (call 19): 132.6 -> 113.8 us on that layer, CycleGAN step 76.5 -> 74.7 ms.  B200GAN_WG_NB256=0 switches it off.
+  // 128 x 256 output tiles: the 128-channel operand is re-read and re-transposed half as often (a 256 -> 256 3x3 layer
+  // pulls 9 jobs x 4 tiles x 33 MB = 1.2 GB through L2 with 128 x 128 tiles).  B200GAN_WG_NB256=0 switches it off.
   static const int nb256 = getenv("B200GAN_WG_NB256") ? atoi(getenv("B200GAN_WG_NB256")) : 1;
   if (nb256 && nch % 256 == 0) pl.NB = 256;
   pl.mtotal = mch;
@@ -346,22 +321,19 @@ static bool wg_plan(const b200gan_conv_geom *g, WgPlan &pl) {
   // pixel grid the contraction runs over = grid of the dense operand (low-res grid for the upsample fold)
   pl.Ho = up2 ? g->H : (g->transposed ? g->H : g->P);
   pl.Wo = up2 ? g->W : (g->transposed ? g->W : g->Q);
-  // 64-pixel stages for the 64-wide B operand (two CTAs per SM still fit with two stages); 128-wide keeps 32
-  static const bool pix64_wide = getenv("B200GAN_WG_PIX128") && atoi(getenv("B200GAN_WG_PIX128")) == 64;  // experiment
-  pl.pix = ((pl.NB == 64 || (pl.NB == 128 && pix64_wide)) && wg_pix_pref() == 64 && (int64_t)pl.Ho * pl.Wo >= 64) ? 64 : 32;
-  const int pl2 = pl.pix == 64 ? 6 : 5;
+  const int pl2 = 5;  // log2(WG_PIX)
   pl.bwl = ilog2c(pl.Wo);
   if (pl.bwl > pl2) pl.bwl = pl2;
   pl.bhl = ilog2c(pl.Ho);
   if (pl.bhl > pl2 - pl.bwl) pl.bhl = pl2 - pl.bwl;
   pl.tiles_w = ceil_div(pl.Wo, 1 << pl.bwl);
   pl.tiles_h = ceil_div(pl.Ho, 1 << pl.bhl);
-  pl.ipb = pl.pix >> (pl.bwl + pl.bhl);  // images per box (>1 only when the whole map has fewer pixels than a stage)
+  pl.ipb = WG_PIX >> (pl.bwl + pl.bhl);  // images per box (>1 only when the whole map has fewer pixels than a stage)
   int64_t tt = (int64_t)ceil_div(g->N, pl.ipb) * pl.tiles_w * pl.tiles_h;
   if (tt > (1 << 30)) return false;
   pl.tiles_total = (int)tt;
   int ctas_per_split = pl.njobs * pl.mtiles * pl.ntiles;
-  int ns = (2 * 148 + ctas_per_split - 1) / ctas_per_split;
+  int ns = (2 * num_sms() + ctas_per_split - 1) / ctas_per_split;
   int max_ns = pl.tiles_total / 8;
   if (max_ns < 1) max_ns = 1;
   if (ns > max_ns) ns = max_ns;
@@ -382,23 +354,23 @@ size_t tc_wgrad_workspace_floats(const b200gan_conv_geom *g) {
   return (size_t)pl.njobs * pl.mtotal * pl.ldn;
 }
 
-template <int NB, int STAGES, int PIX>
+template <int NB, int STAGES>
 static int launch_wg(const CUtensorMap &tmX, const CUtensorMap &tmY, const CUtensorMap &tmP, const WgParams &p, dim3 grid,
                      cudaStream_t st) {
-  constexpr int SMEM = STAGES * (4 + NB / 32) * (PIX * 128) + 1024 + 256;
+  constexpr int SMEM = WgSmem<NB, STAGES>::TOTAL;
   static std::atomic<uint64_t> attr_done{0};
-  if (int e = ensure_dynamic_smem(wgrad_tc_kernel<NB, STAGES, PIX>, SMEM, attr_done)) return e;
-  wgrad_tc_kernel<NB, STAGES, PIX><<<grid, WG_THREADS, SMEM, st>>>(tmX, tmY, tmP, p);
+  if (int e = ensure_dynamic_smem(wgrad_tc_kernel<NB, STAGES>, SMEM, attr_done)) return e;
+  wgrad_tc_kernel<NB, STAGES><<<grid, WG_THREADS, SMEM, st>>>(tmX, tmY, tmP, p);
   B2_LAUNCH_CHECK();
   return B200GAN_OK;
 }
 
 int tc_wgrad(const b200gan_conv_geom *g, const float *x, const float *dy, float *dw, float *ws, cudaStream_t st) {
   WgPlan pl;
-  if (!wg_plan(g, pl)) B2_UNSUPPORTED("tcgen05 wgrad: geometry not supported");
-  B2_CHECK_ARG(ws != nullptr, "tcgen05 wgrad: workspace required");
+  if (!wg_plan(g, pl)) B2_UNSUPPORTED("tensor-core wgrad: geometry not supported");
+  B2_CHECK_ARG(ws != nullptr, "tensor-core wgrad: workspace required");
   B2_CHECK_ARG(((uintptr_t)x % 16 == 0) && ((uintptr_t)dy % 16 == 0) && ((uintptr_t)ws % 16 == 0),
-               "tcgen05 wgrad: pointers must be 16-byte aligned");
+               "tensor-core wgrad: pointers must be 16-byte aligned");
   const bool up2 = g->up == 2;
   const int st2 = g->stride == 2;
   WgParams p;
@@ -430,8 +402,6 @@ int tc_wgrad(const b200gan_conv_geom *g, const float *x, const float *dy, float 
   p.tiles_total = pl.tiles_total; p.tiles_per_split = pl.tps;
   p.s_is_a = pl.s_is_a; p.mtiles = pl.mtiles; p.ntiles = pl.ntiles; p.ldn = pl.ldn; p.mtotal = pl.mtotal;
   p.partial = ws;
-  p.lbo = pl.pix * 128;
-  p.sbo = 512;
 
   // operand tensors: Conv2d: S = x [N][H][W][C], D = dy [N][P][Q][K]; ConvTranspose2d: S = dy, D = x
   const float *sptr = g->transposed ? dy : x, *dptr = g->transposed ? x : dy;
@@ -448,7 +418,7 @@ int tc_wgrad(const b200gan_conv_geom *g, const float *x, const float *dy, float 
       dims[0] = 2 * Cs; dims[1] = Ws / 2; dims[2] = 2; dims[3] = Hs / 2; dims[4] = g->N;
       strides[0] = 2 * Cs * 4; strides[1] = Ws * Cs * 4; strides[2] = 2 * Ws * Cs * 4; strides[3] = Hs * Ws * Cs * 4;
     }
-    if (int e = make_tmap_f32(&tmX, sptr, 5, dims, strides, box, 1)) return e;
+    if (int e = make_tmap_f32(&tmX, sptr, 5, dims, strides, box)) return e;
   }
   {
     uint64_t dims[5], strides[4];
@@ -459,7 +429,7 @@ int tc_wgrad(const b200gan_conv_geom *g, const float *x, const float *dy, float 
       dims[0] = 2 * Cd; dims[1] = Wd / 2; dims[2] = 2; dims[3] = Hd / 2; dims[4] = g->N;
       strides[0] = 2 * Cd * 4; strides[1] = Wd * Cd * 4; strides[2] = 2 * Wd * Cd * 4; strides[3] = Hd * Wd * Cd * 4;
     }
-    if (int e = make_tmap_f32(&tmY, dptr, 5, dims, strides, box, 1)) return e;
+    if (int e = make_tmap_f32(&tmY, dptr, 5, dims, strides, box)) return e;
   }
   CUtensorMap tmP;
   {
@@ -470,12 +440,10 @@ int tc_wgrad(const b200gan_conv_geom *g, const float *x, const float *dy, float 
   }
   B2_CUDA(cudaMemsetAsync(ws, 0, (size_t)pl.njobs * pl.mtotal * pl.ldn * sizeof(float), st));
   dim3 grid((unsigned)pl.nsplits, (unsigned)pl.njobs, (unsigned)(pl.mtiles * pl.ntiles));
-  int rc = pl.NB == 256 ? launch_wg<256, 2, 32>(tmX, tmY, tmP, p, grid, st)
-           : pl.NB == 128 ? (pl.pix == 64 ? launch_wg<128, 2, 64>(tmX, tmY, tmP, p, grid, st)
-                                        : launch_wg<128, 3, 32>(tmX, tmY, tmP, p, grid, st))
-           : pl.NB == 64 ? (pl.pix == 64 ? launch_wg<64, 2, 64>(tmX, tmY, tmP, p, grid, st)
-                                         : launch_wg<64, 4, 32>(tmX, tmY, tmP, p, grid, st))
-                         : launch_wg<32, 4, 32>(tmX, tmY, tmP, p, grid, st);
+  int rc = pl.NB == 256 ? launch_wg<256, 2>(tmX, tmY, tmP, p, grid, st)
+           : pl.NB == 128 ? launch_wg<128, 3>(tmX, tmY, tmP, p, grid, st)
+           : pl.NB == 64 ? launch_wg<64, 4>(tmX, tmY, tmP, p, grid, st)
+                         : launch_wg<32, 4>(tmX, tmY, tmP, p, grid, st);
   if (rc) return rc;
   WgReduceP rp;
   rp.K = g->K; rp.C = g->C; rp.R = g->R; rp.S = g->S; rp.njobs = pl.njobs;
@@ -490,7 +458,7 @@ int tc_wgrad(const b200gan_conv_geom *g, const float *x, const float *dy, float 
     B2_LAUNCH_CHECK();
     return B200GAN_OK;
   }
-  unsigned blocks = (unsigned)(ceil_div64(total, 256) > 2368 ? 2368 : ceil_div64(total, 256));
+  unsigned blocks = (unsigned)(ceil_div64(total, 256) > num_sms() * 16 ? num_sms() * 16 : ceil_div64(total, 256));
   wgrad_reduce_kernel<<<blocks, 256, 0, st>>>(ws, dw, rp);
   B2_LAUNCH_CHECK();
   return B200GAN_OK;

@@ -1,7 +1,7 @@
 """A small stand-alone GAN training script written in the API idiom of the reference's scripts -- torch.nn classes looked
 up by attribute on `nn` at model-construction time, `nn.Sequential(*layers)`, name-based weight init through `.apply`,
 `torch.cuda.FloatTensor(numpy_array)`, `Variable`, `.type(Tensor)`, `loss.cuda()`, torchvision's MNIST loader -- so that
-the launcher (b200gan/launch.py) can be exercised END TO END ON A GPU BOX, where /root/reference does not exist.  It is
+the launcher (b200gan/launch.py) can be exercised END TO END without the reference checkout.  It is
 not a copy of any reference script: two-stage generator, three-block discriminator, its own option names."""
 import argparse
 

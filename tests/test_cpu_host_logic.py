@@ -1,5 +1,5 @@
 """Host-side logic of the C ABI and of the module planner, without a GPU: geometry validation, which pass of which
-reference layer the tcgen05 path takes, workspace / packed sizes, error reporting.  None of these calls launches a
+reference layer the wgmma path takes, workspace / packed sizes, error reporting.  None of these calls launches a
 kernel (the library's host entry points validate before they touch CUDA)."""
 import ctypes
 import itertools
@@ -23,7 +23,7 @@ def _geom(x_shape, w_shape, stride, pad, up=1, transposed=False, pads=None):
 DCGAN_LAYERS = [
     ("G conv1 up2 128->128 @16", (128, 128, 16, 16), (128, 128, 3, 3), 1, 1, 2, (True, True, True)),
     ("G conv2 up2 128->64 @32", (128, 128, 32, 32), (64, 128, 3, 3), 1, 1, 2, (True, True, True)),
-    # (fused into the tail kernels in the step; stand-alone, its forward takes the narrow-output tcgen05 form)
+    # (fused into the tail kernels in the step; stand-alone, its forward takes the narrow-output wgmma form)
     ("G conv3 64->1 @64", (128, 64, 64, 64), (1, 64, 3, 3), 1, 1, 1, (True, False, False)),
     ("D conv1 1->16 s2 @64", (128, 1, 64, 64), (16, 1, 3, 3), 2, 1, 1, (False, False, False)),
     ("D conv2 16->32 s2 @32", (128, 16, 32, 32), (32, 16, 3, 3), 2, 1, 1, (False, False, False)),
@@ -60,7 +60,7 @@ def test_planner_mirror_never_claims_more_than_the_library():
         actual = ops.tc_supported(g, 0)
         if claimed:
             assert actual, (cin, cout, k, stride, up, tr)
-        narrow = cout < 32 and cin % 32 == 0 and stride == 1 and up == 1 and not tr   # forward-only tcgen05 form
+        narrow = cout < 32 and cin % 32 == 0 and stride == 1 and up == 1 and not tr   # forward-only wgmma form
         if (cin % 32 or cout % 32) and not narrow:
             assert not actual
         if narrow:
@@ -88,7 +88,7 @@ def test_pix2pix_and_cyclegan_hot_layers_are_tensor_core_eligible():
     for xs, ws, stride, pad in [((1, 6, 256, 256), (64, 6, 4, 4), 2, 1), ((2, 3, 70, 70), (64, 3, 7, 7), 1, 0)]:
         g, _ = _geom(xs, ws, stride, pad)
         assert not ops.tc_supported(g, 0)
-    # few-output-channel layers: forward on tcgen05 (narrow form), gradients fp32 -- the 1-channel PatchGAN head
+    # few-output-channel layers: forward on wgmma (narrow form), gradients fp32 -- the 1-channel PatchGAN head
     # (pix2pix/models.py:127) and the 3-channel output conv (cyclegan/models.py:82, on the reflection-padded map)
     for xs, ws, stride, pad in [((1, 512, 17, 17), (1, 512, 4, 4), 1, 1), ((2, 64, 70, 70), (3, 64, 7, 7), 1, 0)]:
         g, _ = _geom(xs, ws, stride, pad)
@@ -125,10 +125,10 @@ def test_packed_and_workspace_sizes():
         assert lib.b200gan_packed_weight_floats(ctypes.byref(g), pack) == 9 * 128 * 64
     for pack in (_lib.PACK_TC_FPROP_UP2, _lib.PACK_TC_DGRAD_UP2):  # four phases x four pre-summed 2x2 taps
         assert lib.b200gan_packed_weight_floats(ctypes.byref(g), pack) == 16 * 128 * 64
-    # tcgen05 weight gradient: one [Cin x Cout] partial per (phase, tap) job; SIMT accumulates in place
+    # wgmma weight gradient: one [Cin x Cout] partial per (phase, tap) job; SIMT accumulates in place
     assert lib.b200gan_conv2d_wgrad_workspace_floats(ctypes.byref(g), _lib.ALGO_TC) == 16 * 128 * 64
     assert lib.b200gan_conv2d_wgrad_workspace_floats(ctypes.byref(g), _lib.ALGO_SIMT) == 0
-    # tcgen05 dgrad of the fold writes dx directly; the SIMT path goes through the upsampled gradient
+    # wgmma dgrad of the fold writes dx directly; the SIMT path goes through the upsampled gradient
     assert lib.b200gan_conv2d_dgrad_workspace_floats(ctypes.byref(g), _lib.ALGO_TC) == 0
     assert lib.b200gan_conv2d_dgrad_workspace_floats(ctypes.byref(g), _lib.ALGO_SIMT) == 128 * 128 * 64 * 64
     g1, _ = _geom((128, 64, 8, 8), (128, 64, 3, 3), 2, 1)

@@ -212,36 +212,38 @@ def test_wgan_gp_oracle_and_closed_form_against_reference_golden(golden_dir):
     assert abs(np.linalg.norm(dw2) - fix["dW2_norm"]) < 1e-5 * fix["dW2_norm"]
 
 
-REF = "/root/reference/implementations"
-
-
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference checkout not present on this box")
-def test_launcher_runs_unmodified_gan_script_on_cpu_config0():
-    """BASELINE config 0: implementations/gan/gan.py, 28x28 synthetic, batch 64, CPU -- the unmodified script
-    under the launcher with the drop-in classes patched in (MLP: stock ops through the same classes) prints the
-    same losses as the stock run."""
-    from b200gan import launch
-    args = ["--n_epochs", "1", "--batch_size", "64", "--sample_interval", "1000"]
-    ours = launch.run(os.path.join(REF, "gan", "gan.py"), args, iters=3, seed=0, stock=False, quiet=True)
-    stock = launch.run(os.path.join(REF, "gan", "gan.py"), args, iters=3, seed=0, stock=True, quiet=True)
-    lines = [l for l in ours["__b200_stdout__"].splitlines() if "[D loss" in l]
+def test_launcher_trains_a_reference_idiom_mlp_script_on_cpu_like_stock():
+    """BASELINE config 0 on a project-owned script (tests/scripts/mini_mlpgan: Linear / BatchNorm1d / LeakyReLU MLPs,
+    synthetic MNIST, CPU): three training iterations under the launcher with the drop-in classes patched in print the
+    same losses as the stock run of the same script."""
+    from b200gan import launch, nn as bnn
+    script = os.path.join(os.path.dirname(os.path.abspath(__file__)), "scripts", "mini_mlpgan", "mini_mlpgan.py")
+    args = ["--epochs", "1", "--batch_size", "32"]
+    ours = launch.run(script, args, iters=3, seed=0, stock=False, quiet=True)
+    stock = launch.run(script, args, iters=3, seed=0, stock=True, quiet=True)
+    lines = [l for l in ours["__b200_stdout__"].splitlines() if "[D " in l]
     assert len(lines) == 3
     assert ours["__b200_stdout__"] == stock["__b200_stdout__"]
-    assert type(ours["generator"].model[1]).__name__ == "LeakyReLU"
-    from b200gan import nn as bnn
-    assert isinstance(ours["generator"].model, bnn.Sequential)
-    assert not isinstance(stock["generator"].model, bnn.Sequential)
+    assert isinstance(ours["G"].net, bnn.Sequential) and isinstance(ours["G"].net[0], bnn.Linear)
+    assert type(ours["G"].net[1]).__name__ == "LeakyReLU"
+    assert not isinstance(stock["G"].net, bnn.Sequential)
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference checkout not present on this box")
-def test_launcher_builds_dcgan_with_drop_in_modules():
+def test_launcher_builds_drop_in_modules_with_the_stock_init_draws():
+    """launch.run() of a stand-alone script in the reference's API idiom (tests/scripts/mini_convgan, no training
+    iterations): the model is built from the drop-in classes and draws the same initial parameters as the stock run of
+    the same script."""
     from b200gan import launch, nn as bnn
-    g = launch.run(os.path.join(REF, "dcgan", "dcgan.py"), ["--n_epochs", "0", "--img_size", "32"], iters=1, seed=0,
-                   quiet=True)
-    gen, ref = g["generator"], ref_models.build_dcgan(32, seed=0)[0]
-    assert isinstance(gen.conv_blocks, bnn.Sequential) and isinstance(gen.conv_blocks[2], bnn.Conv2d)
-    for k, v in ref.state_dict().items():   # same init draws as the stock run of the same script
-        assert torch.equal(gen.state_dict()[k], v), k
+    script = os.path.join(os.path.dirname(os.path.abspath(__file__)), "scripts", "mini_convgan", "mini_convgan.py")
+    args = ["--epochs", "0", "--side", "32"]
+    ours = launch.run(script, args, iters=1, seed=0, quiet=True)
+    stock = launch.run(script, args, iters=1, seed=0, stock=True, quiet=True)
+    assert isinstance(ours["G"].body, bnn.Sequential) and isinstance(ours["G"].body[2], bnn.Conv2d)
+    assert isinstance(ours["D"].body[0], bnn.Conv2d)
+    assert not isinstance(stock["G"].body, bnn.Sequential)
+    for net in ("G", "D"):
+        for k, v in stock[net].state_dict().items():
+            assert torch.equal(ours[net].state_dict()[k], v), (net, k)
 
 
 def test_pix2pix_and_cyclegan_oracle_against_reference_golden(golden_dir):

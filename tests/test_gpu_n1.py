@@ -1,7 +1,7 @@
 """SURVEY.md section 8(f) N1: the ConvTranspose2d + BatchNorm2d(.8) + ReLU stacks of context_encoder/models.py:10-37 and
 ccgan/models.py:10-42 (the stack BASELINE's north star names), including the 1x1 bottleneck Conv2d(512, 4000, 1)
 (context_encoder/models.py:30): fusion plan and parity of outputs / every parameter gradient against stock torch fp32,
-with the stock-TF32 yardstick (these layers all run on tcgen05)."""
+with the stock-TF32 yardstick (these layers all run on wgmma)."""
 import copy
 
 import pytest

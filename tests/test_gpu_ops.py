@@ -49,7 +49,7 @@ CONV_CASES = [  # cin, cout, k, stride, pad, H, W, N   -- every geometry of SURV
     (128, 64, 3, 1, 1, 24, 20, 3),   # tensor-core with ragged tiles
     (256, 256, 3, 1, 0, 18, 18, 1),  # cyclegan residual conv on a padded map
     (64, 128, 7, 1, 3, 16, 16, 1),
-    (64, 256, 3, 1, 1, 64, 48, 7),   # 256-wide tcgen05 tiles in fprop (>= 148 tiles), ragged
+    (64, 256, 3, 1, 1, 64, 48, 7),   # 256-wide tiles in fprop (>= 132 tiles), ragged
     (256, 32, 3, 2, 1, 64, 64, 8),   # ... and in the (scatter-form, four-phase) data gradient
 ]
 
@@ -128,7 +128,7 @@ def test_conv_golden_vectors_from_torch_cpu(golden_dir):
 @pytest.mark.parametrize("cin,cout,h,w,n", [(128, 128, 16, 16, 4), (128, 64, 32, 32, 2), (64, 64, 8, 8, 3),
                                             (32, 16, 6, 5, 2)])
 def test_upsample_conv_folded(cin, cout, h, w, n):
-    """Upsample(x2) -> Conv3x3 inside a Sequential: the 4-phase fold (tcgen05) or the gather (SIMT)."""
+    """Upsample(x2) -> Conv3x3 inside a Sequential: the 4-phase fold (wgmma) or the gather (SIMT)."""
     bnn = _mods()
     torch.manual_seed(3)
     ref = torch.nn.Sequential(torch.nn.Upsample(scale_factor=2), torch.nn.Conv2d(cin, cout, 3, 1, 1)).cuda()
@@ -153,8 +153,8 @@ def test_upsample_conv_folded(cin, cout, h, w, n):
                                                  ("in", 32, 64, 16, 8, 2), ("bn", 32, 192, 4, 4, 5)])
 def test_upsample_conv_norm_act_all_phase_kernel(norm, cin, cout, h, w, n, slope):
     """Upsample -> Conv3x3 -> BatchNorm/InstanceNorm -> LeakyReLU (dcgan.py:54-57; cyclegan/models.py:73-78).  With
-    64 (mod 128) output channels the forward runs in the all-phase tcgen05 kernel: 9 shifted operand tiles feed four
-    TMEM accumulators, the norm statistics are summed over the four phases in the epilogue.  Ragged and < 128-pixel
+    64 (mod 128) output channels the forward runs in the all-phase wgmma kernel: 9 shifted operand tiles feed four
+    register accumulators, the norm statistics are summed over the four phases in the epilogue.  Ragged and < 128-pixel
     maps exercise TMA clipping; the InstanceNorm case needs one image per tile.
 
     Gradients: a TF32 forward leaves a few pre-activations with |norm(z)| < 5e-4 on the other side of the LeakyReLU
@@ -432,7 +432,7 @@ def test_all_phase_kernel_unmasked_gradient_vs_stock_cudnn_tf32():
 @pytest.mark.parametrize("n,hw", [(4, 8), (16, 4), (2, 16)])
 def test_deep_unet_layers_split_k(n, hw):
     """pix2pix/models.py:62-73: Conv2d(C, C, 4, 2, 1, bias=False) -> InstanceNorm2d -> LeakyReLU and ConvTranspose2d(...,
-    bias=False) -> InstanceNorm2d -> ReLU at 4x4 .. 16x16 pixels: a handful of output tiles, so the tcgen05 kernel splits
+    bias=False) -> InstanceNorm2d -> ReLU at 4x4 .. 16x16 pixels: a handful of output tiles, so the wgmma kernel splits
     the (tap, k-chunk) loop over CTAs and adds raw partial tiles with TMA reduce-stores; the norm statistics then come
     from a separate pass.  Forward, input gradient, weight gradients vs stock torch fp32."""
     bnn = _mods()

@@ -1,6 +1,6 @@
 """GPU parity of the fused Generator tail (csrc/tail.cu): BatchNorm2d -> LeakyReLU/ReLU -> Conv2d(C, K<=3, 3, 1, 1)
 -> Tanh (dcgan.py:60-63) against stock torch fp32 on the same GPU: output, the gradient that flows into the preceding
-conv, and every parameter gradient.  The forward conv runs on tcgen05 (TF32 operands): 1e-3 on the output; the backward
+conv, and every parameter gradient.  The forward conv runs on wgmma (TF32 operands): 1e-3 on the output; the backward
 kernels are fp32, so the gradients only see the TF32 forward through tanh'."""
 import pytest
 import torch

@@ -106,12 +106,12 @@ def test_multi_tensor_adam_in_a_cuda_graph():
 
 
 def test_adam_step_invalidates_the_packed_weight_caches():
-    """The optimizer kernel writes parameters through raw pointers; the conv modules' packed (tcgen05 / SIMT) weight
+    """The optimizer kernel writes parameters through raw pointers; the conv modules' packed (wgmma / SIMT) weight
     copies are keyed on the tensor version counter, which optim.Adam bumps.  Forward after a step must use the NEW
     weights (fprop and dgrad read packed copies)."""
     from b200gan import nn as bnn, optim
     torch.manual_seed(9)
-    for cin, cout in ((64, 64), (3, 8)):      # tcgen05 path and SIMT path
+    for cin, cout in ((64, 64), (3, 8)):      # wgmma path and SIMT path
         ours = bnn.Conv2d(cin, cout, 3, 1, 1).cuda()
         ref = torch.nn.Conv2d(cin, cout, 3, 1, 1).cuda()
         ref.load_state_dict(ours.state_dict())

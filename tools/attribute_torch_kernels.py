@@ -1,11 +1,11 @@
 """Which Python lines launch the small torch kernels of the DCGAN step?
 
-The final launch list of round 1 (profiles/r1_launch_list_dcgan_step_final.txt) has 186 torch kernels (fills, element-wise
-ops, multi-tensor Adam, RNG) worth ~0.88 ms of a 3.76 ms step next to 152 libb200gan kernels.  This tool runs a few EAGER
+The DCGAN step launches torch kernels (fills, element-wise ops, multi-tensor Adam, RNG) next to the libb200gan
+kernels.  This tool runs a few EAGER
 steps (no CUDA graph) under torch.profiler with Python stacks and prints, per kernel name, how often it runs per step and
 the innermost frames of this repository that caused it.  GPU only:
 
-    gpurun -- 'python tools/attribute_torch_kernels.py > gpurun_out/torch_kernels.txt'
+    python tools/attribute_torch_kernels.py > torch_kernels.txt
 """
 import collections
 import os

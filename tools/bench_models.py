@@ -1,5 +1,5 @@
 """Step throughput of BASELINE configs 2-4 (WGAN-GP 32x32 bs64, Pix2Pix 256x256 bs16, CycleGAN 256x256 bs8) on one
-B200 with the drop-in modules, next to the same step on stock torch (cuDNN, TF32 default = the reference's own GPU
+H100 with the drop-in modules, next to the same step on stock torch (cuDNN, TF32 default = the reference's own GPU
 path).  Eager loops (no CUDA graph), CUDA-event timing.  Prints one JSON line per config.
 
     python tools/bench_models.py [--steps 10] [--only pix2pix|cyclegan|wgan_gp]

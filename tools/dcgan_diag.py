@@ -1,5 +1,5 @@
 """Where does DCGAN gradient error come from?  Per-parameter relative error of
-  (a) b200gan auto (tcgen05 TF32 for the big convs)   vs stock torch fp32 (cuDNN, TF32 off)
+  (a) b200gan auto (wgmma TF32 for the big convs)     vs stock torch fp32 (cuDNN, TF32 off)
   (b) b200gan simt (pure fp32 kernels)                vs stock torch fp32
   (c) stock torch with TF32 ON (the reference's default GPU path) vs stock torch fp32
 on identical inputs/parameters.  (c) is the yardstick: it is "the reference's own PyTorch/cuDNN path"."""

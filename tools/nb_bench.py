@@ -2,7 +2,7 @@
 the BASELINE size (batch 128, 64x64): 20 launches captured in a CUDA graph, CUDA events around 10 replays (operands of one
 layer fit in L2: these are the warm numbers the training step sees; the step's ncu launch list is the cold view).  Each
 launch includes the wrapper's memset nodes (statistics / sums buffers).
-    python tools/nb_bench.py            # run on the GPU box
+    python tools/nb_bench.py            # needs the GPU
 """
 import os
 import sys

@@ -2,7 +2,7 @@
 of the four DCGAN discriminator layers, forward and data gradient, one pass (N = 128) and the grouped D-step pass
 (N = 256, two statistics groups), CUDA-graph timed like tools/nb_bench.py.  Prints the planner's own choice next to the
 best candidate.
-    python tools/nb_sweep.py            # run on the GPU box
+    python tools/nb_sweep.py            # needs the GPU
 """
 import os
 import sys

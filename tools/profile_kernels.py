@@ -79,7 +79,7 @@ def main():
                 fn = lambda: ops.conv_wgrad(g, x, dy, tuple(wt.shape), True, ALGO_AUTO)  # noqa: E731
             ms = timeit(fn, a.iters)
             fl = flops_exec if tc else flops_ref
-            rows.append((name, pname, "tcgen05" if tc else "simt", ms * 1e3, fl / ms / 1e9, act_bytes / ms / 1e6))
+            rows.append((name, pname, "wgmma" if tc else "simt", ms * 1e3, fl / ms / 1e9, act_bytes / ms / 1e6))
     print(f"{'layer':28s} {'pass':6s} {'path':8s} {'us':>9s} {'TFLOP/s':>9s} {'GB/s(act)':>10s}")
     for r in rows:
         print(f"{r[0]:28s} {r[1]:6s} {r[2]:8s} {r[3]:9.1f} {r[4]:9.2f} {r[5]:10.0f}")

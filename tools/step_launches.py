@@ -1,7 +1,7 @@
 """One training step's launch list out of an `ncu --metrics gpu__time_duration.sum --csv` log of bench.py: finds the
 period of the kernel-name sequence at the end of the log (graph replays repeat the step) and aggregates ONE period.
 
-    python tools/step_launches.py gpurun_out/launches.csv [top]
+    python tools/step_launches.py launches.csv [top]
 """
 import collections
 import csv
