@@ -4,13 +4,15 @@
 // (reference: autograd of nn.Conv2d, dcgan.py:168,182 -> cudnnConvolutionBackwardFilter).
 //
 // As a GEMM the contraction runs over PIXELS, so both operands arrive "MN-major": a TMA box {32 channels, BW, 1, BH,
-// ipb} (32 pixels) lands in shared memory as 32 pixel rows x 128 B (128-byte swizzle).  wgmma takes TF32 operands only
-// K-major, so the consumer warpgroups transpose every stage into K-major 128B-swizzled tiles (channel rows of 32
-// pixels; double-buffered, so the transpose of stage i overlaps the MMAs of stage i-1).  The operand with a multiple of
-// 128 channels is A (M = 128: two warpgroups of 64 rows), the other is B (N = 32..256).  Zero padding = TMA
-// out-of-bounds fill on the shifted x box.  The upsample-folded convolution (dcgan.py:54-55,58-59) contributes 16
-// (phase, tap) jobs that read dy through the phase view {2K, Q/2, 2, P/2, N}; a second kernel folds them back into the
-// 3x3 filter.
+// ipb} (32 pixels) lands in shared memory as 32 pixel rows x 128 B (128-byte swizzle).  wgmma takes TF32 operands from
+// shared memory only K-major.  The operand with a multiple of 128 channels is A (M = 128: two warpgroups of 64 rows);
+// it goes to wgmma as register fragments, loaded with 32-bit LDS straight from the TMA stage.  The other, B (N =
+// 32..256), is transposed by the consumer warpgroups into a K-major 128B-swizzled tile (channel rows of 32 pixels;
+// double-buffered, so that stage i+1 is prepared while the MMAs of stage i run).  Inside every 8-pixel k slice both
+// operands take the pixels in the order 0 2 4 6 1 3 5 7 (wg_kpos), which makes the fragment loads free of bank
+// conflicts.  Zero padding = TMA out-of-bounds fill on the shifted x box.  The upsample-folded convolution
+// (dcgan.py:54-55,58-59) contributes 16 (phase, tap) jobs that read dy through the phase view {2K, Q/2, 2, P/2, N}; a
+// second kernel folds them back into the 3x3 filter.
 //
 // Parallelisation: grid = (pixel splits, jobs, M-tiles x N-tiles).  Every CTA accumulates its pixel range in
 // registers, stages the tile in shared memory and adds it into the job's [M'][N'] matrix with a TMA reduce-store
@@ -48,20 +50,26 @@ struct WgParams {
   float *partial;                 // [job][M'][N'], zeroed by the host; splits accumulate with TMA reduce-add
 };
 
-// shared memory: TMA ring | two K-major operand buffers; after the last MMA the front is the staging tile
+// shared memory: TMA ring | two K-major B buffers; after the last MMA the front is the staging tile
 template <int NB, int STAGES>
 struct WgSmem {
   static constexpr int A_BYTES = 4 * WG_CHUNK_BYTES;            // 128 channels
   static constexpr int B_BYTES = (NB / 32) * WG_CHUNK_BYTES;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int RING = STAGES * STAGE_BYTES;
-  static constexpr int T_BYTES = 128 * 128 + NB * 128;          // A^T (128 rows) + B^T (NB rows), 32 pixels each
+  static constexpr int T_BYTES = NB * 128;                      // B^T: NB channel rows of 32 pixels
   static constexpr int STAGING = (NB / 32) * 16384;
   static constexpr int MAIN = RING + 2 * T_BYTES > STAGING ? RING + 2 * T_BYTES : STAGING;
   static constexpr int TOTAL = MAIN + 1024 + 256;
+  static_assert(TOTAL <= 232448, "wgrad_tc_kernel: shared memory");
 };
 
 __device__ __forceinline__ void wg_consumers_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+
+// K position of pixel row p of a stage: inside each 8-pixel k slice, even pixels take positions 0..3 and odd ones 4..7.
+// Thread (l%4) of an A fragment then reads pixels 2(l%4) and 2(l%4) + 1, whose rows have distinct 128-byte swizzle
+// phases for the four values of l%4: the 32 lanes of one fragment load hit 32 different banks.
+__device__ __forceinline__ int wg_kpos(int p) { return (p & ~7) | ((p & 7) >> 1) | ((p & 1) << 2); }
 
 template <int NB, int STAGES>
 __global__ void __launch_bounds__(WG_THREADS, 1)
@@ -86,14 +94,15 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
     tma_prefetch_desc(&tmY);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 256);  // every consumer thread, once its transpose reads of the stage are done
+      mbar_init(&empty[s], 256);  // every consumer thread, once its fragment and transpose reads of the stage are done
     }
     fence_barrier_init();
   }
   __syncthreads();
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    setmaxnreg_dec<40>();
+    if (warp == 0 && lane == 0) {
       const WgJob jb = p.jobs[job];
       const CUtensorMap *mapA = p.s_is_a ? &tmX : &tmY;   // tmX = shifted operand S, tmY = dense operand D
       const CUtensorMap *mapB = p.s_is_a ? &tmY : &tmX;
@@ -128,41 +137,76 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
         }
       }
     }
-  } else if (warp >= 4 && iters > 0) {
+  } else {
+    setmaxnreg_inc<232>();  // 128 x 40 + 256 x 232 registers = the 384 x 168 the kernel starts with
+    if (iters == 0) return;
     const int ct = threadIdx.x - 128;
     const int half = ct >> 7;           // MMA rows [64 * half, +64) of the 128 x NB tile
-    const int tp = ct & 31, tq = ct >> 5;  // transpose: pixel row tp, 16-byte column tq (4 channels) of every chunk
+    const int tp = ct & 31, tq = ct >> 5;  // B transpose: pixel row tp, 16-byte column tq (4 channels) of every chunk
+    const int tk = wg_kpos(tp);
+    // A fragments (wgmma_tf32_rs): warp wq of this warpgroup holds channels 64 * half + 16 * wq + [0, 16), i.e.
+    // channels ac, ac + 8 of 32-channel chunk 2 * half + wq / 2; its k slice j reads pixels 8j + 2(l%4) (+1)
+    const int wq = tq & 3;
+    const int ac = 16 * (wq & 1) + (lane >> 2), ap = 2 * (lane & 3);
+    const int abase = (2 * half + (wq >> 1)) * WG_CHUNK_BYTES + ap * 128 + (ac & 3) * 4;
+    const uint32_t aoff[4] = {
+        (uint32_t)(abase + ((((ac >> 2)) ^ ap) << 4)),                  // a0: channel ac,     pixel ap
+        (uint32_t)(abase + ((((ac >> 2) + 2) ^ ap) << 4)),              // a1: channel ac + 8, pixel ap
+        (uint32_t)(abase + 128 + ((((ac >> 2)) ^ (ap + 1)) << 4)),      // a2: channel ac,     pixel ap + 1
+        (uint32_t)(abase + 128 + ((((ac >> 2) + 2) ^ (ap + 1)) << 4))}; // a3: channel ac + 8, pixel ap + 1
     float acc[NB / 2];                  // the first MMA overwrites it (scale_d = 0)
     int stage = 0;
     uint32_t phase = 0;
-    for (int it = 0; it < iters; ++it) {
-      uint8_t *ta = smem + L::RING + (it & 1) * L::T_BYTES;  // A^T: 128 rows x 128 B, then B^T: NB rows x 128 B
+    // stage `it` -> A fragments fa and the K-major B tile of buffer it & 1; the ring slot is released afterwards
+    auto prepare = [&](int it, uint32_t(&fa)[16]) {
+      uint8_t *tb = smem + L::RING + (it & 1) * L::T_BYTES;  // B^T: NB rows x 128 B
       mbar_wait(&full[stage], phase);
       wg_consumers_sync();  // both warpgroups' MMAs of iteration it-2 (which read this buffer) have retired
       const uint8_t *src = smem + stage * L::STAGE_BYTES;
 #pragma unroll
-      for (int c = 0; c < 4 + NB / 32; ++c) {
-        const float4 v = *reinterpret_cast<const float4 *>(src + c * WG_CHUNK_BYTES + tp * 128 + ((tq ^ (tp & 7)) << 4));
+      for (int k = 0; k < WG_PIX / 8; ++k)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) fa[4 * k + j] = *reinterpret_cast<const uint32_t *>(src + aoff[j] + k * 1024);
+#pragma unroll
+      for (int c = 0; c < NB / 32; ++c) {
+        const float4 v = *reinterpret_cast<const float4 *>(src + L::A_BYTES + c * WG_CHUNK_BYTES + tp * 128 +
+                                                           ((tq ^ (tp & 7)) << 4));
         const float e[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
-          const int r = c * 32 + tq * 4 + i;  // A rows 0..127, then B rows
-          *reinterpret_cast<float *>(ta + r * 128 + (((tp >> 2) ^ (r & 7)) << 4) + (tp & 3) * 4) = e[i];
+          const int r = c * 32 + tq * 4 + i;
+          *reinterpret_cast<float *>(tb + r * 128 + (((tk >> 2) ^ (r & 7)) << 4) + (tk & 3) * 4) = e[i];
         }
       }
       mbar_arrive(&empty[stage]);
       fence_proxy_async();  // generic-proxy smem writes -> visible to wgmma
       wg_consumers_sync();
-      const uint32_t sa = smem_u32(ta) + half * 8192, sb = smem_u32(ta) + 128 * 128;
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < WG_PIX / 8; ++k)
-        wgmma_tf32<NB>(acc, gmma_desc_sw128(sa + k * 32), gmma_desc_sw128(sb + k * 32), (it > 0 || k > 0) ? 1u : 0u);
-      wgmma_commit();
-      wgmma_wait<1>();
       if (++stage == STAGES) {
         stage = 0;
         phase ^= 1;
+      }
+    };
+    auto mma = [&](int it, const uint32_t(&fa)[16]) {
+      const uint32_t sb = smem_u32(smem + L::RING + (it & 1) * L::T_BYTES);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < WG_PIX / 8; ++k)
+        wgmma_tf32_rs<NB>(acc, fa + 4 * k, gmma_desc_sw128(sb + k * 32), (it > 0 || k > 0) ? 1u : 0u);
+      wgmma_commit();
+    };
+    // the MMAs of stage i run while stage i+1 is prepared into the other fragment set and B buffer; a wgmma's
+    // register operands are all defined before it is issued, so ptxas keeps the wgmma pipeline asynchronous
+    uint32_t fa0[16], fa1[16];
+    prepare(0, fa0);
+#pragma unroll 1
+    for (int it = 0; it < iters; it += 2) {
+      mma(it, fa0);
+      if (it + 1 < iters) prepare(it + 1, fa1);
+      wgmma_wait<0>();
+      if (it + 1 < iters) {
+        mma(it + 1, fa1);
+        if (it + 2 < iters) prepare(it + 2, fa0);
+        wgmma_wait<0>();
       }
     }
     wgmma_wait<0>();
@@ -332,12 +376,23 @@ static bool wg_plan(const b200gan_conv_geom *g, WgPlan &pl) {
   int64_t tt = (int64_t)ceil_div(g->N, pl.ipb) * pl.tiles_w * pl.tiles_h;
   if (tt > (1 << 30)) return false;
   pl.tiles_total = (int)tt;
-  int ctas_per_split = pl.njobs * pl.mtiles * pl.ntiles;
-  int ns = (2 * num_sms() + ctas_per_split - 1) / ctas_per_split;
+  // pixel splits: one CTA per SM fits (shared memory), so the kernel takes waves x (stages per CTA + fill and epilogue,
+  // about 8 stages).  Pick the split count with the least of that; a last wave that is nearly empty costs as much as a
+  // full one (16 jobs x 17 splits on 132 SMs ran 3 waves where 16 x 8 runs one of twice the length).
+  const int64_t ctas_per_split = (int64_t)pl.njobs * pl.mtiles * pl.ntiles;
   int max_ns = pl.tiles_total / 8;
   if (max_ns < 1) max_ns = 1;
-  if (ns > max_ns) ns = max_ns;
-  if (ns < 1) ns = 1;
+  if (max_ns > 4 * num_sms()) max_ns = 4 * num_sms();
+  int ns = 1;
+  int64_t best = -1;
+  for (int s = 1; s <= max_ns; ++s) {
+    const int64_t waves = ceil_div64(s * ctas_per_split, num_sms());
+    const int64_t cost = waves * (ceil_div(pl.tiles_total, s) + 8);
+    if (best < 0 || cost < best) {
+      best = cost;
+      ns = s;
+    }
+  }
   pl.tps = ceil_div(pl.tiles_total, ns);
   pl.nsplits = ceil_div(pl.tiles_total, pl.tps);
   return true;
@@ -440,10 +495,10 @@ int tc_wgrad(const b200gan_conv_geom *g, const float *x, const float *dy, float 
   }
   B2_CUDA(cudaMemsetAsync(ws, 0, (size_t)pl.njobs * pl.mtotal * pl.ldn * sizeof(float), st));
   dim3 grid((unsigned)pl.nsplits, (unsigned)pl.njobs, (unsigned)(pl.mtiles * pl.ntiles));
-  int rc = pl.NB == 256 ? launch_wg<256, 2>(tmX, tmY, tmP, p, grid, st)
-           : pl.NB == 128 ? launch_wg<128, 3>(tmX, tmY, tmP, p, grid, st)
-           : pl.NB == 64 ? launch_wg<64, 4>(tmX, tmY, tmP, p, grid, st)
-                         : launch_wg<32, 4>(tmX, tmY, tmP, p, grid, st);
+  int rc = pl.NB == 256 ? launch_wg<256, 3>(tmX, tmY, tmP, p, grid, st)
+           : pl.NB == 128 ? launch_wg<128, 6>(tmX, tmY, tmP, p, grid, st)
+           : pl.NB == 64 ? launch_wg<64, 8>(tmX, tmY, tmP, p, grid, st)
+                         : launch_wg<32, 8>(tmX, tmY, tmP, p, grid, st);
   if (rc) return rc;
   WgReduceP rp;
   rp.K = g->K; rp.C = g->C; rp.R = g->R; rp.S = g->S; rp.njobs = pl.njobs;
