@@ -291,8 +291,7 @@ class NormFn(torch.autograd.Function):
         ctx.spec = spec
         # LeakyReLU / ReLU masks are recomputed from x in backward (sign of x * scale + shift): y need not be kept
         c_ = x.shape[1]
-        mask_from_x = (ops.Config.norm_fast and spec.act in (ACT_LRELU, ACT_RELU) and c_ % 4 == 0 and c_ // 4 <= 256
-                       and 256 % (c_ // 4) == 0)
+        mask_from_x = spec.act in (ACT_LRELU, ACT_RELU) and c_ % 4 == 0 and c_ // 4 <= 256 and 256 % (c_ // 4) == 0
         need_y = spec.act != ACT_NONE and not mask_from_x
         ctx.save_for_backward(x, y if need_y else None, mean_rstd, gamma, scale_shift if mask_from_x else None)
         return y

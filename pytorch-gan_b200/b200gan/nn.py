@@ -528,7 +528,7 @@ class Sequential(_T["Sequential"]):
 
     def _run_chain(self, chain, x, nchw_out):
         """Execute a _ChainStep through the fused kernels, or return None if the runtime shapes do not qualify."""
-        if not ops.Config.fuse_narrow_chain or ops.Config.algo == "simt_generic":
+        if not ops.Config.fuse_narrow_chain:
             return None
         shape = tuple(x.shape)
         plan = _chain_plan(chain, shape)

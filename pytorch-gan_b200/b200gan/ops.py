@@ -23,14 +23,8 @@ class Config:
     # a fused Sequential fed an NCHW-contiguous tensor returns an NCHW-contiguous tensor (what a script may .view,
     # dcgan.py:96) only for feature maps of at most this many pixels; larger maps stay channels_last
     contiguous_hw_limit = 64
-    # BatchNorm2d -> act -> Conv2d(C, K<=3, 3, 1, 1) -> act as the fused tail kernels (csrc/tail.cu)
-    fuse_tail = os.environ.get("B200GAN_FUSE_TAIL", "1") not in ("", "0")
     # [Conv2d -> LeakyReLU -> Dropout2d -> BatchNorm2d] runs of narrow layers as the fused chain (csrc/narrow_block.cu)
     fuse_narrow_chain = os.environ.get("B200GAN_FUSE_CHAIN", "1") not in ("", "0")
-    # train.dcgan_step: discriminator(real) and discriminator(fake) as ONE grouped pass through the fused chain
-    batch_d_passes = os.environ.get("B200GAN_BATCH_D", "1") not in ("", "0")
-    # norm kernels: fixed-channel-group fast paths (csrc/norm.cu) and activation mask recomputed from x in backward
-    norm_fast = os.environ.get("B200GAN_NORM_FAST", "1") not in ("", "0")
 
 
 def _stream():
@@ -283,7 +277,7 @@ def tail_desc(a_shape, k, act_mid, slope, act_out):
 
 
 def tail_supported(a_shape, k, act_mid, slope, act_out):
-    if Config.algo == "simt" or not Config.fuse_tail:
+    if Config.algo == "simt":
         return False
     return bool(_lib.load().b200gan_tail_supported(ctypes.byref(tail_desc(a_shape, k, act_mid, slope, act_out))))
 

@@ -46,7 +46,7 @@ def _d_passes_batchable(discriminator, real_imgs, loss):
     that the fused chain covers completely, `adv_layer` without batch-dependent modules, zoo.DCGANDiscriminator /
     dcgan.py:73-99), a mean-reduced element-wise loss, training mode."""
     from . import nn as bnn
-    if not ops.Config.batch_d_passes or not getattr(discriminator, "_b200_batchable_passes", False):
+    if not getattr(discriminator, "_b200_batchable_passes", False):
         return False
     if not (discriminator.training and real_imgs.is_cuda and real_imgs.dim() == 4 and real_imgs.dtype == torch.float32):
         return False

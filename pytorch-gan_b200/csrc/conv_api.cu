@@ -104,33 +104,6 @@ int validate_geom(const b200gan_conv_geom *g) {
 }
 
 // ---- weight packing ---------------------------------------------------------------------------
-// order 0: dst[t][ci][co], order 1: dst[t][co][ci]; t = r*S + s.
-__global__ void pack_kernel(const float *__restrict__ src, float *__restrict__ dst, int R, int S, int Cin,
-                            int Cout, int transposed, int order, int rtf) {
-  int64_t total = (int64_t)R * S * Cin * Cout;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total;
-       i += (int64_t)gridDim.x * blockDim.x) {
-    int ci, co;
-    int64_t t;
-    if (order == 0) {
-      co = (int)(i % Cout);
-      t = i / Cout;
-      ci = (int)(t % Cin);
-      t /= Cin;
-    } else {
-      ci = (int)(i % Cin);
-      t = i / Cin;
-      co = (int)(t % Cout);
-      t /= Cout;
-    }
-    int s = (int)(t % S), r = (int)(t / S);
-    int64_t si = transposed ? (((int64_t)ci * Cout + co) * R + r) * S + s
-                            : (((int64_t)co * Cin + ci) * R + r) * S + s;
-    float v = src[si];
-    dst[i] = rtf ? round_tf32(v) : v;
-  }
-}
-
 // 3x3 s1 p1 conv behind a nearest x2 upsample == four 2x2 "phase" filters on the low-res input:
 // out[2i+a][2j+b] = sum_{dr,ds in {0,1}} x[i+a-1+dr][j+b-1+ds] * Wf[a][b][dr][ds]
 // Wf[a][b][dr][ds] = sum_{r in Rset(a,dr)} sum_{s in Rset(b,ds)} W[r][s],
@@ -139,30 +112,11 @@ __device__ __forceinline__ void up2_rset(int a, int d, int &lo, int &hi) {
   if (a == 0) { lo = d == 0 ? 0 : 1; hi = d == 0 ? 0 : 2; }
   else        { lo = d == 0 ? 0 : 2; hi = d == 0 ? 1 : 2; }
 }
-__global__ void pack_up2_kernel(const float *__restrict__ src, float *__restrict__ dst, int Cin, int Cout,
-                                int order) {
-  int64_t total = (int64_t)16 * Cin * Cout;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total;
-       i += (int64_t)gridDim.x * blockDim.x) {
-    int ci, co;
-    int64_t t;
-    if (order == 0) { co = (int)(i % Cout); t = i / Cout; ci = (int)(t % Cin); t /= Cin; }
-    else            { ci = (int)(i % Cin);  t = i / Cin;  co = (int)(t % Cout); t /= Cout; }
-    int tap = (int)(t % 4), ph = (int)(t / 4);
-    int a = ph >> 1, b = ph & 1, dr = tap >> 1, ds = tap & 1;
-    int rlo, rhi, slo, shi;
-    up2_rset(a, dr, rlo, rhi);
-    up2_rset(b, ds, slo, shi);
-    float v = 0.f;
-    for (int r = rlo; r <= rhi; ++r)
-      for (int s = slo; s <= shi; ++s) v += src[(((int64_t)co * Cin + ci) * 3 + r) * 3 + s];
-    dst[i] = round_tf32(v);
-  }
-}
 
 // ---- every packed copy of an optimizer's weights in ONE launch ---------------------------------------------------
 // The weights change once per optimizer step, and every conv keeps 1-2 packed copies (fprop / dgrad layouts): per-copy
-// pack launches were 21 of the DCGAN step's launches.  The job table travels as a kernel argument.
+// pack launches were 21 of the DCGAN step's launches.  The job table travels as a kernel argument; a single copy
+// (b200gan_pack_weights) is a table of one job.
 constexpr int PACK_MAX_JOBS = 24;
 constexpr int PACK_CHUNK = 256 * 8;  // packed elements per block
 struct PackJob {
@@ -290,43 +244,52 @@ __global__ void __launch_bounds__(256) pack_multi_kernel(const __grid_constant__
 
 using namespace b200gan;
 
+// Validate one packing job and append it to the table (tb.count < PACK_MAX_JOBS; tb.block_begin[tb.count] holds the
+// blocks of the jobs before it).
+static int pack_table_add(PackTable &tb, const b200gan_conv_geom *g, int pack, const float *w, float *packed) {
+  if (int e = validate_geom(g)) return e;
+  B2_CHECK_ARG(w && packed, "pack_weights: null pointer");
+  B2_CHECK_ARG(pack >= B200GAN_PACK_SIMT_FPROP && pack <= B200GAN_PACK_TC_DGRAD_UP2, "pack_weights: unknown pack id %d", pack);
+  if (pack == B200GAN_PACK_TC_FPROP_UP2 || pack == B200GAN_PACK_TC_DGRAD_UP2)
+    B2_CHECK_ARG(!g->transposed && g->up == 2 && g->R == 3 && g->S == 3 && g->stride == 1 && g->pad_t == 1 &&
+                     g->pad_l == 1 && g->pad_b == 1 && g->pad_r == 1 && g->pad_mode == B200GAN_PAD_ZERO,
+                 "pack_weights: UP2 fold needs a 3x3 s1 p1 zero-padded conv behind a x2 upsample");
+  PackJob &j = tb.job[tb.count];
+  j.src = w; j.dst = packed;
+  j.R = g->R; j.S = g->S; j.Cin = g->C; j.Cout = g->K; j.transposed = g->transposed;
+  j.kind = pack;
+  j.total = (long long)b200gan_packed_weight_floats(g, pack);
+  int blocks = tb.block_begin[tb.count];
+  j.tiles_ci = 0;
+  if (j.R * j.S <= PACK_RS_MAX && j.Cin >= PACK_CI_T && j.Cout >= PACK_CO_T) {
+    j.tiles_ci = ceil_div(j.Cin, PACK_CI_T);
+    blocks += j.tiles_ci * ceil_div(j.Cout, PACK_CO_T);
+  } else {
+    blocks += (int)ceil_div64(j.total, PACK_CHUNK);
+  }
+  tb.block_begin[++tb.count] = blocks;
+  return B200GAN_OK;
+}
+
+static int pack_table_launch(const PackTable &tb, cudaStream_t st) {
+  const int blocks = tb.block_begin[tb.count];
+  if (blocks > 0) {
+    pack_multi_kernel<<<(unsigned)blocks, 256, 0, st>>>(tb);
+    B2_LAUNCH_CHECK();
+  }
+  return B200GAN_OK;
+}
+
 extern "C" int b200gan_pack_weights_multi(const b200gan_pack_job *jobs, int32_t count, void *stream) {
   B2_CHECK_ARG(count >= 0 && (count == 0 || jobs != nullptr), "pack_weights_multi: bad arguments");
   cudaStream_t st = as_stream(stream);
   for (int base = 0; base < count; base += PACK_MAX_JOBS) {
     PackTable tb;
-    const int c = count - base < PACK_MAX_JOBS ? count - base : PACK_MAX_JOBS;
-    int blocks = 0;
-    for (int i = 0; i < c; ++i) {
-      const b200gan_pack_job &jb = jobs[base + i];
-      if (int e = validate_geom(&jb.geom)) return e;
-      B2_CHECK_ARG(jb.w && jb.packed, "pack_weights_multi: job %d has a null pointer", base + i);
-      B2_CHECK_ARG(jb.pack >= B200GAN_PACK_SIMT_FPROP && jb.pack <= B200GAN_PACK_TC_DGRAD_UP2, "pack_weights_multi: pack id");
-      const bool up2 = jb.pack == B200GAN_PACK_TC_FPROP_UP2 || jb.pack == B200GAN_PACK_TC_DGRAD_UP2;
-      if (up2)
-        B2_CHECK_ARG(!jb.geom.transposed && jb.geom.up == 2 && jb.geom.R == 3 && jb.geom.S == 3,
-                     "pack_weights_multi: UP2 fold needs a 3x3 conv behind a x2 upsample");
-      PackJob &j = tb.job[i];
-      j.src = jb.w; j.dst = jb.packed;
-      j.R = jb.geom.R; j.S = jb.geom.S; j.Cin = jb.geom.C; j.Cout = jb.geom.K; j.transposed = jb.geom.transposed;
-      j.kind = jb.pack;
-      j.total = (long long)b200gan_packed_weight_floats(&jb.geom, jb.pack);
-      tb.block_begin[i] = blocks;
-      static const bool tile_mode = !(getenv("B200GAN_PACK_TILED") && atoi(getenv("B200GAN_PACK_TILED")) == 0);
-      j.tiles_ci = 0;
-      if (tile_mode && j.R * j.S <= PACK_RS_MAX && j.Cin >= PACK_CI_T && j.Cout >= PACK_CO_T) {
-        j.tiles_ci = ceil_div(j.Cin, PACK_CI_T);
-        blocks += j.tiles_ci * ceil_div(j.Cout, PACK_CO_T);
-      } else {
-        blocks += (int)ceil_div64(j.total, PACK_CHUNK);
-      }
-    }
-    tb.block_begin[c] = blocks;
-    tb.count = c;
-    if (blocks > 0) {
-      pack_multi_kernel<<<(unsigned)blocks, 256, 0, st>>>(tb);
-      B2_LAUNCH_CHECK();
-    }
+    tb.count = 0;
+    tb.block_begin[0] = 0;
+    for (int i = base; i < count && tb.count < PACK_MAX_JOBS; ++i)
+      if (int e = pack_table_add(tb, &jobs[i].geom, jobs[i].pack, jobs[i].w, jobs[i].packed)) return e;
+    if (int e = pack_table_launch(tb, st)) return e;
   }
   return B200GAN_OK;
 }
@@ -356,36 +319,11 @@ extern "C" size_t b200gan_packed_weight_floats(const b200gan_conv_geom *g, int p
 
 extern "C" int b200gan_pack_weights(const b200gan_conv_geom *g, int pack, const float *w, float *packed,
                                     void *stream) {
-  if (int e = validate_geom(g)) return e;
-  B2_CHECK_ARG(w && packed, "pack_weights: null pointer");
-  cudaStream_t st = as_stream(stream);
-  int64_t total = (int64_t)b200gan_packed_weight_floats(g, pack);
-  unsigned blocks = (unsigned)(ceil_div64(total, 256) > 1184 ? 1184 : ceil_div64(total, 256));
-  switch (pack) {
-    case B200GAN_PACK_SIMT_FPROP:
-      pack_kernel<<<blocks, 256, 0, st>>>(w, packed, g->R, g->S, g->C, g->K, g->transposed, 0, 0);
-      break;
-    case B200GAN_PACK_SIMT_DGRAD:
-      pack_kernel<<<blocks, 256, 0, st>>>(w, packed, g->R, g->S, g->C, g->K, g->transposed, 1, 0);
-      break;
-    case B200GAN_PACK_TC_FPROP:
-      pack_kernel<<<blocks, 256, 0, st>>>(w, packed, g->R, g->S, g->C, g->K, g->transposed, 1, 1);
-      break;
-    case B200GAN_PACK_TC_DGRAD:
-      pack_kernel<<<blocks, 256, 0, st>>>(w, packed, g->R, g->S, g->C, g->K, g->transposed, 0, 1);
-      break;
-    case B200GAN_PACK_TC_FPROP_UP2:
-    case B200GAN_PACK_TC_DGRAD_UP2:
-      B2_CHECK_ARG(!g->transposed && g->up == 2 && g->R == 3 && g->S == 3 && g->stride == 1 && g->pad_t == 1 &&
-                       g->pad_l == 1 && g->pad_b == 1 && g->pad_r == 1 && g->pad_mode == B200GAN_PAD_ZERO,
-                   "pack_weights: UP2 fold needs a 3x3 s1 p1 zero-padded conv behind a x2 upsample");
-      pack_up2_kernel<<<blocks, 256, 0, st>>>(w, packed, g->C, g->K, pack == B200GAN_PACK_TC_FPROP_UP2 ? 1 : 0);
-      break;
-    default:
-      B2_CHECK_ARG(false, "pack_weights: unknown pack id %d", pack);
-  }
-  B2_LAUNCH_CHECK();
-  return B200GAN_OK;
+  PackTable tb;
+  tb.count = 0;
+  tb.block_begin[0] = 0;
+  if (int e = pack_table_add(tb, g, pack, w, packed)) return e;
+  return pack_table_launch(tb, as_stream(stream));
 }
 
 extern "C" int b200gan_conv2d_supported(const b200gan_conv_geom *g, int pass, int algo) {

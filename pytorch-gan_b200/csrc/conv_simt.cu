@@ -13,17 +13,6 @@
 
 namespace b200gan {
 
-// conv_narrow.cu: experimental one-thread-per-pixel kernels for the <= 64-channel layers, taken only with B200GAN_NARROW=1
-bool narrow_enabled();
-bool narrow_gather_ok(int C, int K, int R, int S, int stride, int pad_mode, int up, const void *x, const void *wp,
-                      const void *y);
-int narrow_gather(int N, int H, int W, int C, int P, int Q, int K, int R, int S, int stride, int pad_t, int pad_l, int mode,
-                  const b200gan_epilogue *ep, const float *x, const float *wp, float *y, cudaStream_t st);
-bool narrow_wgrad_ok(int64_t gathered_floats, int Cg, int Cd, int R, int S, int pad_mode, int up, const void *xg,
-                     const void *dn);
-int narrow_wgrad(int N, int H, int W, int Cg, int P, int Q, int Cd, int R, int S, int stride, int pad_t, int pad_l,
-                 const float *xg, const float *dn, float *dw, cudaStream_t st);
-
 struct GatherP {
   int N, H, W, C;      // stored (gathered) tensor dims, NHWC
   int P, Q;            // output pixel grid
@@ -794,8 +783,6 @@ int simt_gather_gemm(int N, int H, int W, int C, int P, int Q, int K, int R, int
   e.round_tf32 = ep ? ep->round_tf32 : 0;
   int64_t M = (int64_t)N * P * Q;
   if (M == 0 || K == 0) return B200GAN_OK;
-  if (narrow_enabled() && narrow_gather_ok(C, K, R, S, stride, pad_mode, up, x, wp, y))
-    return narrow_gather(N, H, W, C, P, Q, K, R, S, stride, pad_t, pad_l, mode, ep, x, wp, y, st);
   int Ktot = R * S * C;
   size_t wbytes = (size_t)Ktot * K * sizeof(float);
   const bool aligned = ((uintptr_t)x % 16 == 0) && ((uintptr_t)y % 16 == 0);
@@ -879,8 +866,6 @@ int simt_wgrad(int N, int H, int W, int Cg, int P, int Q, int Cd, int R, int S, 
   int Ktot = R * S * Cg;
   B2_CUDA(cudaMemsetAsync(dw, 0, (size_t)Ktot * Cd * sizeof(float), st));
   if (M == 0) return B200GAN_OK;
-  if (narrow_enabled() && narrow_wgrad_ok((int64_t)N * H * W * Cg, Cg, Cd, R, S, pad_mode, up, xg, dn))
-    return narrow_wgrad(N, H, W, Cg, P, Q, Cd, R, S, stride, pad_t, pad_l, xg, dn, dw, st);
   if (Cd == 1 && R == 3 && S == 3 && stride == 1 && pad_t == 1 && pad_l == 1 && up == 1 && pad_mode == B200GAN_PAD_ZERO &&
       P == H && Q == W && Cg % 4 == 0 && Cg >= 16 && Cg <= 128 && ((uintptr_t)xg % 16 == 0)) {
     const int L = Cg >= 128 ? 32 : (Cg >= 64 ? 16 : (Cg >= 32 ? 8 : 4));

@@ -734,9 +734,8 @@ static int run_tc(const float *in, int N, int Hi, int Wi, int Cc, bool phase_in,
   {
     // 256-wide tiles (A 16 KB + B 32 KB per stage feed 2 x 4 x M64 N256 K8: the 128-channel A box is fetched half as
     // often per output channel) when the layer still gives every SM a CTA
-    static const bool bn256 = !(getenv("B200GAN_TC_BN256") && atoi(getenv("B200GAN_TC_BN256")) == 0);
     const int64_t tiles = (int64_t)p.tiles_w * p.tiles_h * ceil_div(N, BNn) * nphase;
-    if (bn256 && Kout % 256 == 0 && tiles * (Kout / 256) >= num_sms()) BN = 256;
+    if (Kout % 256 == 0 && tiles * (Kout / 256) >= num_sms()) BN = 256;
   }
   p.N = N;
   p.Ho = Ho;
@@ -770,7 +769,6 @@ static int run_tc(const float *in, int N, int Hi, int Wi, int Cc, bool phase_in,
   }
   {
     // few output tiles (deep U-Net layers at 1x1 .. 16x16 pixels): split the contraction so that the machine is used
-    static const bool allow = !(getenv("B200GAN_TC_KSPLIT") && atoi(getenv("B200GAN_TC_KSPLIT")) == 0);
     const bool plain = !p.bias && !p.chan_scale && p.act == B200GAN_ACT_NONE && !p.rtf;
     const int64_t ctas = (int64_t)p.tiles_w * p.tiles_h * ceil_div(N, BNn) * (Kout / BN) * nphase;
     int min_iters = 1 << 30;
@@ -778,7 +776,7 @@ static int run_tc(const float *in, int N, int Hi, int Wi, int Cc, bool phase_in,
       const int it = (tap_begin[z + 1] - tap_begin[z]) * p.kchunks;
       if (it < min_iters) min_iters = it;
     }
-    if (allow && plain && !narrow_k && ctas < num_sms() && min_iters >= 16) {
+    if (plain && !narrow_k && ctas < num_sms() && min_iters >= 16) {
       int ks = (int)((2 * num_sms() + ctas - 1) / ctas);
       if (ks > min_iters / 8) ks = min_iters / 8;
       if (ks > 32) ks = 32;
@@ -1009,8 +1007,7 @@ int tc_fprop(const b200gan_conv_geom *g, const b200gan_epilogue *ep, const float
   const b200gan_epilogue *e = ep ? &e2 : nullptr;
   if (g->up == 2) {
     // 64-wide output tiles: all four phases in one CTA (9 operand fetches per k-chunk instead of 16)
-    static const bool allphase = !(getenv("B200GAN_UP2_ALLPHASE") && atoi(getenv("B200GAN_UP2_ALLPHASE")) == 0);
-    if (allphase && g->K % 128 != 0 && g->K % 64 == 0)
+    if (g->K % 128 != 0 && g->K % 64 == 0)
       return run_up2_allphase(x, g->N, g->H, g->W, g->C, packed, g->K, e, y, st);
     // phase (a,b): out[2i+a][2j+b] = sum_{dr,ds} x[i+a-1+dr][j+b-1+ds] * Wf[a][b][dr][ds]
     TcTap taps[TC_MAX_TAPS];

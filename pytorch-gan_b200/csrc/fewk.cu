@@ -12,10 +12,11 @@
 // load), a lane group register-tiles 8 pixels of a row, and the weights come from shared memory as one LDS.128 per 32
 // FMAs:
 //   fewk_fprop  dot products over channels finished with a butterfly across the lanes of a group
-//   fewk_dgrad  dx[h, w, 4c] accumulated from a register window of dz (uniform loads); the nearest-neighbour
-//               upsample's backward (sum over the 2x2 children) is part of the same accumulation
+//   fewk_dgrad  dx[h, w, 4c] accumulated from a register window of dz (uniform loads)
 //   fewk_wgrad  a warp owns one filter row and streams output rows; per-block slabs + the fixed-order reduce kernel
-// The folded nearest-neighbour upsample (g->up == 2) only changes the address computation (source pixel = index >> 1).
+// A nearest-neighbour x2 upsample in front of a zero-padded 3x3 / 4x4 conv runs on folded filters (the *_up2 kernels
+// below; the data gradient's upsample backward is part of their accumulation).  Elsewhere (forward and weight gradient
+// with reflection padding or 7x7) the upsample only changes the address computation (source pixel = index >> 1).
 #include "tc_common.cuh"
 #include <string.h>
 
@@ -132,8 +133,9 @@ fewk_fprop_kernel(const __grid_constant__ FewkP p) {
 }
 
 // ---- data gradient --------------------------------------------------------------------------------------------------
-// thread group = 8 source pixels of a row x 4 channels per lane; zero padding only.  dynamic smem: w [R*S][K][C]
-template <int S, int K, int UP>
+// thread group = 8 pixels of a row x 4 channels per lane; zero padding, no upsample (fewk_dgrad_up2_kernel folds it).
+// dynamic smem: w [R*S][K][C]
+template <int S, int K>
 __global__ void __launch_bounds__(256)
 fewk_dgrad_kernel(const __grid_constant__ FewkP p) {
   extern __shared__ __align__(16) float w_s[];
@@ -145,7 +147,7 @@ fewk_dgrad_kernel(const __grid_constant__ FewkP p) {
   const int tiles_w = fk_cdiv(p.W, p.G * FK_PX), tiles_h = fk_cdiv(p.H, 8);
   const int ntiles = p.N * tiles_h * tiles_w;
   const int chunk = p.CL * 4;
-  constexpr int WIN = FK_PX * UP + S - 1;   // dz columns a row of 8 source pixels touches
+  constexpr int WIN = FK_PX + S - 1;   // dz columns a row of 8 pixels touches
   for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
     const int tw = tile % tiles_w, th = (tile / tiles_w) % tiles_h, n = tile / (tiles_w * tiles_h);
     const int h = th * 8 + warp, w0 = (tw * p.G + grp) * FK_PX;
@@ -154,11 +156,10 @@ fewk_dgrad_kernel(const __grid_constant__ FewkP p) {
       float4 acc[FK_PX];
 #pragma unroll
       for (int px = 0; px < FK_PX; ++px) acc[px] = make_float4(0.f, 0.f, 0.f, 0.f);
-      const int qstart = w0 * UP + p.pad_l - (S - 1);
+      const int qstart = w0 + p.pad_l - (S - 1);
 #pragma unroll 1
-      for (int ar = 0; ar < UP * p.R; ++ar) {
-        const int a = ar / p.R, r = ar % p.R;
-        const int prow = h * UP + a + p.pad_t - r;   // output row whose tap r reads virtual row h * UP + a
+      for (int r = 0; r < p.R; ++r) {
+        const int prow = h + p.pad_t - r;   // output row whose tap r reads row h
         if (prow < 0 || prow >= p.P) continue;
         const float *drow = p.dy + ((int64_t)(n * p.P + prow) * p.Q) * K;
         float dzw[WIN][K];
@@ -175,9 +176,7 @@ fewk_dgrad_kernel(const __grid_constant__ FewkP p) {
           for (int k = 0; k < K; ++k) {
             const float4 w4 = *reinterpret_cast<const float4 *>(w_s + ((r * S + s) * K + k) * p.C + cb + cl * 4);
 #pragma unroll
-            for (int px = 0; px < FK_PX; ++px)
-#pragma unroll
-              for (int b = 0; b < UP; ++b) axpy4(acc[px], dzw[px * UP + b + (S - 1) - s][k], w4);
+            for (int px = 0; px < FK_PX; ++px) axpy4(acc[px], dzw[px + (S - 1) - s][k], w4);
           }
         }
       }
@@ -551,14 +550,9 @@ static bool fewk_geom_ok(const b200gan_conv_geom *g) {
   if ((size_t)g->R * g->S * g->K * g->C * sizeof(float) > 160 * 1024) return false;
   return true;
 }
-static bool fewk_enabled() {
-  static const bool on = !(getenv("B200GAN_FEWK") && atoi(getenv("B200GAN_FEWK")) == 0);
-  return on;
-}
-
 // pas: 0 fprop, 1 dgrad, 2 wgrad
 bool fewk_ok(const b200gan_conv_geom *g, int pas) {
-  if (!fewk_enabled() || !fewk_geom_ok(g)) return false;
+  if (!fewk_geom_ok(g)) return false;
   if (pas == 1 && g->pad_mode != B200GAN_PAD_ZERO) return false;   // the mirrored border folds back in pad2d_bwd
   if (pas == 1 && g->S == 7 && g->up == 2) return false;
   return true;
@@ -576,8 +570,7 @@ static void fewk_fill(FewkP &p, const b200gan_conv_geom *g) {
 
 
 static bool fewk_fold_on(const b200gan_conv_geom *g) {
-  static const bool on = !(getenv("B200GAN_FEWK_FOLD") && atoi(getenv("B200GAN_FEWK_FOLD")) == 0);
-  return on && g->up == 2 && g->pad_mode == B200GAN_PAD_ZERO && (g->S == 3 || g->S == 4);
+  return g->up == 2 && g->pad_mode == B200GAN_PAD_ZERO && (g->S == 3 || g->S == 4);
 }
 template <int S> static size_t fewk_fold_smem(const b200gan_conv_geom *g) {
   return (size_t)Fold<S>::NFT * Fold<S>::NFT * g->K * g->C * sizeof(float);
@@ -655,18 +648,18 @@ int fewk_fprop(const b200gan_conv_geom *g, const b200gan_epilogue *ep, const flo
   return fewk_fprop_launch<7>(p, g->K, grid, smem, st);
 }
 
-template <int S, int UP>
+template <int S>
 static int fewk_dgrad_launch(const FewkP &p, int K, int grid, size_t smem, cudaStream_t st) {
   static std::atomic<uint64_t> d1{0}, d2{0}, d3{0}, d4{0};
   switch (K) {
-    case 1: if (int e = ensure_dynamic_smem(fewk_dgrad_kernel<S, 1, UP>, 160 * 1024, d1)) return e;
-            fewk_dgrad_kernel<S, 1, UP><<<grid, 256, smem, st>>>(p); break;
-    case 2: if (int e = ensure_dynamic_smem(fewk_dgrad_kernel<S, 2, UP>, 160 * 1024, d2)) return e;
-            fewk_dgrad_kernel<S, 2, UP><<<grid, 256, smem, st>>>(p); break;
-    case 3: if (int e = ensure_dynamic_smem(fewk_dgrad_kernel<S, 3, UP>, 160 * 1024, d3)) return e;
-            fewk_dgrad_kernel<S, 3, UP><<<grid, 256, smem, st>>>(p); break;
-    default: if (int e = ensure_dynamic_smem(fewk_dgrad_kernel<S, 4, UP>, 160 * 1024, d4)) return e;
-            fewk_dgrad_kernel<S, 4, UP><<<grid, 256, smem, st>>>(p); break;
+    case 1: if (int e = ensure_dynamic_smem(fewk_dgrad_kernel<S, 1>, 160 * 1024, d1)) return e;
+            fewk_dgrad_kernel<S, 1><<<grid, 256, smem, st>>>(p); break;
+    case 2: if (int e = ensure_dynamic_smem(fewk_dgrad_kernel<S, 2>, 160 * 1024, d2)) return e;
+            fewk_dgrad_kernel<S, 2><<<grid, 256, smem, st>>>(p); break;
+    case 3: if (int e = ensure_dynamic_smem(fewk_dgrad_kernel<S, 3>, 160 * 1024, d3)) return e;
+            fewk_dgrad_kernel<S, 3><<<grid, 256, smem, st>>>(p); break;
+    default: if (int e = ensure_dynamic_smem(fewk_dgrad_kernel<S, 4>, 160 * 1024, d4)) return e;
+            fewk_dgrad_kernel<S, 4><<<grid, 256, smem, st>>>(p); break;
   }
   B2_LAUNCH_CHECK();
   return B200GAN_OK;
@@ -686,13 +679,9 @@ int fewk_dgrad(const b200gan_conv_geom *g, const float *dy, const float *packed,
     if (g->S == 3) return fewk_dgrad_up2_launch<3>(p, g->K, grid, fewk_fold_smem<3>(g), st);
     return fewk_dgrad_up2_launch<4>(p, g->K, grid, fewk_fold_smem<4>(g), st);
   }
-  if (g->up == 2) {
-    if (g->S == 3) return fewk_dgrad_launch<3, 2>(p, g->K, grid, smem, st);
-    return fewk_dgrad_launch<4, 2>(p, g->K, grid, smem, st);
-  }
-  if (g->S == 3) return fewk_dgrad_launch<3, 1>(p, g->K, grid, smem, st);
-  if (g->S == 4) return fewk_dgrad_launch<4, 1>(p, g->K, grid, smem, st);
-  return fewk_dgrad_launch<7, 1>(p, g->K, grid, smem, st);
+  if (g->S == 3) return fewk_dgrad_launch<3>(p, g->K, grid, smem, st);
+  if (g->S == 4) return fewk_dgrad_launch<4>(p, g->K, grid, smem, st);
+  return fewk_dgrad_launch<7>(p, g->K, grid, smem, st);
 }
 
 static int fk_wg_blocks() { return num_sms() * 2; }

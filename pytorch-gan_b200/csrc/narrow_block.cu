@@ -8,7 +8,7 @@
 // gradient, BatchNorm statistics / finalize / apply / backward reduce / backward apply / parameter gradients, ...).
 // Here a layer l keeps only a_l = dropout(lrelu(conv_l(x_l) + b_l)) and the batch sums of a_l in memory; the normalised
 // tensor x_{l+1} = BN_l(a_l) is never written:
-//   nbk_fprop   x_l = a_{l-1} * scale + shift applied while gathering (BatchNorm "apply" of the producer folded into the
+//   nbk_fprop2  x_l = a_{l-1} * scale + shift applied while gathering (BatchNorm "apply" of the producer folded into the
 //               consumer's loads; zero padding stays zero), bias + LeakyReLU + Dropout2d scale in registers, the sums
 //               / sums of squares the NEXT BatchNorm needs reduced in the epilogue (warp shuffles -> one fp64 atomic per
 //               channel and block).  The BatchNorm finalisation (mean, rstd, running statistics) happens in the prologue
@@ -17,7 +17,7 @@
 //               dgrad accumulated, + the bias gradient.
 //   nbk_wgrad   dW_l from dz_l and x_l (recomputed from a_{l-1} while staging the patch in shared memory); thread =
 //               (input channel, 4 output channels) x all taps in registers, pixels streamed through shared memory.
-//   nbk_dgrad   G_l = transposed gather of dz_l by stride-parity class + the sums BN_{l-1}'s backward needs, in the epilogue.
+//   nbk_dgrad2  G_l = transposed gather of dz_l by stride-parity class + the sums BN_{l-1}'s backward needs, in the epilogue.
 //   nbk_tail_*  BN_4 apply fused with the NHWC -> NCHW layout change the script's .view needs (dcgan.py:96), and back.
 // G_l is the gradient w.r.t. the VIRTUAL tensor x_l; the BatchNorm backward is finished by the consumer (nbk_dz of layer
 // l-1) once the sums are complete.  See b200gan/functional.py (NbConvFn, NbTailFn) for the autograd wiring.
@@ -86,135 +86,7 @@ __device__ __forceinline__ float warp_sum(float v) {
 constexpr int NB_MAXC = 128;
 constexpr int NB_MAX_GROUPS = 4;   // statistics groups per batch (NbBn::groups)
 
-// ---- forward ------------------------------------------------------------------------------------------------------
-struct NbFprop {
-  const float *x, *wp, *bias, *cs;
-  float *y;
-  double *out_stats;
-  NbBn in_bn;
-  float *rm, *rv;
-  long long *nbt;
-  float momentum;
-  int N, H, W, C, P, Q, K, R, S, stride, pad_t, pad_l;
-  float slope;
-  int act;
-  int Mpad;  // output pixels rounded up to a multiple of the block size: every block has ONE channel group
-};
-
-// thread = (channel group kg, output pixel m); kg is uniform per block, lanes are consecutive pixels
-template <int KT>
-__global__ void __launch_bounds__(256)
-nbk_fprop_kernel(const __grid_constant__ NbFprop p) {
-  __shared__ float sc_s[NB_MAXC], sh_s[NB_MAXC];
-  __shared__ float red[8][2 * KT];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const bool has_in = p.in_bn.stats != nullptr;
-  if (has_in && tid < p.C) {
-    float mean, rstd, sc, sh;
-    nb_bn_consts(p.in_bn, p.C, tid, mean, rstd, sc, sh);
-    sc_s[tid] = sc;
-    sh_s[tid] = sh;
-    if (blockIdx.x == 0 && p.rm) nb_update_running(p.in_bn, p.C, tid, p.rm, p.rv, p.momentum);
-  }
-  if (has_in && blockIdx.x == 0 && tid == 0 && p.nbt) *p.nbt += 1;
-  __syncthreads();
-
-  const int64_t M = (int64_t)p.N * p.P * p.Q;
-  const int64_t t = (int64_t)blockIdx.x * 256 + tid;
-  const int kg = (int)(t / p.Mpad);
-  const int64_t m = t % p.Mpad;
-  const bool valid = m < M;
-  const int k0 = kg * KT;
-  float acc[KT];
-#pragma unroll
-  for (int j = 0; j < KT; ++j) acc[j] = 0.f;
-  int n = 0, po = 0, qo = 0;
-  if (valid) {
-    qo = (int)(m % p.Q);
-    const int64_t t2 = m / p.Q;
-    po = (int)(t2 % p.P);
-    n = (int)(t2 / p.P);
-    for (int r = 0; r < p.R; ++r) {
-      const int ih = po * p.stride - p.pad_t + r;
-      if (ih < 0 || ih >= p.H) continue;
-      for (int s = 0; s < p.S; ++s) {
-        const int iw = qo * p.stride - p.pad_l + s;
-        if (iw < 0 || iw >= p.W) continue;
-        const float *xp = p.x + ((int64_t)(n * p.H + ih) * p.W + iw) * p.C;
-        const float *wt = p.wp + (int64_t)(r * p.S + s) * p.C * p.K + k0;
-        if ((p.C & 3) == 0) {
-          for (int c = 0; c < p.C; c += 4) {
-            const float4 xv = __ldg(reinterpret_cast<const float4 *>(xp + c));
-            float xs[4] = {xv.x, xv.y, xv.z, xv.w};
-            if (has_in) {
-#pragma unroll
-              for (int j = 0; j < 4; ++j) xs[j] = fmaf(xs[j], sc_s[c + j], sh_s[c + j]);
-            }
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const float *wr = wt + (int64_t)(c + j) * p.K;
-#pragma unroll
-              for (int u = 0; u < KT / 4; ++u) {
-                const float4 w4 = __ldg(reinterpret_cast<const float4 *>(wr + 4 * u));
-                acc[4 * u + 0] = fmaf(xs[j], w4.x, acc[4 * u + 0]);
-                acc[4 * u + 1] = fmaf(xs[j], w4.y, acc[4 * u + 1]);
-                acc[4 * u + 2] = fmaf(xs[j], w4.z, acc[4 * u + 2]);
-                acc[4 * u + 3] = fmaf(xs[j], w4.w, acc[4 * u + 3]);
-              }
-            }
-          }
-        } else {
-          for (int c = 0; c < p.C; ++c) {
-            float xs = __ldg(xp + c);
-            if (has_in) xs = fmaf(xs, sc_s[c], sh_s[c]);
-            const float *wr = wt + (int64_t)c * p.K;
-#pragma unroll
-            for (int u = 0; u < KT / 4; ++u) {
-              const float4 w4 = __ldg(reinterpret_cast<const float4 *>(wr + 4 * u));
-              acc[4 * u + 0] = fmaf(xs, w4.x, acc[4 * u + 0]);
-              acc[4 * u + 1] = fmaf(xs, w4.y, acc[4 * u + 1]);
-              acc[4 * u + 2] = fmaf(xs, w4.z, acc[4 * u + 2]);
-              acc[4 * u + 3] = fmaf(xs, w4.w, acc[4 * u + 3]);
-            }
-          }
-        }
-      }
-    }
-#pragma unroll
-    for (int j = 0; j < KT; ++j) {
-      float v = acc[j];
-      if (p.bias) v += __ldg(p.bias + k0 + j);
-      v = nb_act(v, p.act, p.slope);
-      if (p.cs) v *= __ldg(p.cs + (int64_t)n * p.K + k0 + j);
-      acc[j] = v;
-    }
-    float *yo = p.y + m * p.K + k0;
-#pragma unroll
-    for (int u = 0; u < KT / 4; ++u)
-      *reinterpret_cast<float4 *>(yo + 4 * u) = make_float4(acc[4 * u], acc[4 * u + 1], acc[4 * u + 2], acc[4 * u + 3]);
-  }
-  if (p.out_stats) {
-#pragma unroll
-    for (int j = 0; j < KT; ++j) {
-      const float v = valid ? acc[j] : 0.f;
-      const float s1 = warp_sum(v), s2 = warp_sum(v * v);
-      if (lane == 0) {
-        red[warp][j] = s1;
-        red[warp][KT + j] = s2;
-      }
-    }
-    __syncthreads();
-    if (tid < 2 * KT) {
-      float tsum = 0.f;
-#pragma unroll
-      for (int wi = 0; wi < 8; ++wi) tsum += red[wi][tid];
-      const int j = tid % KT;
-      atomicAdd(p.out_stats + (tid < KT ? 0 : p.K) + k0 + j, (double)tsum);
-    }
-  }
-}
-
-// ---- shared-memory staged kernels (v2) ----------------------------------------------------------------------------------
+// ---- forward: shared-memory staged kernels -------------------------------------------------------------------------
 // Copy a [rows][cols][C] window of an NHWC image into shared memory with channel pitch CP, applying v * sc + sh to
 // elements inside the image; positions outside are 0 (zero padding comes after the normalisation) or mirrored.
 // src_img == nullptr (tile hangs over the batch): all zeros.  Consecutive threads read consecutive channels: coalesced.
@@ -707,122 +579,6 @@ nbk_wgrad_reduce_kernel(const float *__restrict__ ws, float *__restrict__ dw, in
 }
 
 // ---- data gradient + the sums of the upstream BatchNorm's backward ----------------------------------------------------------
-struct NbDgrad {
-  const float *dz, *wp, *a_prev;
-  float *g_out;
-  double *sums;  // [2][C] (null: no BatchNorm in front of this layer)
-  NbBn in_bn;
-  int N, H, W, C, P, Q, K, R, S, stride, pad_t, pad_l;
-  int Mpad;      // pixels of the largest parity class rounded up to the block size
-};
-// G[n][h][w][c] = sum_{r,s,k} dz[n][(h + pad - r)/stride][(w + pad - s)/stride][k] * w[r][s][k][c] where the division is
-// exact.  blockIdx.z = stride-parity class of (h, w): all pixels of a class use the same taps.  wp: [tap][K][C].
-template <int KT>
-__global__ void __launch_bounds__(256)
-nbk_dgrad_kernel(const __grid_constant__ NbDgrad p) {
-  __shared__ float mean_s[NB_MAXC], rstd_s[NB_MAXC];
-  __shared__ float red[8][2 * KT];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const bool has_in = p.sums != nullptr;
-  if (has_in && tid < p.C) {
-    float sc, sh;
-    nb_bn_consts(p.in_bn, p.C, tid, mean_s[tid], rstd_s[tid], sc, sh);
-  }
-  __syncthreads();
-  const int st = p.stride;
-  const int cls = blockIdx.z;
-  const int pa = cls / st, pb = cls % st;               // first row / column of the class
-  const int r0 = (pa + p.pad_t) % st, s0 = (pb + p.pad_l) % st;
-  const int Rc = r0 < p.R ? (p.R - r0 + st - 1) / st : 0, Sc = s0 < p.S ? (p.S - s0 + st - 1) / st : 0;
-  const int Hc = pa < p.H ? (p.H - pa + st - 1) / st : 0, Wc = pb < p.W ? (p.W - pb + st - 1) / st : 0;
-  const int64_t Mc = (int64_t)p.N * Hc * Wc;
-  const int64_t t = (int64_t)blockIdx.x * 256 + tid;
-  const int cg = (int)(t / p.Mpad);
-  const int64_t m = t % p.Mpad;
-  const bool valid = m < Mc;
-  const int c0 = cg * KT;
-  float acc[KT];
-#pragma unroll
-  for (int j = 0; j < KT; ++j) acc[j] = 0.f;
-  int64_t opix = 0;
-  if (valid) {
-    const int w = pb + st * (int)(m % Wc);
-    const int64_t t2 = m / Wc;
-    const int h = pa + st * (int)(t2 % Hc);
-    const int n = (int)(t2 / Hc);
-    opix = (int64_t)(n * p.H + h) * p.W + w;
-    for (int ir = 0; ir < Rc; ++ir) {
-      const int r = r0 + st * ir;
-      const int th = h + p.pad_t - r;
-      if (th < 0) continue;
-      const int ph = th / st;
-      if (ph >= p.P) continue;
-      for (int is = 0; is < Sc; ++is) {
-        const int s = s0 + st * is;
-        const int tw = w + p.pad_l - s;
-        if (tw < 0) continue;
-        const int pw = tw / st;
-        if (pw >= p.Q) continue;
-        const float *dp = p.dz + ((int64_t)(n * p.P + ph) * p.Q + pw) * p.K;
-        const float *wt = p.wp + (int64_t)(r * p.S + s) * p.K * p.C + c0;
-        for (int k = 0; k < p.K; k += 4) {
-          const float4 dv = __ldg(reinterpret_cast<const float4 *>(dp + k));
-          const float ds[4] = {dv.x, dv.y, dv.z, dv.w};
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const float *wr = wt + (int64_t)(k + j) * p.C;
-            if (KT % 4 == 0) {
-#pragma unroll
-              for (int u = 0; u < KT / 4; ++u) {
-                const float4 w4 = __ldg(reinterpret_cast<const float4 *>(wr + 4 * u));
-                acc[4 * u + 0] = fmaf(ds[j], w4.x, acc[4 * u + 0]);
-                acc[4 * u + 1] = fmaf(ds[j], w4.y, acc[4 * u + 1]);
-                acc[4 * u + 2] = fmaf(ds[j], w4.z, acc[4 * u + 2]);
-                acc[4 * u + 3] = fmaf(ds[j], w4.w, acc[4 * u + 3]);
-              }
-            } else {
-#pragma unroll
-              for (int u = 0; u < KT; ++u) acc[u] = fmaf(ds[j], __ldg(wr + u), acc[u]);
-            }
-          }
-        }
-      }
-    }
-    float *go = p.g_out + opix * p.C + c0;
-    if (KT % 4 == 0) {
-#pragma unroll
-      for (int u = 0; u < KT / 4; ++u)
-        *reinterpret_cast<float4 *>(go + 4 * u) = make_float4(acc[4 * u], acc[4 * u + 1], acc[4 * u + 2], acc[4 * u + 3]);
-    } else {
-#pragma unroll
-      for (int j = 0; j < KT; ++j) go[j] = acc[j];
-    }
-  }
-  if (has_in) {
-#pragma unroll
-    for (int j = 0; j < KT; ++j) {
-      float g = 0.f, gx = 0.f;
-      if (valid) {
-        const float ah = (__ldg(p.a_prev + opix * p.C + c0 + j) - mean_s[c0 + j]) * rstd_s[c0 + j];
-        g = acc[j];
-        gx = acc[j] * ah;
-      }
-      const float s1 = warp_sum(g), s2 = warp_sum(gx);
-      if (lane == 0) {
-        red[warp][j] = s1;
-        red[warp][KT + j] = s2;
-      }
-    }
-    __syncthreads();
-    if (tid < 2 * KT) {
-      float tsum = 0.f;
-#pragma unroll
-      for (int wi = 0; wi < 8; ++wi) tsum += red[wi][tid];
-      atomicAdd(p.sums + (tid < KT ? 0 : p.C) + c0 + (tid % KT), (double)tsum);
-    }
-  }
-}
-
 struct NbDgrad2 {
   const float *dz, *wp, *a_prev;
   float *g_out;
@@ -834,7 +590,7 @@ struct NbDgrad2 {
   int PRm, PCm;     // window rows / columns of the class with the most taps (shared-memory carve-up)
   int tapsm;        // most taps of a class
 };
-// Data gradient, v2: blockIdx.z = stride-parity class (all its pixels use the same Rc x Sc taps), the dz window of the
+// Data gradient: blockIdx.z = stride-parity class (all its pixels use the same Rc x Sc taps), the dz window of the
 // tile and the class's slice of the weights staged in shared memory; lanes = consecutive class pixels (consecutive dz
 // pixels: conflict-free float4 reads with pitch K + 4), the KT input channels of a thread read weights as broadcasts.
 // dynamic smem: w [tapsm*K][KB] | window [TN][PRm][PCm][KP] | mean, rstd [C] | red [8][2*KT]
@@ -1122,10 +878,6 @@ static int pow2ceil(int v) {
   while (r < v) r *= 2;
   return r;
 }
-static bool nb_v1() {
-  static const bool v1 = getenv("B200GAN_NB_V1") && atoi(getenv("B200GAN_NB_V1")) != 0;
-  return v1;
-}
 constexpr size_t NB_SMEM_MAX = 200 * 1024;
 
 struct NbPlan {
@@ -1214,7 +966,7 @@ extern "C" int b200gan_nb_supported(const b200gan_conv_geom *g);
 extern "C" int b200gan_nb_groups_supported(const b200gan_conv_geom *g, int32_t groups) {
   if (!b200gan_nb_supported(g)) return 0;
   if (groups <= 1) return 1;
-  if (nb_v1() || groups > NB_MAX_GROUPS || g->N % groups != 0) return 0;
+  if (groups > NB_MAX_GROUPS || g->N % groups != 0) return 0;
   return nb_plan_fprop(g, groups).ok && nb_plan_dgrad(g, groups).ok ? 1 : 0;
 }
 
@@ -1227,7 +979,7 @@ extern "C" int b200gan_nb_supported(const b200gan_conv_geom *g) {
   if (g->C > 1 && (g->C % 4 != 0)) return 0;
   if (g->R * g->S != 9 && g->R * g->S != 16) return 0;
   if ((int64_t)g->R * g->S * g->C * g->K * 4 > (int64_t)512 * 1024) return 0;
-  if (!nb_v1() && (!nb_plan_fprop(g).ok || !nb_plan_dgrad(g).ok)) return 0;
+  if (!nb_plan_fprop(g).ok || !nb_plan_dgrad(g).ok) return 0;
   return 1;
 }
 
@@ -1270,13 +1022,12 @@ static int nb_fprop2_launch(const b200gan_conv_geom *g, const NbBn &in_bn, float
 // network: pix2pix/models.py:76,118  Conv2d(3 | 6, 64, 4, 2, 1); cyclegan/models.py:49-50  ReflectionPad2d(3) +
 // Conv2d(3, 64, 7)), where a tensor-core tile has no K dimension to speak of.
 bool nb_plain_fprop_ok(const b200gan_conv_geom *g) {
-  if (nb_v1() || !g || g->transposed || g->up != 1) return false;
+  if (!g || g->transposed || g->up != 1) return false;
   if (g->pad_mode != B200GAN_PAD_ZERO && g->pad_mode != B200GAN_PAD_REFLECT) return false;
   if (g->stride != 1 && g->stride != 2) return false;
   if (g->C < 1 || g->C > 8 || g->K < 16 || g->K > NB_MAXC || g->K % 16 != 0) return false;
   if (g->R != g->S || (g->R != 3 && g->R != 4 && g->R != 7)) return false;
-  static const bool on = !(getenv("B200GAN_NB_PLAIN") && atoi(getenv("B200GAN_NB_PLAIN")) == 0);
-  return on && nb_plan_fprop(g).ok;
+  return nb_plan_fprop(g).ok;
 }
 int nb_plain_fprop(const b200gan_conv_geom *g, const b200gan_epilogue *ep, const float *x, const float *packed, float *y,
                    cudaStream_t st) {
@@ -1296,30 +1047,13 @@ extern "C" int b200gan_nb_fprop(const b200gan_conv_geom *g, const b200gan_nb_bn 
   if (groups < 1) groups = 1;
   B2_CHECK_ARG(!(in_bn && in_bn->stats) || (in_bn->groups > 1 ? in_bn->groups : 1) == groups,
                "nb_fprop: the input edge and the call disagree on the statistics group count");
-  B2_CHECK_ARG(groups == 1 || !nb_v1(), "nb_fprop: statistics groups need the staged kernels");
   B2_CHECK_ARG(x && packed && y, "nb_fprop: null pointer");
   B2_CHECK_ARG((((uintptr_t)x | (uintptr_t)packed | (uintptr_t)y) & 15) == 0, "nb_fprop: pointers must be 16-byte aligned");
   cudaStream_t st = as_stream(stream);
   if (out_stats) B2_CUDA(cudaMemsetAsync(out_stats, 0, (size_t)groups * 2 * g->K * sizeof(double), st));
-  const int64_t M = (int64_t)g->N * g->P * g->Q;
-  if (M == 0) return B200GAN_OK;
-  NbFprop p;
-  p.x = x; p.wp = packed; p.bias = bias; p.cs = chan_scale; p.y = y; p.out_stats = out_stats;
-  p.in_bn = to_bn(in_bn);
-  p.rm = running_mean; p.rv = running_var; p.nbt = reinterpret_cast<long long *>(num_batches_tracked); p.momentum = momentum;
-  p.N = g->N; p.H = g->H; p.W = g->W; p.C = g->C; p.P = g->P; p.Q = g->Q; p.K = g->K; p.R = g->R; p.S = g->S;
-  p.stride = g->stride; p.pad_t = g->pad_t; p.pad_l = g->pad_l; p.slope = slope; p.act = act;
-  if (!nb_v1())
-    return nb_fprop2_launch(g, p.in_bn, p.rm, p.rv, p.nbt, momentum, x, packed, bias, act, slope, chan_scale, y, out_stats,
-                            0, 0, groups, st);
-  // v1 (B200GAN_NB_V1=1): direct gathers from global memory
-  const int KT = (g->K % 8 == 0 && M * (g->K / 8) >= num_sms() * 512) ? 8 : 4;
-  p.Mpad = (int)(ceil_div64(M, 256) * 256);
-  const unsigned blocks = (unsigned)((int64_t)(g->K / KT) * (p.Mpad / 256));
-  if (KT == 8) nbk_fprop_kernel<8><<<blocks, 256, 0, st>>>(p);
-  else nbk_fprop_kernel<4><<<blocks, 256, 0, st>>>(p);
-  B2_LAUNCH_CHECK();
-  return B200GAN_OK;
+  if ((int64_t)g->N * g->P * g->Q == 0) return B200GAN_OK;
+  return nb_fprop2_launch(g, to_bn(in_bn), running_mean, running_var, reinterpret_cast<long long *>(num_batches_tracked),
+                          momentum, x, packed, bias, act, slope, chan_scale, y, out_stats, 0, 0, groups, st);
 }
 
 extern "C" int b200gan_nb_dz(int32_t N, int64_t PQ, int32_t K, const float *g, const float *a, const float *chan_scale,
@@ -1527,14 +1261,13 @@ static int nb_dgrad2_launch(const b200gan_conv_geom *g, const float *dz, const f
 // Stand-alone data gradient of a layer with a handful of INPUT channels (the discriminators' first conv, whose input
 // gradient flows back into the generator: pix2pix/models.py:118 Conv2d(6, 64, 4, 2, 1); cyclegan/models.py:116).
 bool nb_plain_dgrad_ok(const b200gan_conv_geom *g) {
-  if (nb_v1() || !g || g->transposed || g->up != 1 || g->pad_mode != B200GAN_PAD_ZERO) return false;
+  if (!g || g->transposed || g->up != 1 || g->pad_mode != B200GAN_PAD_ZERO) return false;
   if (g->stride != 1 && g->stride != 2) return false;
   if (g->pad_t != g->pad_b || g->pad_l != g->pad_r) return false;
   if (g->C < 1 || g->C > 8 || (g->C != 1 && g->C != 3 && g->C != 6 && g->C % 4 != 0)) return false;
   if (g->K < 4 || g->K > NB_MAXC || g->K % 4 != 0) return false;
   if (g->R * g->S != 9 && g->R * g->S != 16 && !(g->R == 7 && g->S == 7 && g->stride == 1)) return false;
-  static const bool on = !(getenv("B200GAN_NB_PLAIN") && atoi(getenv("B200GAN_NB_PLAIN")) == 0);
-  return on && nb_plan_dgrad(g).ok;
+  return nb_plan_dgrad(g).ok;
 }
 int nb_plain_dgrad(const b200gan_conv_geom *g, const float *dy, const float *packed, float *dx, cudaStream_t st) {
   if ((int64_t)g->N * g->H * g->W == 0) return B200GAN_OK;
@@ -1551,24 +1284,9 @@ extern "C" int b200gan_nb_dgrad(const b200gan_conv_geom *g, const float *dz, con
   B2_CHECK_ARG(!sums || (in_bn && in_bn->stats && a_prev), "nb_dgrad: sums need the upstream BatchNorm and its input");
   cudaStream_t st = as_stream(stream);
   const int dgroups = (in_bn && in_bn->stats && in_bn->groups > 1) ? in_bn->groups : 1;
-  B2_CHECK_ARG(dgroups == 1 || !nb_v1(), "nb_dgrad: statistics groups need the staged kernels");
   if (sums) B2_CUDA(cudaMemsetAsync(sums, 0, (size_t)dgroups * 2 * g->C * sizeof(double), st));
   if ((int64_t)g->N * g->H * g->W == 0) return B200GAN_OK;
-  NbDgrad p;
-  p.dz = dz; p.wp = packed; p.a_prev = a_prev; p.g_out = g_out; p.sums = sums; p.in_bn = to_bn(in_bn);
-  p.N = g->N; p.H = g->H; p.W = g->W; p.C = g->C; p.P = g->P; p.Q = g->Q; p.K = g->K; p.R = g->R; p.S = g->S;
-  p.stride = g->stride; p.pad_t = g->pad_t; p.pad_l = g->pad_l;
-  const int st_ = g->stride;
-  if (!nb_v1()) return nb_dgrad2_launch(g, dz, packed, p.in_bn, a_prev, g_out, sums, st);
-  const int64_t Mc = (int64_t)g->N * ceil_div(g->H, st_) * ceil_div(g->W, st_);  // class 0 is the largest
-  p.Mpad = (int)(ceil_div64(Mc, 256) * 256);
-  const int KT = g->C % 8 == 0 ? ((Mc * (g->C / 8) * st_ * st_ >= num_sms() * 512) ? 8 : 4) : (g->C % 4 == 0 ? 4 : 1);
-  dim3 grid((unsigned)((int64_t)(g->C / KT) * (p.Mpad / 256)), 1, (unsigned)(st_ * st_));
-  if (KT == 8) nbk_dgrad_kernel<8><<<grid, 256, 0, st>>>(p);
-  else if (KT == 4) nbk_dgrad_kernel<4><<<grid, 256, 0, st>>>(p);
-  else nbk_dgrad_kernel<1><<<grid, 256, 0, st>>>(p);
-  B2_LAUNCH_CHECK();
-  return B200GAN_OK;
+  return nb_dgrad2_launch(g, dz, packed, to_bn(in_bn), a_prev, g_out, sums, st);
 }
 
 static int tail_grid(int64_t total, int C) {

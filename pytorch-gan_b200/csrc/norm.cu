@@ -359,8 +359,7 @@ norm_bwd_apply_v4_kernel(const float *__restrict__ dy, const float *__restrict__
 }
 
 static bool fast_path(const b200gan_norm_desc *d, const void *a, const void *b, const void *c, const void *e) {
-  static const bool enabled = !(getenv("B200GAN_NORM_FAST") && atoi(getenv("B200GAN_NORM_FAST")) == 0);
-  if (!enabled || d->C % 4 != 0) return false;
+  if (d->C % 4 != 0) return false;
   const int CV = d->C / 4;
   if (CV > 256 || 256 % CV != 0) return false;
   return (((uintptr_t)a | (uintptr_t)b | (uintptr_t)c | (uintptr_t)e) & 15) == 0;

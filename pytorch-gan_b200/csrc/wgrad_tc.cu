@@ -354,9 +354,8 @@ static bool wg_plan(const b200gan_conv_geom *g, WgPlan &pl) {
   const int mch = pl.s_is_a ? pl.sch : pl.dch, nch = pl.s_is_a ? pl.dch : pl.sch;
   pl.NB = nch % 128 == 0 ? 128 : (nch % 64 == 0 ? 64 : 32);
   // 128 x 256 output tiles: the 128-channel operand is re-read and re-transposed half as often (a 256 -> 256 3x3 layer
-  // pulls 9 jobs x 4 tiles x 33 MB = 1.2 GB through L2 with 128 x 128 tiles).  B200GAN_WG_NB256=0 switches it off.
-  static const int nb256 = getenv("B200GAN_WG_NB256") ? atoi(getenv("B200GAN_WG_NB256")) : 1;
-  if (nb256 && nch % 256 == 0) pl.NB = 256;
+  // pulls 9 jobs x 4 tiles x 33 MB = 1.2 GB through L2 with 128 x 128 tiles)
+  if (nch % 256 == 0) pl.NB = 256;
   pl.mtotal = mch;
   pl.ldn = nch;
   pl.mtiles = mch / 128;
@@ -504,8 +503,7 @@ int tc_wgrad(const b200gan_conv_geom *g, const float *x, const float *dy, float 
   rp.K = g->K; rp.C = g->C; rp.R = g->R; rp.S = g->S; rp.njobs = pl.njobs;
   rp.s_is_a = pl.s_is_a; rp.up2 = up2 ? 1 : 0; rp.transposed = g->transposed ? 1 : 0; rp.mtotal = pl.mtotal; rp.ldn = pl.ldn;
   int64_t total = (int64_t)g->K * g->C * g->R * g->S;
-  static const bool tiled = !(getenv("B200GAN_WG_REDUCE_TILED") && atoi(getenv("B200GAN_WG_REDUCE_TILED")) == 0);
-  if (tiled && g->R * g->S <= WR_TAPS && g->K >= 32 && g->C >= 32) {
+  if (g->R * g->S <= WR_TAPS && g->K >= 32 && g->C >= 32) {
     const bool col_is_k = (pl.s_is_a != 0) != (g->transposed != 0);
     const int ncol = col_is_k ? g->K : g->C, nrow = col_is_k ? g->C : g->K;
     const unsigned tiles = (unsigned)(ceil_div(ncol, WR_COL) * ceil_div(nrow, WR_ROW));

@@ -1,5 +1,7 @@
 """GPU parity of the flat-buffer Adam entry point (b200gan_adam_step) against torch.optim.Adam with the reference's
 hyper-parameters (dcgan.py:134-135: lr 2e-4, betas (0.5, 0.999), eps 1e-8, no weight decay, no amsgrad)."""
+import itertools
+
 import pytest
 import torch
 
@@ -136,10 +138,37 @@ def test_adam_step_invalidates_the_packed_weight_caches():
         assert rel_err(ours.weight, ref.weight) < 2e-2
 
 
+def _reference_pack(w, kind, transposed):
+    """The packed layout of include/b200gan.h restated in torch: taps outermost, then [ci][co] or [co][ci]; the x2-upsample
+    kinds sum the 3x3 taps of each phase tap in fp32, r-major then s, from 0; the TC kinds round to TF32 as
+    cvt.rna.tf32.f32 does (to nearest, ties away from zero)."""
+    from b200gan import _lib
+    wk = w.transpose(0, 1) if transposed else w          # [co][ci][r][s]; ConvTranspose2d stores [ci][co][r][s]
+    if kind in (_lib.PACK_TC_FPROP_UP2, _lib.PACK_TC_DGRAD_UP2):
+        rset = {(0, 0): (0,), (0, 1): (1, 2), (1, 0): (0, 1), (1, 1): (2,)}   # 3x3 taps behind phase a, tap d
+        taps = []
+        for a, b, dr, ds in itertools.product((0, 1), repeat=4):            # t = (2a + b) * 4 + 2dr + ds
+            v = torch.zeros_like(wk[:, :, 0, 0])
+            for r in rset[a, dr]:
+                for s in rset[b, ds]:
+                    v = v + wk[:, :, r, s]
+            taps.append(v)
+        packed = torch.stack(taps)                                           # [16][co][ci]
+    else:
+        packed = wk.permute(2, 3, 0, 1).flatten(0, 1)                        # [r*S + s][co][ci]
+    if kind in (_lib.PACK_SIMT_FPROP, _lib.PACK_TC_DGRAD, _lib.PACK_TC_DGRAD_UP2):
+        packed = packed.transpose(1, 2)                                      # [tap][ci][co]
+    packed = packed.contiguous()
+    if kind != _lib.PACK_SIMT_FPROP and kind != _lib.PACK_SIMT_DGRAD:
+        packed = ((packed.view(torch.int32) + 0x1000) & ~0x1FFF).view(torch.float32)
+    return packed.flatten()
+
+
 def test_multi_pack_is_bit_identical_to_the_per_layer_pack():
-    """b200gan_pack_weights_multi (one launch per optimizer step, tiles transposed through shared memory) against
-    b200gan_pack_weights (one launch per copy): every layout, Conv2d and ConvTranspose2d parameters, ragged channel
-    counts, the folded x2-upsample layouts -- index arithmetic only, so bit-exact."""
+    """b200gan_pack_weights (one copy) and b200gan_pack_weights_multi (one launch per optimizer step) against the packed
+    layout restated in torch: every layout, Conv2d and ConvTranspose2d parameters, ragged channel counts, a layer too
+    narrow for the shared-memory tiles (element-wise mode), the folded x2-upsample layouts -- index arithmetic only, so
+    bit-exact."""
     from b200gan import ops
     from b200gan import _lib
     torch.manual_seed(11)
@@ -151,15 +180,15 @@ def test_multi_pack_is_bit_identical_to_the_per_layer_pack():
     cases.append(((2, 3, 16, 16), (64, 3, 4, 4), 2, (1, 1, 1, 1), 1, False, plain))          # too narrow for tiles
     cases.append(((2, 128, 16, 16), (64, 128, 3, 3), 1, (1, 1, 1, 1), 2, False,
                   (_lib.PACK_TC_FPROP_UP2, _lib.PACK_TC_DGRAD_UP2)))
-    jobs, singles = [], []
+    jobs, refs = [], []
     for xs, ws, st, pads, up, tr, kinds in cases:
         w = torch.randn(*ws, device="cuda")
         g, _ = ops.make_geom(xs, ws, st, pads, 0, up, tr)
         for kind in kinds:
-            single = ops.pack_weights(g, w, kind)
-            buf = torch.full_like(single, float("nan"))
-            jobs.append((g, kind, w, buf))
-            singles.append(single)
+            ref = _reference_pack(w, kind, tr)
+            assert torch.equal(ops.pack_weights(g, w, kind), ref), (tuple(w.shape), kind)
+            jobs.append((g, kind, w, torch.full_like(ref, float("nan"))))
+            refs.append(ref)
     ops.pack_weights_multi(jobs)
-    for (g, kind, w, buf), single in zip(jobs, singles):
-        assert torch.equal(buf, single), (tuple(w.shape), kind)
+    for (g, kind, w, buf), ref in zip(jobs, refs):
+        assert torch.equal(buf, ref), (tuple(w.shape), kind)
