@@ -117,17 +117,25 @@ struct TcParams {
     if (p.trace) p.trace[((size_t)blockIdx.z * gridDim.x + blockIdx.x) * 64 + (slot)] = clock64(); \
   } while (0)
 
-__device__ __forceinline__ float warp_colsum32(float (&v)[32], int lane) {
+// One butterfly step per template instance: in a single loop over `off` the compiler does not unroll the inner loop,
+// whose trip count depends on `off`, so v and the epilogue's other 32-element arrays were indexed at run time and
+// lived in local memory (a 256-byte stack frame), which made the statistics epilogue several times slower.
+template <int OFF>
+__device__ __forceinline__ void colsum_step(float (&v)[32], int lane) {
+  const bool upper = (lane & OFF) != 0;
 #pragma unroll
-  for (int off = 16; off >= 1; off >>= 1) {
-    const bool upper = (lane & off) != 0;
-#pragma unroll
-    for (int i = 0; i < off; ++i) {
-      float send = upper ? v[i] : v[i + off];
-      float keep = upper ? v[i + off] : v[i];
-      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-    }
+  for (int i = 0; i < OFF; ++i) {
+    float send = upper ? v[i] : v[i + OFF];
+    float keep = upper ? v[i + OFF] : v[i];
+    v[i] = keep + __shfl_xor_sync(0xffffffffu, send, OFF);
   }
+}
+__device__ __forceinline__ float warp_colsum32(float (&v)[32], int lane) {
+  colsum_step<16>(v, lane);
+  colsum_step<8>(v, lane);
+  colsum_step<4>(v, lane);
+  colsum_step<2>(v, lane);
+  colsum_step<1>(v, lane);
   return v[0];  // sum over the 32 lanes of column `lane`
 }
 
@@ -538,10 +546,11 @@ conv_tc_up2_allphase_kernel(const __grid_constant__ CUtensorMap tmA, const __gri
         if (it < 16) TC_TRACE(2 + it);
         mbar_arrive_expect_tx(&full[stage], TC_A_BYTES + sp.nb * MP_B_BYTES);
         tma_load_5d(sa, &tmA, &full[stage], kc * TC_BK, w0 + sp.dw, 0, h0 + sp.dh, n0);
-#pragma unroll 1
-        for (int u = 0; u < sp.nb; ++u)
-          tma_load_2d(sa + TC_A_BYTES + u * MP_B_BYTES, &tmB, &full[stage], kc * TC_BK,
-                      sp.bt[u] * p.kout_total + ntile * BN);
+#pragma unroll
+        for (int u = 0; u < MP_MAX_USES; ++u)
+          if (u < sp.nb)
+            tma_load_2d(sa + TC_A_BYTES + u * MP_B_BYTES, &tmB, &full[stage], kc * TC_BK,
+                        sp.bt[u] * p.kout_total + ntile * BN);
         if (++kc == p.kchunks) {
           kc = 0;
           ++step;
