@@ -52,8 +52,8 @@ enum { B200GAN_PAD_ZERO = 0, B200GAN_PAD_REFLECT = 1 };
 
 /* packed-weight layouts produced by b200gan_pack_weights() */
 enum {
-  B200GAN_PACK_SIMT_FPROP = 0, /* [R][S][Cin][Cout]   : conv fprop / convT dgrad, SIMT        */
-  B200GAN_PACK_SIMT_DGRAD = 1, /* [R][S][Cout][Cin]   : conv dgrad / convT fprop, SIMT        */
+  B200GAN_PACK_SIMT_FPROP = 0, /* [R][S][Cin][Cout]   : fprop (Conv2d and ConvTranspose2d), SIMT */
+  B200GAN_PACK_SIMT_DGRAD = 1, /* [R][S][Cout][Cin]   : dgrad (Conv2d and ConvTranspose2d), SIMT */
   B200GAN_PACK_TC_FPROP = 2,   /* [R*S][Cout][Cin]    tf32-rounded, K-major, wgmma fprop      */
   B200GAN_PACK_TC_DGRAD = 3,   /* [R*S][Cin][Cout]    tf32-rounded, taps flipped, dgrad       */
   B200GAN_PACK_TC_FPROP_UP2 = 4, /* [4 phases][4 taps][Cout][Cin]: 3x3 s1 p1 conv folded with a
@@ -88,7 +88,9 @@ typedef struct b200gan_conv_geom {
 /* Epilogue fused into fprop:  y = chan_scale[n,k] * act(conv + bias[k])  (each part optional).
  * stats (optional) receives, atomically accumulated in fp64, the per-group sums of y and y*y
  * that the following BatchNorm2d / InstanceNorm2d needs: stats[0..G) = sum, stats[G..2G) =
- * sum of squares, G = K (stats_per_sample == 0) or N*K (== 1).  Caller zeroes it. */
+ * sum of squares, G = K (stats_per_sample == 0) or N*K (== 1).  Caller zeroes it.  Both kinds
+ * are produced for every algorithm and tiling: where the kernel cannot fuse them (e.g. a wgmma
+ * tile that spans two images) the library adds one b200gan_norm_stats pass on the same stream. */
 typedef struct b200gan_epilogue {
   const float *bias;       /* [K] or NULL                                                  */
   int32_t act;             /* B200GAN_ACT_*                                                */
@@ -126,7 +128,7 @@ int b200gan_pack_weights_multi(const b200gan_pack_job *jobs, int32_t count, void
 int b200gan_conv2d_supported(const b200gan_conv_geom *g, int pass, int algo);
 
 /* y[N][P][Q][K] = epilogue(conv(x, w)).  `packed` must be the layout the algorithm wants:
- * SIMT: PACK_SIMT_FPROP (Conv2d) / PACK_SIMT_DGRAD (ConvTranspose2d);
+ * SIMT: PACK_SIMT_FPROP (Conv2d and ConvTranspose2d alike);
  * TC  : PACK_TC_FPROP, or PACK_TC_FPROP_UP2 when g->up == 2.
  * Replaces cudnnConvolutionForward behind nn.Conv2d.forward (dcgan.py:69,95). */
 int b200gan_conv2d_fprop(const b200gan_conv_geom *g, const b200gan_epilogue *ep, const float *x,

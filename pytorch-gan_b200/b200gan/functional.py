@@ -13,8 +13,8 @@ import torch
 
 from . import ops
 from ._lib import ConvGeom
-from ._lib import (ACT_LRELU, ACT_NONE, ACT_RELU, ACT_SIGMOID, ACT_TANH, ALGO_AUTO, ALGO_SIMT, ALGO_TC, PACK_SIMT_DGRAD,
-                   PACK_SIMT_FPROP, PACK_TC_DGRAD, PACK_TC_DGRAD_UP2, PACK_TC_FPROP, PACK_TC_FPROP_UP2, PAD_ZERO)
+from ._lib import (ACT_LRELU, ACT_NONE, ACT_RELU, ACT_SIGMOID, ACT_TANH, ALGO_SIMT,  # noqa: F401 (re-exported)
+                   PACK_SIMT_DGRAD, PACK_SIMT_FPROP, PAD_ZERO)
 
 
 @dataclass(frozen=True)
@@ -95,25 +95,6 @@ def refresh_packs(params):
             cache.mark_fresh(w)
 
 
-def _pow2ceil(v):
-    p = 1
-    while p < v:
-        p *= 2
-    return p
-
-
-def _tc_tile_is_one_image(g, spec):
-    """True when a 128-pixel tile of the wgmma fprop never spans two images, the condition for fusing
-    per-sample (InstanceNorm) sums into its epilogue (mirrors the tile choice in conv_tc.cu:run_tc)."""
-    if spec.up == 2:
-        ho, wo = g.H, g.W                 # per-phase grid of the upsample fold
-    elif spec.transposed and spec.stride == 2:
-        ho, wo = g.P // 2, g.Q // 2       # per-phase grid of the scatter form
-    else:
-        ho, wo = g.P, g.Q
-    return min(_pow2ceil(wo), 128) * _pow2ceil(ho) >= 128
-
-
 def _as_cl(t):
     return t if ops.is_cl(t) else ops.to_cl(t)
 
@@ -128,30 +109,21 @@ class ConvFn(torch.autograd.Function):
         x = _as_cl(x)
         g, _ = ops.make_geom(tuple(x.shape), tuple(weight.shape), spec.stride, spec.pads, spec.pad_mode, spec.up,
                              spec.transposed)
-        w = weight.detach()
-        if ops.tc_supported(g, 0) and not (g.K < 32 and chan_scale is not None):
-            algo = ALGO_TC
-            packed = cache.get(g, w, PACK_TC_FPROP_UP2 if spec.up == 2 else PACK_TC_FPROP)
-        else:
-            algo = ALGO_SIMT
-            packed = cache.get(g, w, PACK_SIMT_FPROP)
+        algo, kind = ops.conv_plan(g, 0, chan_scale)
+        packed = cache.get(g, weight.detach(), kind)
         stats = None
         if spec.stats is not None:
             stats = ops.zero_scratch(x.device, 2 * (g.N * g.K if spec.stats else g.K))
-        fuse_stats = stats is not None and not (algo == ALGO_TC and spec.stats and not _tc_tile_is_one_image(g, spec))
         y = ops.conv_fprop(g, x, packed, algo, bias=None if bias is None else bias.detach(), act=spec.act,
-                           slope=spec.slope, chan_scale=chan_scale, stats=stats if fuse_stats else None,
-                           stats_per_sample=bool(spec.stats), round_tf32=spec.rtf_out)
-        if stats is not None and not fuse_stats:
-            stats = None  # caller computes them with a separate pass
+                           slope=spec.slope, chan_scale=chan_scale, stats=stats, stats_per_sample=bool(spec.stats),
+                           round_tf32=spec.rtf_out)
         ctx.spec, ctx.cache, ctx.g = spec, cache, g
         ctx.has_bias = bias is not None
         need_y = spec.act != ACT_NONE
         ctx.save_for_backward(x, weight, y if need_y else None, chan_scale)
-        if spec.stats is not None:
-            if stats is None:
-                stats = torch.empty(0, device=x.device, dtype=torch.float64)
+        if stats is not None:
             ctx.mark_non_differentiable(stats)
+            ctx.set_materialize_grads(False)  # no zero-filled gradient is launched for the statistics output
             return y, stats
         return y
 
@@ -160,7 +132,10 @@ class ConvFn(torch.autograd.Function):
         if torch.is_grad_enabled():
             # autograd.grad(..., create_graph=True): the gradient penalty of a conv critic (stargan.py:142-161,
             # dragan.py:144-167) differentiates THROUGH this backward -- build it from differentiable nodes
-            return _conv_backward_differentiable(ctx, dy)
+            if ctx.spec.up != 1 or ctx.spec.pad_mode != PAD_ZERO:
+                raise NotImplementedError("b200gan: double backward through a conv with a folded upsample / reflection "
+                                          "padding")
+            return _conv_backward_differentiable(ctx, dy) + (None, None, None)
         x, weight, y, chan_scale = ctx.saved_tensors
         spec, g = ctx.spec, ctx.g
         dy = _as_cl(dy)
@@ -169,14 +144,9 @@ class ConvFn(torch.autograd.Function):
         else:
             dz = dy
         dx = dw = db = None
-        w = weight.detach()
         if ctx.needs_input_grad[0]:
-            if ops.tc_supported(g, 1):
-                packed = ctx.cache.get(g, w, PACK_TC_DGRAD_UP2 if spec.up == 2 else PACK_TC_DGRAD)
-                dx = ops.conv_dgrad(g, dz, packed, ALGO_TC)
-            else:
-                packed = ctx.cache.get(g, w, PACK_SIMT_DGRAD)
-                dx = ops.conv_dgrad(g, dz, packed, ALGO_SIMT)
+            algo, kind = ops.conv_plan(g, 1)
+            dx = ops.conv_dgrad(g, dz, ctx.cache.get(g, weight.detach(), kind), algo)
         want_db = ctx.has_bias and ctx.needs_input_grad[2]
         if want_db and dz is not dy and spec.rtf_dz:
             # dz was rounded to TF32 for the tensor-core passes; a bias gradient is a sum with heavy cancellation
@@ -184,8 +154,7 @@ class ConvFn(torch.autograd.Function):
             db = ops.bias_grad(dy, y, chan_scale, spec.act, spec.slope)
             want_db = False
         if ctx.needs_input_grad[1] or want_db:
-            algo = ALGO_SIMT if ops.Config.algo == "simt" else ALGO_AUTO
-            dw, db2 = ops.conv_wgrad(g, x, dz, tuple(weight.shape), want_db, algo)
+            dw, db2 = ops.conv_wgrad(g, x, dz, tuple(weight.shape), want_db, ops.conv_plan(g, 2)[0])
             db = db2 if want_db else db
             if not ctx.needs_input_grad[1]:
                 dw = None
@@ -197,23 +166,17 @@ class ConvFn(torch.autograd.Function):
 #   D = dgrad(dz, w)  (= dF/dx applied to dz):   dD/d(dz) applied to u = fprop(u, w),   dD/dw applied to u = wgrad(u, dz)
 #   W = wgrad(x, dz)  (= dF/dw applied to dz):   dW/dx applied to v  = dgrad(dz, v),    dW/d(dz) applied to v = fprop(x, v)
 def _plain_fprop(g, x, w):
-    tc = ops.tc_supported(g, 0)
-    kind = (PACK_TC_FPROP_UP2 if g.up == 2 else PACK_TC_FPROP) if tc else PACK_SIMT_FPROP
-    if g.transposed and not tc:
-        kind = PACK_SIMT_DGRAD
-    return ops.conv_fprop(g, x, ops.pack_weights(g, w, kind), ALGO_TC if tc else ALGO_SIMT)
+    algo, kind = ops.conv_plan(g, 0)
+    return ops.conv_fprop(g, x, ops.pack_weights(g, w, kind), algo)
 
 
 def _plain_dgrad(g, dz, w):
-    tc = ops.tc_supported(g, 1)
-    kind = (PACK_TC_DGRAD_UP2 if g.up == 2 else PACK_TC_DGRAD) if tc else PACK_SIMT_DGRAD
-    if g.transposed and not tc:
-        kind = PACK_SIMT_FPROP
-    return ops.conv_dgrad(g, dz, ops.pack_weights(g, w, kind), ALGO_TC if tc else ALGO_SIMT)
+    algo, kind = ops.conv_plan(g, 1)
+    return ops.conv_dgrad(g, dz, ops.pack_weights(g, w, kind), algo)
 
 
 def _plain_wgrad(g, x, dz, wshape):
-    return ops.conv_wgrad(g, x, dz, wshape, False, ALGO_SIMT if ops.Config.algo == "simt" else ALGO_AUTO)[0]
+    return ops.conv_wgrad(g, x, dz, wshape, False, ops.conv_plan(g, 2)[0])[0]
 
 
 class ConvDgradFn(torch.autograd.Function):
@@ -251,27 +214,28 @@ class ConvWgradFn(torch.autograd.Function):
 
 
 def _conv_backward_differentiable(ctx, dy):
+    """(dx, dw, db) of a conv block [+bias] [act] [* Dropout2d scale] from differentiable nodes, for a backward under
+    autograd.grad(..., create_graph=True).  ctx: a ConvFn / NbConvFn context, which saves (x, weight, y, chan_scale)
+    and has .spec (act, slope), .g and .has_bias.  dz is rebuilt from (y, act, slope, chan_scale)."""
     x, weight, y, chan_scale = ctx.saved_tensors
-    spec, g = ctx.spec, ctx.g
-    if spec.up != 1 or spec.pad_mode != PAD_ZERO:
-        raise NotImplementedError("b200gan: double backward through a conv with a folded upsample / reflection padding")
+    act, slope, g = ctx.spec.act, ctx.spec.slope, ctx.g
+    if chan_scale is not None and act in (ACT_TANH, ACT_SIGMOID):
+        raise NotImplementedError("b200gan: double backward through Dropout2d fused with tanh / sigmoid")
     dz = dy
-    if spec.act == ACT_LRELU:
-        dz = dz * torch.where(y > 0, 1.0, spec.slope)      # piecewise constant mask: no second-order term
-    elif spec.act == ACT_RELU:
+    if act == ACT_LRELU:
+        dz = dz * torch.where(y > 0, 1.0, slope)           # piecewise constant mask: no second-order term
+    elif act == ACT_RELU:
         dz = dz * (y > 0).to(dy.dtype)
-    elif spec.act == ACT_TANH:
+    elif act == ACT_TANH:
         dz = dz * (1 - y * y)                              # y is this node's (differentiable) output
-    elif spec.act == ACT_SIGMOID:
+    elif act == ACT_SIGMOID:
         dz = dz * (y * (1 - y))
     if chan_scale is not None:
         dz = dz * chan_scale.view(chan_scale.shape[0], chan_scale.shape[1], 1, 1)
-        if spec.act in (ACT_TANH, ACT_SIGMOID):
-            raise NotImplementedError("b200gan: double backward through Dropout2d fused with tanh / sigmoid")
     dx = ConvDgradFn.apply(dz, weight, g) if ctx.needs_input_grad[0] else None
     dw = ConvWgradFn.apply(x, dz, g, tuple(weight.shape)) if ctx.needs_input_grad[1] else None
     db = dz.sum((0, 2, 3)) if (ctx.has_bias and ctx.needs_input_grad[2]) else None
-    return dx, dw, db, None, None, None
+    return dx, dw, db
 
 
 
@@ -282,8 +246,6 @@ class NormFn(torch.autograd.Function):
     def forward(ctx, x, gamma, beta, stats, running_mean, running_var, nbt, spec: NormSpec):
         ops._require_cuda(x, "norm input")
         x = _as_cl(x)
-        if stats is not None and stats.numel() == 0:
-            stats = None
         y, mean_rstd, scale_shift = ops.norm_forward(
             x, None if gamma is None else gamma.detach(), None if beta is None else beta.detach(), running_mean,
             running_var, nbt, spec.per_sample, spec.eps, spec.momentum, spec.act, spec.slope, stats, spec.rtf_out,
@@ -333,7 +295,7 @@ class TailFn(torch.autograd.Function):
     def forward(ctx, a, stats, gamma, beta, running_mean, running_var, nbt, weight, bias, spec: TailSpec):
         ops._require_cuda(a, "tail input")
         a = _as_cl(a)
-        if stats is None or stats.numel() == 0:
+        if stats is None:
             stats = ops.norm_stats(a, False)
         mean_rstd, scale_shift = ops.norm_finalize(
             tuple(a.shape), stats, None if gamma is None else gamma.detach(), None if beta is None else beta.detach(),
@@ -512,17 +474,7 @@ class NbConvFn(torch.autograd.Function):
             if in_edge is not None or out_edge is not None:
                 raise NotImplementedError("b200gan: double backward through a fused conv chain with BatchNorm2d; set "
                                           "B200GAN_FUSE_CHAIN=0 for this model")
-            dz = gy
-            if spec.act == ACT_LRELU:
-                dz = dz * torch.where(y > 0, 1.0, spec.slope)
-            elif spec.act == ACT_RELU:
-                dz = dz * (y > 0).to(gy.dtype)
-            if chan_scale is not None:
-                dz = dz * chan_scale.view(chan_scale.shape[0], chan_scale.shape[1], 1, 1)
-            gx = ConvDgradFn.apply(dz, weight, g) if ctx.needs_input_grad[0] else None
-            dw = ConvWgradFn.apply(x, dz, g, tuple(weight.shape)) if ctx.needs_input_grad[1] else None
-            db = dz.sum((0, 2, 3)) if (ctx.has_bias and ctx.needs_input_grad[2]) else None
-            return (gx, dw, db) + (None,) * 10
+            return _conv_backward_differentiable(ctx, gy) + (None,) * 10
         gy, y, x = gy.detach(), y.detach(), x.detach()
         if out_edge is not None and out_edge.sums is None:
             raise RuntimeError("b200gan: fused conv chain: the consumer of this layer did not run its backward first")

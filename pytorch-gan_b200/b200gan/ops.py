@@ -10,8 +10,9 @@ import os
 import torch
 
 from . import _lib
-from ._lib import (ACT_NONE, ALGO_SIMT, ALGO_TC, PAD_REFLECT, PAD_ZERO, ConvGeom, Epilogue, GpMlpDesc, NbBn, NormDesc,
-                   TailDesc)
+from ._lib import (ACT_NONE, ALGO_AUTO, ALGO_SIMT, ALGO_TC, PACK_SIMT_DGRAD, PACK_SIMT_FPROP, PACK_TC_DGRAD,
+                   PACK_TC_DGRAD_UP2, PACK_TC_FPROP, PACK_TC_FPROP_UP2, PAD_REFLECT, PAD_ZERO, ConvGeom, Epilogue,
+                   GpMlpDesc, NbBn, NormDesc, TailDesc)
 
 CL = torch.channels_last
 
@@ -116,6 +117,21 @@ def tc_supported(g, pas):
     if Config.algo == "simt":
         return False
     return bool(_lib.load().b200gan_conv2d_supported(ctypes.byref(g), pas, ALGO_TC))
+
+
+def conv_plan(g, pas, chan_scale=None):
+    """(algo, packed layout) of pass `pas` (0 fprop, 1 dgrad, 2 wgrad) of a convolution: the one place that decides
+    which kernel family runs it and which packed weight copy that kernel reads.  The layout follows the pass, whether or
+    not the conv is transposed.  The weight gradient reads no packed copy (layout None) and lets the library route it.
+    `chan_scale`: the forward carries a Dropout2d scale, which the narrow-output (K < 32) wgmma form does not fuse."""
+    if pas == 2:
+        return (ALGO_SIMT if Config.algo == "simt" else ALGO_AUTO), None
+    tc = tc_supported(g, pas) and not (pas == 0 and g.K < 32 and chan_scale is not None)
+    if not tc:
+        return ALGO_SIMT, (PACK_SIMT_FPROP if pas == 0 else PACK_SIMT_DGRAD)
+    if pas == 0:
+        return ALGO_TC, (PACK_TC_FPROP_UP2 if g.up == 2 else PACK_TC_FPROP)
+    return ALGO_TC, (PACK_TC_DGRAD_UP2 if g.up == 2 else PACK_TC_DGRAD)
 
 
 def pack_weights(g, w, kind, out=None):

@@ -54,6 +54,15 @@ void set_error(const char *fmt, ...) {
   va_end(ap);
 }
 
+// The b200gan_epilogue statistics of a conv whose kernel did not fuse them: one b200gan_norm_stats pass over its output
+// y [N][HW][C], on the same stream.
+int conv_stats_pass(const float *y, int N, int HW, int C, int per_sample, double *stats, cudaStream_t st) {
+  b200gan_norm_desc nd;
+  memset(&nd, 0, sizeof(nd));
+  nd.N = N; nd.HW = HW; nd.C = C; nd.per_sample = per_sample;
+  return b200gan_norm_stats(&nd, y, stats, st);
+}
+
 int num_sms() {
   static std::atomic<int> cache[64];
   int dev = 0;
@@ -332,11 +341,6 @@ extern "C" int b200gan_conv2d_supported(const b200gan_conv_geom *g, int pass, in
   return tc_supported(g, pass);
 }
 
-static int resolve_algo(const b200gan_conv_geom *g, int pass, int algo) {
-  if (algo == B200GAN_ALGO_AUTO) return tc_supported(g, pass) ? B200GAN_ALGO_TC : B200GAN_ALGO_SIMT;
-  return algo;
-}
-
 extern "C" int b200gan_conv2d_fprop(const b200gan_conv_geom *g, const b200gan_epilogue *ep, const float *x,
                                     const float *packed, float *y, int algo, void *stream) {
   if (int e = validate_geom(g)) return e;
@@ -359,19 +363,37 @@ extern "C" int b200gan_conv2d_fprop(const b200gan_conv_geom *g, const b200gan_ep
                           g->pad_mode, g->up, g->transposed ? 1 : 0, ep, x, packed, y, st);
   }
   if (rc) return rc;
-  if (ep && ep->stats) {
-    b200gan_norm_desc nd;
-    memset(&nd, 0, sizeof(nd));
-    nd.N = g->N; nd.HW = g->P * g->Q; nd.C = g->K; nd.per_sample = ep->stats_per_sample;
-    return b200gan_norm_stats(&nd, y, ep->stats, stream);
-  }
+  if (ep && ep->stats) return conv_stats_pass(y, g->N, g->P * g->Q, g->K, ep->stats_per_sample, ep->stats, st);
   return B200GAN_OK;
 }
 
+// The kernel route of each gradient pass (ALGO_AUTO resolves here).  The entry point and its workspace query both
+// switch on it, so the size a caller allocates always belongs to the path that runs.
+enum class DgradRoute { Tc, Transposed, Fewk, Staged, Virtual };
+
+static DgradRoute dgrad_route(const b200gan_conv_geom *g, int algo) {
+  if (algo == B200GAN_ALGO_AUTO ? tc_supported(g, 1) : algo == B200GAN_ALGO_TC) return DgradRoute::Tc;
+  if (g->transposed) return DgradRoute::Transposed;     // SIMT gather over dy
+  if (fewk_ok(g, 1)) return DgradRoute::Fewk;           // K <= 4 output channels, stride 1
+  if (nb_plain_dgrad_ok(g)) return DgradRoute::Staged;  // few input channels
+  return DgradRoute::Virtual;  // gradient of the virtual input, folded back through reflection padding / x2 upsample
+}
+
+enum class WgradRoute { Tc, Fewk, Staged, Simt };
+
+static WgradRoute wgrad_route(const b200gan_conv_geom *g, int algo) {
+  if (algo == B200GAN_ALGO_AUTO ? tc_supported(g, 2) : algo == B200GAN_ALGO_TC) return WgradRoute::Tc;
+  // K <= 4 output channels, stride 1 (the image / patch output layers): lanes = input channels
+  if (fewk_ok(g, 2)) return WgradRoute::Fewk;
+  // narrow layers (C or K small): patch + dy tile staged in shared memory, all taps of a (c, 4k) set in registers;
+  // beyond ~2e10 MACs (wide layers that are not tensor-core shaped) the generic kernel's larger tiles win
+  if (nb_wgrad_ok(g) && (int64_t)g->N * g->P * g->Q * g->K * g->C * g->R * g->S <= (int64_t)2e10)
+    return WgradRoute::Staged;
+  return WgradRoute::Simt;
+}
+
 extern "C" size_t b200gan_conv2d_dgrad_workspace_floats(const b200gan_conv_geom *g, int algo) {
-  if (!g || g->transposed) return 0;
-  if (resolve_algo(g, 1, algo) == B200GAN_ALGO_TC) return 0;
-  if (fewk_ok(g, 1) || nb_plain_dgrad_ok(g)) return 0;
+  if (!g || dgrad_route(g, algo) != DgradRoute::Virtual) return 0;
   size_t n = 0;
   int Hv = g->H * g->up, Wv = g->W * g->up;
   if (g->pad_mode == B200GAN_PAD_REFLECT)
@@ -386,17 +408,21 @@ extern "C" int b200gan_conv2d_dgrad(const b200gan_conv_geom *g, const float *dy,
   B2_CHECK_ARG(dy && packed && dx, "conv2d_dgrad: null pointer");
   B2_CHECK_ARG(algo != B200GAN_ALGO_AUTO, "conv2d_dgrad: pass SIMT or TC explicitly");
   cudaStream_t st = as_stream(stream);
-  if (algo == B200GAN_ALGO_TC) {
-    if (!tc_supported(g, 1)) B2_UNSUPPORTED("conv2d_dgrad: geometry not supported by the tensor-core path");
-    return tc_dgrad(g, dy, packed, dx, st);
+  switch (dgrad_route(g, algo)) {
+    case DgradRoute::Tc:
+      if (!tc_supported(g, 1)) B2_UNSUPPORTED("conv2d_dgrad: geometry not supported by the tensor-core path");
+      return tc_dgrad(g, dy, packed, dx, st);
+    case DgradRoute::Transposed:
+      // dx[n,ih,iw,c] = sum_{r,s,k} dy[n, ih*stride - pad + r, iw*stride - pad + s, k] * w[c,k,r,s]
+      return simt_gather_gemm(g->N, g->P, g->Q, g->K, g->H, g->W, g->C, g->R, g->S, g->stride, g->pad_t, g->pad_l,
+                              B200GAN_PAD_ZERO, 1, 0, nullptr, dy, packed, dx, st);
+    case DgradRoute::Fewk:
+      return fewk_dgrad(g, dy, packed, dx, st);
+    case DgradRoute::Staged:
+      return nb_plain_dgrad(g, dy, packed, dx, st);
+    case DgradRoute::Virtual:
+      break;
   }
-  if (g->transposed) {
-    // dx[n,ih,iw,c] = sum_{r,s,k} dy[n, ih*stride - pad + r, iw*stride - pad + s, k] * w[c,k,r,s]
-    return simt_gather_gemm(g->N, g->P, g->Q, g->K, g->H, g->W, g->C, g->R, g->S, g->stride, g->pad_t, g->pad_l,
-                            B200GAN_PAD_ZERO, 1, 0, nullptr, dy, packed, dx, st);
-  }
-  if (fewk_ok(g, 1)) return fewk_dgrad(g, dy, packed, dx, st);
-  if (nb_plain_dgrad_ok(g)) return nb_plain_dgrad(g, dy, packed, dx, st);
   int Hv = g->H * g->up, Wv = g->W * g->up;
   bool reflect = g->pad_mode == B200GAN_PAD_REFLECT;
   B2_CHECK_ARG(!(reflect || g->up == 2) || workspace, "conv2d_dgrad: workspace required for reflect / upsample");
@@ -436,17 +462,14 @@ extern "C" int b200gan_conv2d_dgrad(const b200gan_conv_geom *g, const float *dy,
   return B200GAN_OK;
 }
 
-static bool nb_wgrad_routed(const b200gan_conv_geom *g) {
-  // narrow layers only: beyond ~2e10 MACs (wide layers that are not tensor-core shaped) the generic kernel's larger
-  // tiles win
-  return nb_wgrad_ok(g) && (int64_t)g->N * g->P * g->Q * g->K * g->C * g->R * g->S <= (int64_t)2e10;
-}
-
 extern "C" size_t b200gan_conv2d_wgrad_workspace_floats(const b200gan_conv_geom *g, int algo) {
   if (!g) return 0;
-  if (resolve_algo(g, 2, algo) == B200GAN_ALGO_TC) return tc_wgrad_workspace_floats(g);
-  if (fewk_ok(g, 2)) return fewk_wgrad_workspace_floats(g);
-  if (nb_wgrad_routed(g)) return nb_wgrad_workspace_floats(g);
+  switch (wgrad_route(g, algo)) {
+    case WgradRoute::Tc: return tc_wgrad_workspace_floats(g);
+    case WgradRoute::Fewk: return fewk_wgrad_workspace_floats(g);
+    case WgradRoute::Staged: return nb_wgrad_workspace_floats(g);
+    case WgradRoute::Simt: break;
+  }
   return 0;
 }
 
@@ -455,23 +478,26 @@ extern "C" int b200gan_conv2d_wgrad(const b200gan_conv_geom *g, const float *x, 
   if (int e = validate_geom(g)) return e;
   B2_CHECK_ARG(x && dy && dw, "conv2d_wgrad: null pointer");
   cudaStream_t st = as_stream(stream);
-  int a = resolve_algo(g, 2, algo);
-  int rc;
-  if (a == B200GAN_ALGO_TC) {
-    if (!tc_supported(g, 2)) B2_UNSUPPORTED("conv2d_wgrad: geometry not supported by the tensor-core path");
-    rc = tc_wgrad(g, x, dy, dw, workspace, st);
-  } else if (fewk_ok(g, 2)) {
-    // K <= 4 output channels, stride 1 (the image / patch output layers): lanes = input channels
-    rc = fewk_wgrad(g, x, dy, dw, workspace, st);
-  } else if (nb_wgrad_routed(g)) {
-    // narrow layers (C or K small): patch + dy tile staged in shared memory, all taps of a (c, 4k) set in registers
-    rc = nb_wgrad_run(g, nullptr, x, dy, dw, workspace, st);
-  } else if (g->transposed) {
-    rc = simt_wgrad(g->N, g->P, g->Q, g->K, g->H, g->W, g->C, g->R, g->S, g->stride, g->pad_t, g->pad_l,
-                    B200GAN_PAD_ZERO, 1, dy, x, dw, st);
-  } else {
-    rc = simt_wgrad(g->N, g->H, g->W, g->C, g->P, g->Q, g->K, g->R, g->S, g->stride, g->pad_t, g->pad_l,
-                    g->pad_mode, g->up, x, dy, dw, st);
+  int rc = B200GAN_OK;
+  switch (wgrad_route(g, algo)) {
+    case WgradRoute::Tc:
+      if (!tc_supported(g, 2)) B2_UNSUPPORTED("conv2d_wgrad: geometry not supported by the tensor-core path");
+      rc = tc_wgrad(g, x, dy, dw, workspace, st);
+      break;
+    case WgradRoute::Fewk:
+      rc = fewk_wgrad(g, x, dy, dw, workspace, st);
+      break;
+    case WgradRoute::Staged:
+      rc = nb_wgrad_run(g, nullptr, x, dy, dw, workspace, st);
+      break;
+    case WgradRoute::Simt:
+      if (g->transposed)
+        rc = simt_wgrad(g->N, g->P, g->Q, g->K, g->H, g->W, g->C, g->R, g->S, g->stride, g->pad_t, g->pad_l,
+                        B200GAN_PAD_ZERO, 1, dy, x, dw, st);
+      else
+        rc = simt_wgrad(g->N, g->H, g->W, g->C, g->P, g->Q, g->K, g->R, g->S, g->stride, g->pad_t, g->pad_l,
+                        g->pad_mode, g->up, x, dy, dw, st);
+      break;
   }
   if (rc) return rc;
   if (db) return simt_colsum(dy, db, (int64_t)g->N * g->P * g->Q, g->K, st);

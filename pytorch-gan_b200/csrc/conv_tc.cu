@@ -99,7 +99,7 @@ struct TcParams {
   const float *bias;
   const float *chan_scale;
   double *stats;
-  int32_t stats_groups;  // G: ldk (BatchNorm) or N*ldk (InstanceNorm: per-sample groups, tile = one image)
+  int32_t stats_groups;  // G: ldk (BatchNorm) or N*ldk (InstanceNorm: per-sample groups; see tc_setup)
   int32_t stats_per_sample;
   int32_t act;
   float slope;
@@ -650,10 +650,48 @@ conv_tc_up2_allphase_kernel(const __grid_constant__ CUtensorMap tmA, const __gri
 }
 
 // ---- host ----------------------------------------------------------------------------------------
+int conv_stats_pass(const float *y, int N, int HW, int C, int per_sample, double *stats, cudaStream_t st);  // conv_api.cu
+
 static int ilog2_ceil(int v) {
   int l = 0;
   while ((1 << l) < v) ++l;
   return l;
+}
+
+// Set-up shared by run_tc and run_up2_allphase: the 128-pixel tile of an N x Ho x Wo grid per phase (BW x BH pixels
+// of BNn images; returns BNn), the epilogue and the trace.  Per-sample sums fuse only when a tile is one image;
+// otherwise *deferred takes the statistics buffer and the caller runs conv_stats_pass after the conv.
+template <class Params>
+static int tc_setup(Params &p, int N, int Ho, int Wo, int ldk, const b200gan_epilogue *ep, double **deferred) {
+  int bwl = ilog2_ceil(Wo);
+  if (bwl > 7) bwl = 7;
+  int bhl = ilog2_ceil(Ho);
+  if (bhl > 7 - bwl) bhl = 7 - bwl;
+  const int BNn = TC_BM / ((1 << bwl) * (1 << bhl));
+  p.bw_log2 = bwl;
+  p.bh_log2 = bhl;
+  p.tiles_w = ceil_div(Wo, 1 << bwl);
+  p.tiles_h = ceil_div(Ho, 1 << bhl);
+  p.N = N;
+  p.Ho = Ho;
+  p.Wo = Wo;
+  p.ldk = ldk;
+  p.bias = ep ? ep->bias : nullptr;
+  p.chan_scale = ep ? ep->chan_scale : nullptr;
+  p.stats = ep ? ep->stats : nullptr;
+  p.stats_per_sample = ep ? ep->stats_per_sample : 0;
+  p.stats_groups = p.stats_per_sample ? N * ldk : ldk;
+  p.act = ep ? ep->act : 0;
+  p.slope = ep ? ep->slope : 0.f;
+  p.rtf = ep ? ep->round_tf32 : 0;
+  *deferred = nullptr;
+  if (p.stats && p.stats_per_sample && BNn != 1) {
+    *deferred = p.stats;
+    p.stats = nullptr;
+  }
+  p.trace = nullptr;
+  if (const char *tv = getenv("B200GAN_TC_TRACE")) p.trace = reinterpret_cast<long long *>(strtoull(tv, nullptr, 0));
+  return BNn;
 }
 
 template <int BN, int STAGES>
@@ -731,39 +769,19 @@ static int run_tc(const float *in, int N, int Hi, int Wi, int Cc, bool phase_in,
   for (int i = 0; i < total_taps; ++i) p.taps[i] = taps[i];
   p.kout_total = Kout;
   p.kchunks = Cc / TC_BK;
-  int bwl = ilog2_ceil(Wo);
-  if (bwl > 7) bwl = 7;
-  int bhl = ilog2_ceil(Ho);
-  if (bhl > 7 - bwl) bhl = 7 - bwl;
-  const int BW = 1 << bwl, BH = 1 << bhl, BNn = TC_BM / (BW * BH);
-  p.bw_log2 = bwl;
-  p.bh_log2 = bhl;
-  p.tiles_w = ceil_div(Wo, BW);
-  p.tiles_h = ceil_div(Ho, BH);
+  double *deferred_stats;
+  const int BNn = tc_setup(p, N, Ho, Wo, ldk, ep, &deferred_stats);
+  const int BW = 1 << p.bw_log2, BH = 1 << p.bh_log2;
   {
     // 256-wide tiles (A 16 KB + B 32 KB per stage feed 2 x 4 x M64 N256 K8: the 128-channel A box is fetched half as
     // often per output channel) when the layer still gives every SM a CTA
     const int64_t tiles = (int64_t)p.tiles_w * p.tiles_h * ceil_div(N, BNn) * nphase;
     if (Kout % 256 == 0 && tiles * (Kout / 256) >= num_sms()) BN = 256;
   }
-  p.N = N;
-  p.Ho = Ho;
-  p.Wo = Wo;
   for (int i = 0; i < 4; ++i) {
     p.out_dc[i] = i < nphase ? out_dc[i] : 0;
     p.out_da[i] = i < nphase ? out_da[i] : 0;
   }
-  p.ldk = ldk;
-  p.bias = ep ? ep->bias : nullptr;
-  p.chan_scale = ep ? ep->chan_scale : nullptr;
-  p.stats = ep ? ep->stats : nullptr;
-  p.stats_per_sample = ep ? ep->stats_per_sample : 0;
-  p.stats_groups = p.stats_per_sample ? N * ldk : ldk;
-  if (p.stats && p.stats_per_sample && BNn != 1)
-    B2_UNSUPPORTED("tensor-core fprop: per-sample statistics need one image per tile (H*W >= 128 per phase)");
-  p.act = ep ? ep->act : 0;
-  p.slope = ep ? ep->slope : 0.f;
-  p.rtf = ep ? ep->round_tf32 : 0;
   p.y = y;
   p.narrow_k = narrow_k;
   if (narrow_k) {
@@ -771,7 +789,6 @@ static int run_tc(const float *in, int N, int Hi, int Wi, int Cc, bool phase_in,
     B2_CHECK_ARG(!p.chan_scale, "tensor-core conv: Dropout2d scale with fewer than 32 output channels");
   }
   p.ksplit = 1;
-  double *deferred_stats = nullptr;
   if (narrow_k && p.stats) {  // statistics of a narrow layer: separate pass
     deferred_stats = p.stats;
     p.stats = nullptr;
@@ -798,8 +815,6 @@ static int run_tc(const float *in, int N, int Hi, int Wi, int Cc, bool phase_in,
       }
     }
   }
-  p.trace = nullptr;
-  if (const char *tv = getenv("B200GAN_TC_TRACE")) p.trace = reinterpret_cast<long long *>(strtoull(tv, nullptr, 0));
   B2_CHECK_ARG(((uintptr_t)in % 16 == 0) && ((uintptr_t)packedB % 16 == 0) && ((uintptr_t)y % 16 == 0),
                "tensor-core conv: pointers must be 16-byte aligned");
   if (p.ksplit > 1) {
@@ -856,15 +871,8 @@ static int run_tc(const float *in, int N, int Hi, int Wi, int Cc, bool phase_in,
   else if (BN == 128) rc = launch_tc<128, 6>(tmA, tmB, tmY, p, grid, st);
   else if (BN == 64) rc = launch_tc<64, 8>(tmA, tmB, tmY, p, grid, st);
   else rc = launch_tc<32, 8>(tmA, tmB, tmY, p, grid, st);
-  if (rc == B200GAN_OK && deferred_stats) {
-    b200gan_norm_desc nd;
-    memset(&nd, 0, sizeof(nd));
-    nd.N = N;
-    nd.HW = phase_out ? 4 * Ho * Wo : Ho * Wo;
-    nd.C = ldk;
-    nd.per_sample = p.stats_per_sample;
-    rc = b200gan_norm_stats(&nd, y, deferred_stats, st);
-  }
+  if (rc == B200GAN_OK && deferred_stats)
+    rc = conv_stats_pass(y, N, phase_out ? 4 * Ho * Wo : Ho * Wo, ldk, p.stats_per_sample, deferred_stats, st);
   return rc;
 }
 
@@ -878,35 +886,13 @@ static int run_up2_allphase(const float *x, int N, int H, int W, int C, const fl
   for (int i = 0; i < MP_STEPS; ++i) p.steps[i] = sched.s[i];
   p.kout_total = K;
   p.kchunks = C / TC_BK;
-  int bwl = ilog2_ceil(W);
-  if (bwl > 7) bwl = 7;
-  int bhl = ilog2_ceil(H);
-  if (bhl > 7 - bwl) bhl = 7 - bwl;
-  const int BW = 1 << bwl, BH = 1 << bhl, BNn = TC_BM / (BW * BH);
-  p.bw_log2 = bwl;
-  p.bh_log2 = bhl;
-  p.tiles_w = ceil_div(W, BW);
-  p.tiles_h = ceil_div(H, BH);
-  p.N = N;
-  p.Ho = H;
-  p.Wo = W;
+  double *deferred_stats;
+  const int BNn = tc_setup(p, N, H, W, K, ep, &deferred_stats);
+  const int BW = 1 << p.bw_log2, BH = 1 << p.bh_log2;
   for (int ph = 0; ph < 4; ++ph) {
     p.out_dc[ph] = (ph & 1) * K;
     p.out_da[ph] = ph >> 1;
   }
-  p.ldk = K;
-  p.bias = ep ? ep->bias : nullptr;
-  p.chan_scale = ep ? ep->chan_scale : nullptr;
-  p.stats = ep ? ep->stats : nullptr;
-  p.stats_per_sample = ep ? ep->stats_per_sample : 0;
-  p.stats_groups = p.stats_per_sample ? N * K : K;
-  if (p.stats && p.stats_per_sample && BNn != 1)
-    B2_UNSUPPORTED("tensor-core fprop: per-sample statistics need one image per tile (H*W >= 128 per phase)");
-  p.act = ep ? ep->act : 0;
-  p.slope = ep ? ep->slope : 0.f;
-  p.rtf = ep ? ep->round_tf32 : 0;
-  p.trace = nullptr;
-  if (const char *tv = getenv("B200GAN_TC_TRACE")) p.trace = reinterpret_cast<long long *>(strtoull(tv, nullptr, 0));
   B2_CHECK_ARG(((uintptr_t)x % 16 == 0) && ((uintptr_t)packed % 16 == 0) && ((uintptr_t)y % 16 == 0),
                "tensor-core conv: pointers must be 16-byte aligned");
   CUtensorMap tmA, tmB, tmY;
@@ -934,6 +920,7 @@ static int run_up2_allphase(const float *x, int N, int H, int W, int C, const fl
   dim3 grid((unsigned)(p.tiles_w * p.tiles_h * ceil_div(N, BNn)), (unsigned)(K / MP_BN), 1);
   conv_tc_up2_allphase_kernel<<<grid, TC_THREADS, SMEM, st>>>(tmA, tmB, tmY, p);
   B2_LAUNCH_CHECK();
+  if (deferred_stats) return conv_stats_pass(y, N, 4 * H * W, K, p.stats_per_sample, deferred_stats, st);
   return B200GAN_OK;
 }
 

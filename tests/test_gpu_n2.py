@@ -25,8 +25,24 @@ def _penalty(d, x_hat):
     return ((grad.reshape(grad.size(0), -1).norm(2, dim=1) - 1) ** 2).mean(), out
 
 
+def _transposed_critic(ns):
+    # a ConvTranspose2d too narrow for the tensor cores: its data gradient and double backward run the SIMT kernels
+    return ns.Sequential(ns.Conv2d(3, 8, 4, stride=2, padding=1), ns.LeakyReLU(0.01),
+                         ns.ConvTranspose2d(8, 6, 4, stride=2, padding=1), ns.LeakyReLU(0.01),
+                         ns.Conv2d(6, 1, 3, stride=1, padding=1))
+
+
 @pytest.mark.parametrize("algo", ["simt", "auto"])
 def test_conv_critic_gradient_penalty(algo):
+    _check_gradient_penalty(_critic, algo)
+
+
+@pytest.mark.parametrize("algo", ["simt", "auto"])
+def test_transposed_conv_critic_gradient_penalty(algo):
+    _check_gradient_penalty(_transposed_critic, algo)
+
+
+def _check_gradient_penalty(make_critic, algo):
     import b200gan
     from b200gan import zoo
     torch.backends.cudnn.allow_tf32 = False
@@ -34,8 +50,8 @@ def test_conv_critic_gradient_penalty(algo):
     prev = b200gan.Config.algo
     b200gan.Config.algo = algo
     try:
-        ref = _critic(zoo.namespace(stock=True)).cuda()
-        ours = _critic(zoo.namespace()).cuda()
+        ref = make_critic(zoo.namespace(stock=True)).cuda()
+        ours = make_critic(zoo.namespace()).cuda()
         ours.load_state_dict(ref.state_dict())
         x = torch.randn(4, 3, 32, 32, device="cuda")
         res = []

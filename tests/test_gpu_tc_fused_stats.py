@@ -1,6 +1,7 @@
 """Fused BatchNorm / InstanceNorm statistics of the wgmma convolutions at sizes with more output tiles than an H100 has
 SMs (ragged maps, one image per tile, 256-wide tiles, the all-phase Upsample(2x)+Conv3x3 kernel), with bias, LeakyReLU
-and a Dropout2d scale in the same epilogue, against fp32 torch."""
+and a Dropout2d scale in the same epilogue, against fp32 torch.  Per-sample sums are also returned when a 128-pixel
+tile spans several images (the library then adds a statistics pass)."""
 import pytest
 import torch
 import torch.nn.functional as F
@@ -36,6 +37,10 @@ CASES = [
     # folded Upsample(2x)+Conv3x3 with 64 output channels: the all-phase kernel, per-sample sums over four phases
     ("allphase_instancenorm", 128, 128, 64, 16, 16, 2, True, True),
     ("allphase_batchnorm", 128, 128, 64, 32, 32, 2, False, False),
+    # 8x8 map: a tile holds two images, so per-sample sums cannot be fused into the epilogue
+    ("instancenorm_tile_spans_images", 512, 64, 64, 8, 8, 1, True, False),
+    # all-phase kernel at 4x4 per phase: eight images per tile
+    ("allphase_instancenorm_tile_spans_images", 2048, 128, 64, 4, 4, 2, True, True),
 ]
 
 

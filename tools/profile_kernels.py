@@ -12,8 +12,6 @@ sys.path.insert(0, os.path.join(ROOT, "pytorch-gan_b200"))
 import torch  # noqa: E402
 
 from b200gan import ops  # noqa: E402
-from b200gan._lib import (ALGO_AUTO, ALGO_SIMT, ALGO_TC, PACK_SIMT_DGRAD, PACK_SIMT_FPROP, PACK_TC_DGRAD,  # noqa: E402
-                          PACK_TC_DGRAD_UP2, PACK_TC_FPROP, PACK_TC_FPROP_UP2)
 
 CL = torch.channels_last
 
@@ -65,18 +63,15 @@ def main():
         act_bytes = (x.numel() + dy.numel()) * 4
         for pas, pname in ((0, "fprop"), (1, "dgrad"), (2, "wgrad")):
             tc = ops.tc_supported(g, pas)
+            algo, kind = ops.conv_plan(g, pas)
             if pas == 0:
-                algo = ALGO_TC if tc else ALGO_SIMT
-                kind = (PACK_TC_FPROP_UP2 if up == 2 else PACK_TC_FPROP) if tc else PACK_SIMT_FPROP
                 packed = ops.pack_weights(g, wt, kind)
                 fn = lambda: ops.conv_fprop(g, x, packed, algo)  # noqa: E731
             elif pas == 1:
-                algo = ALGO_TC if tc else ALGO_SIMT
-                kind = (PACK_TC_DGRAD_UP2 if up == 2 else PACK_TC_DGRAD) if tc else PACK_SIMT_DGRAD
                 packed = ops.pack_weights(g, wt, kind)
                 fn = lambda: ops.conv_dgrad(g, dy, packed, algo)  # noqa: E731
             else:
-                fn = lambda: ops.conv_wgrad(g, x, dy, tuple(wt.shape), True, ALGO_AUTO)  # noqa: E731
+                fn = lambda: ops.conv_wgrad(g, x, dy, tuple(wt.shape), True, algo)  # noqa: E731
             ms = timeit(fn, a.iters)
             fl = flops_exec if tc else flops_ref
             rows.append((name, pname, "wgmma" if tc else "simt", ms * 1e3, fl / ms / 1e9, act_bytes / ms / 1e6))
