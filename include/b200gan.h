@@ -277,6 +277,50 @@ int b200gan_critic_step_mlp(const b200gan_gp_mlp_desc *d, const float *real, con
                             const float *b3, float *losses, float *dW1, float *db1, float *dW2, float *db2, float *dW3,
                             float *db3, float *workspace, void *stream);
 
+/* ---- MLP critic under autograd: forward, backward, double backward of the input gradient --- */
+/* The same critic D(x) = W3 lrelu(W2 lrelu(W1 x + b1) + b2) + b3, Din -> H1 -> H2 -> 1, one LeakyReLU
+ * slope for both activations, as three generic passes with no penalty built in, so that a script's own
+ * autograd.grad(create_graph=True) penalty (wgan_gp.py:125-137, wgan_div.py:143-163) runs every critic GEMM
+ * here (csrc/mlp_critic.cu).  Each is ONE cooperative launch; any N, Din, H1, H2 >= 1; all outputs are
+ * OVERWRITTEN, never accumulated.  Weights in torch layout: W1[H1][Din], W2[H2][H1], W3[H2], b3[1]. */
+typedef struct b200gan_mlp_critic_desc {
+  int32_t N, Din, H1, H2;
+  float slope;
+} b200gan_mlp_critic_desc;
+/* Forward, x[N][Din]:
+ *   h1 = x W1^T + b1,  m1 = (h1 > 0 ? 1 : slope),  a1 = h1 * m1          m1, a1: [N][H1]
+ *   h2 = a1 W2^T + b2, m2 = (h2 > 0 ? 1 : slope),  a2 = h2 * m2          m2, a2: [N][H2]
+ *   out[n] = a2[n] . W3 + b3
+ * m1, a1, m2, a2 are kept for the two backward passes.  No workspace. */
+int b200gan_mlp_critic_fwd(const b200gan_mlp_critic_desc *d, const float *x, const float *W1,
+                           const float *b1, const float *W2, const float *b2, const float *W3,
+                           const float *b3, float *out, float *m1, float *a1, float *m2, float *a2,
+                           void *stream);
+/* First-order backward for the output gradient dout[N]:
+ *   U2 = dout W3 * m2  [N][H2],   U1 = (U2 W2) * m1  [N][H1],   dx = U1 W1  [N][Din]
+ *   dW1 = U1^T x,  dW2 = U2^T a1,  dW3 = dout^T a2,  db1 = sum_n U1,  db2 = sum_n U2,  db3 = sum_n dout.
+ * Every output (dx, dW1, db1, dW2, db2, dW3, db3) may be NULL and is then not computed; x, a1, a2 and W1
+ * are read only for dW1, dW2, dW3 and dx respectively and may otherwise be NULL.  U1, U2: written when
+ * non-NULL (the double backward needs them); when either is NULL `workspace` must hold
+ * b200gan_mlp_critic_bwd_workspace_floats() floats. */
+size_t b200gan_mlp_critic_bwd_workspace_floats(const b200gan_mlp_critic_desc *d);
+int b200gan_mlp_critic_bwd(const b200gan_mlp_critic_desc *d, const float *dout, const float *x,
+                           const float *W1, const float *W2, const float *W3, const float *m1,
+                           const float *a1, const float *m2, const float *a2, float *dx, float *dW1,
+                           float *db1, float *dW2, float *db2, float *dW3, float *db3, float *U1,
+                           float *U2, float *workspace, void *stream);
+/* Double backward of dx = U1 W1 for the gradient u[N][Din] arriving at dx.  The masks are piecewise
+ * constant (LeakyReLU'' = 0 almost everywhere), so:
+ *   dW1 = U1^T u;   t = (u W1^T) * m1;   dW2 = U2^T t;   s = (t W2^T) * m2;
+ *   dW3 = sum_n dout_n s_n;   ddout[n] = s_n . W3   (the gradient w.r.t. dout).
+ * The gradients w.r.t. x and the biases are exactly zero and not produced.  dW1, dW2, dW3, ddout may be
+ * NULL (not computed).  workspace: b200gan_mlp_critic_dbwd_workspace_floats() floats. */
+size_t b200gan_mlp_critic_dbwd_workspace_floats(const b200gan_mlp_critic_desc *d);
+int b200gan_mlp_critic_dbwd(const b200gan_mlp_critic_desc *d, const float *u, const float *dout,
+                            const float *U1, const float *U2, const float *m1, const float *m2,
+                            const float *W1, const float *W2, const float *W3, float *dW1, float *dW2,
+                            float *dW3, float *ddout, float *workspace, void *stream);
+
 /* ---- flat-buffer Adam (torch.optim.Adam semantics: dcgan.py:134-135) --------------------- */
 /* p -= lr * mhat / (sqrt(vhat) + eps), bias-corrected with the step count read from the
  * device (step[0] is incremented by the kernel -> CUDA-graph capturable).  lr, betas and eps

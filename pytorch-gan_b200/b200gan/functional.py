@@ -678,3 +678,64 @@ def critic_step_mlp(critic_layers, real, fake, alpha, lambda_gp):
     l1, l2, l3 = mods[0], mods[2], mods[4]
     return CriticStepMLPFn.apply(real, fake, alpha, l1.weight, l1.bias, l2.weight, l2.bias, l3.weight, l3.bias,
                                  float(mods[1].negative_slope), float(lambda_gp))
+
+
+# ---- the MLP critic under autograd (csrc/mlp_critic.cu) ------------------------------------------------------------
+class MlpCriticFn(torch.autograd.Function):
+    """D(x) = W3 lrelu(W2 lrelu(W1 x + b1) + b2) + b3 (wgan_gp.py:72-78, wgan_div.py:72-78): one launch forward, one
+    launch backward.  Under autograd.grad(..., create_graph=True) -- a gradient penalty the script computes itself
+    (wgan_gp.py:125-137, wgan_div.py:143-163) -- the backward is the differentiable node MlpCriticGradFn, whose own
+    backward is one more launch, so the penalty's double backward never leaves the fused kernels."""
+
+    @staticmethod
+    def forward(ctx, x, w1, b1, w2, b2, w3, b3, slope):
+        out, m1, a1, m2, a2 = ops.mlp_critic_fwd(x.detach(), *[t.detach() for t in (w1, b1, w2, b2, w3, b3)], slope)
+        ctx.save_for_backward(x, w1, w2, w3, m1, a1, m2, a2)
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        x, w1, w2, w3, m1, a1, m2, a2 = ctx.saved_tensors
+        need = tuple(ctx.needs_input_grad[:7])
+        if torch.is_grad_enabled():
+            return MlpCriticGradFn.apply(dout, x, w1, w2, w3, m1, a1, m2, a2, need) + (None,)
+        grads = ops.mlp_critic_bwd(dout, x.detach(), w1.detach(), w2.detach(), w3.detach(), m1, a1, m2, a2, need)
+        return (*grads[:7], None)
+
+
+class MlpCriticGradFn(torch.autograd.Function):
+    """The first-order backward of MlpCriticFn as a differentiable function of (dout, W1, W2, W3): outputs the
+    gradients w.r.t. (x, W1, b1, W2, b2, W3, b3) that `need` asks for (None for the rest).  Only the input gradient
+    dx = dD/dx may be differentiated again (a gradient penalty); its backward is the closed-form double backward, in
+    which x and the biases get exactly zero."""
+
+    @staticmethod
+    def forward(ctx, dout, x, w1, w2, w3, m1, a1, m2, a2, need):
+        ctx.set_materialize_grads(False)  # outputs nothing depends on arrive as None, not as zero-filled tensors
+        grads = ops.mlp_critic_bwd(dout.detach(), x.detach(), w1.detach(), w2.detach(), w3.detach(), m1, a1, m2, a2,
+                                   need, keep_u=True)
+        ctx.save_for_backward(dout, w1, w2, w3, m1, m2, grads[7], grads[8])
+        return grads[:7]
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, gx, *gparams):
+        if any(g is not None for g in gparams):
+            raise NotImplementedError("b200gan: the MLP critic's parameter gradients were differentiated (a penalty on "
+                                      "parameter gradients); only its input gradient dD/dx is differentiable")
+        none = (None,) * 10
+        nig = ctx.needs_input_grad
+        need = (nig[0], nig[2], nig[3], nig[4])
+        if gx is None or not any(need):
+            return none
+        dout, w1, w2, w3, m1, m2, u1, u2 = ctx.saved_tensors
+        ddout, dw1, dw2, dw3 = ops.mlp_critic_dbwd(gx, dout.detach(), u1, u2, m1, m2, w1.detach(), w2.detach(),
+                                                   w3.detach(), need)
+        if ddout is not None:
+            ddout = ddout.view(dout.shape)
+        return (ddout, None, dw1, dw2, dw3) + none[5:]
+
+
+def mlp_critic(x, l1, l2, l3, slope):
+    """Linear l1 -> LeakyReLU(slope) -> Linear l2 -> LeakyReLU(slope) -> Linear l3 (-> 1) on x [N, Din] as MlpCriticFn."""
+    return MlpCriticFn.apply(x, l1.weight, l1.bias, l2.weight, l2.bias, l3.weight, l3.bias, float(slope))

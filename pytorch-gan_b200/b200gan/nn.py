@@ -268,11 +268,13 @@ def _gpu2d_f32(x):
 
 
 class Linear(_T["Linear"]):
-    """nn.Linear.  Inside a Sequential, Linear(K, 1) + Sigmoid -- the head of a discriminator (dcgan.py:92) -- runs as
-    one b200gan kernel per direction (Sequential._forward_2d); on its own it is a plain library GEMM and stays on
-    torch/cuBLAS (wgan_gp.py:46-60,72-78; dcgan.py:50), which also keeps the critic of wgan_gp.py double-differentiable
-    for the script's own autograd.grad(create_graph=True).  A wide output (>= 8192 features: the generator's first
-    layer, dcgan.py:50) uses the TF32 library GEMM like the convolutions behind it."""
+    """nn.Linear.  Inside a Sequential (Sequential._forward_2d), two patterns run as b200gan kernels: Linear(K, 1) +
+    Sigmoid/Tanh -- the head of a discriminator (dcgan.py:92) -- as one kernel per direction, and the whole MLP critic
+    Linear -> LeakyReLU -> Linear -> LeakyReLU -> Linear(-> 1) of wgan_gp.py:72-78 / wgan_div.py:72-78 as one
+    cooperative kernel per pass, double-differentiable for the script's own autograd.grad(create_graph=True)
+    (functional.MlpCriticFn).  Anywhere else it is a plain library GEMM and stays on torch/cuBLAS (wgan_gp.py:46-60;
+    dcgan.py:50).  A wide output (>= 8192 features: the generator's first layer, dcgan.py:50) uses the TF32 library
+    GEMM like the convolutions behind it."""
 
     def forward(self, x):
         if _gpu2d_f32(x) and self.out_features >= 8192 and ops.Config.algo != "simt":
@@ -516,6 +518,28 @@ def _build_plan(mods):
     return fused
 
 
+def mlp_critic_layers(mods, in_features):
+    """(Linear 1, Linear 2, Linear 3, slope) if the module list `mods` is exactly the MLP critic of wgan_gp.py:72-78 /
+    wgan_div.py:72-78 -- Linear(in_features, H1) -> LeakyReLU(s) -> Linear(H1, H2) -> LeakyReLU(s) -> Linear(H2, 1), all
+    with biases, one slope -- which runs as functional.MlpCriticFn; else None.  No side effects."""
+    def plain(m, name):  # the stock class or its drop-in, with no hooks that calling the module would run
+        return (type(m) in (_T[name], REPLACEMENTS[name]) and not m._forward_hooks and not m._forward_pre_hooks
+                and not m._backward_hooks)
+
+    if len(mods) != 5 or not all(plain(mods[i], "Linear") for i in (0, 2, 4)):
+        return None
+    if not all(plain(mods[i], "LeakyReLU") for i in (1, 3)):
+        return None
+    l1, l2, l3 = mods[0], mods[2], mods[4]
+    if any(m.bias is None for m in (l1, l2, l3)) or mods[1].negative_slope != mods[3].negative_slope:
+        return None
+    if l1.in_features != in_features or l2.in_features != l1.out_features or l3.in_features != l2.out_features:
+        return None
+    if l3.out_features != 1:
+        return None
+    return l1, l2, l3, float(mods[1].negative_slope)
+
+
 class Sequential(_T["Sequential"]):
     def _plan(self):
         mods = list(self._modules.values())
@@ -584,8 +608,12 @@ class Sequential(_T["Sequential"]):
         return x
 
     def _forward_2d(self, x):
-        """Matrix input (the adv_layer of a discriminator, dcgan.py:92): Linear(K, 1) + activation as one node."""
+        """Matrix input: the whole MLP critic (wgan_gp.py:72-78) as one node, or Linear(K, 1) + activation (the adv_layer
+        of a discriminator, dcgan.py:92) as one node."""
         mods = list(self._modules.values())
+        critic = mlp_critic_layers(mods, x.shape[1])
+        if critic is not None and x.shape[0] >= 1:
+            return F.mlp_critic(x, *critic)
         i = 0
         while i < len(mods):
             m = mods[i]

@@ -12,7 +12,7 @@ import torch
 from . import _lib
 from ._lib import (ACT_NONE, ALGO_AUTO, ALGO_SIMT, ALGO_TC, PACK_SIMT_DGRAD, PACK_SIMT_FPROP, PACK_TC_DGRAD,
                    PACK_TC_DGRAD_UP2, PACK_TC_FPROP, PACK_TC_FPROP_UP2, PAD_REFLECT, PAD_ZERO, ConvGeom, Epilogue,
-                   GpMlpDesc, NbBn, NormDesc, TailDesc)
+                   GpMlpDesc, MlpCriticDesc, NbBn, NormDesc, TailDesc)
 
 CL = torch.channels_last
 
@@ -581,3 +581,81 @@ def critic_step_mlp(real, fake, alpha, w1, b1, w2, b2, w3, b3, slope, lambda_gp)
                                            b3.data_ptr(), losses.data_ptr(), *[g.data_ptr() for g in grads],
                                            ws.data_ptr(), _stream()), "critic_step_mlp")
     return (losses, *grads)
+
+
+# ---- MLP critic under autograd: Linear -> LeakyReLU -> Linear -> LeakyReLU -> Linear(-> 1) (csrc/mlp_critic.cu) ------
+def _mlp_critic_desc(x, w1, w2, w3, slope):
+    if x.dim() != 2 or w1.dim() != 2 or w2.dim() != 2:
+        raise RuntimeError("b200gan mlp_critic: x, W1 and W2 must be matrices")
+    d = MlpCriticDesc()
+    d.N, d.Din, d.H1, d.H2, d.slope = x.shape[0], x.shape[1], w1.shape[0], w2.shape[0], float(slope)
+    if w1.shape[1] != d.Din or w2.shape[1] != d.H1 or w3.numel() != d.H2 or min(d.N, d.Din, d.H1, d.H2) < 1:
+        raise RuntimeError(f"b200gan mlp_critic: shapes do not chain: x {tuple(x.shape)}, W1 {tuple(w1.shape)}, "
+                           f"W2 {tuple(w2.shape)}, W3 {tuple(w3.shape)}")
+    return d
+
+
+def _f32(name, *ts):
+    for t_ in ts:
+        if t_ is not None:
+            _require_cuda(t_, name)
+    return [None if t_ is None else t_.contiguous() for t_ in ts]
+
+
+def mlp_critic_fwd(x, w1, b1, w2, b2, w3, b3, slope):
+    """D(x) in one launch.  Returns (out [N, 1], m1, a1, m2, a2): the LeakyReLU masks and activations of both hidden
+    layers, which the two backward passes read (see b200gan_mlp_critic_fwd in include/b200gan.h)."""
+    x, w1, b1, w2, b2, w3, b3 = _f32("mlp_critic operand", x, w1, b1, w2, b2, w3, b3)
+    d = _mlp_critic_desc(x, w1, w2, w3, slope)
+    if b1.numel() != d.H1 or b2.numel() != d.H2 or b3.numel() != 1:
+        raise RuntimeError("b200gan mlp_critic: bias sizes do not match the layers")
+    dev, n = x.device, d.N
+    out = torch.empty((n, 1), device=dev, dtype=torch.float32)
+    m1, a1 = (torch.empty((n, d.H1), device=dev, dtype=torch.float32) for _ in range(2))
+    m2, a2 = (torch.empty((n, d.H2), device=dev, dtype=torch.float32) for _ in range(2))
+    _lib.check(_lib.load().b200gan_mlp_critic_fwd(ctypes.byref(d), x.data_ptr(), w1.data_ptr(), b1.data_ptr(),
+                                                  w2.data_ptr(), b2.data_ptr(), w3.data_ptr(), b3.data_ptr(),
+                                                  out.data_ptr(), m1.data_ptr(), a1.data_ptr(), m2.data_ptr(),
+                                                  a2.data_ptr(), _stream()), "mlp_critic_fwd")
+    return out, m1, a1, m2, a2
+
+
+def mlp_critic_bwd(dout, x, w1, w2, w3, m1, a1, m2, a2, need, keep_u=False):
+    """First-order backward for the output gradient dout [N, 1].  need: 7 flags for the gradients of
+    (x, W1, b1, W2, b2, W3, b3); the others come back as None.  Returns (dx, dW1, db1, dW2, db2, dW3, db3, U1, U2), with
+    U1 [N, H1] and U2 [N, H2] (the double backward's operands) only when keep_u."""
+    dout, x, w1, w2, w3, m1, a1, m2, a2 = _f32("mlp_critic operand", dout, x, w1, w2, w3, m1, a1, m2, a2)
+    d = _mlp_critic_desc(x, w1, w2, w3, 0.0)  # the masks carry the slope
+    if dout.numel() != d.N or m1.shape != (d.N, d.H1) or m2.shape != (d.N, d.H2):
+        raise RuntimeError("b200gan mlp_critic_bwd: dout / saved activations do not match the layers")
+    lib, dev, f32 = _lib.load(), x.device, torch.float32
+    shapes = ((d.N, d.Din), tuple(w1.shape), (d.H1,), tuple(w2.shape), (d.H2,), tuple(w3.shape), (1,))
+    grads = [torch.empty(s_, device=dev, dtype=f32) if nd else None for s_, nd in zip(shapes, need)]
+    u1 = torch.empty((d.N, d.H1), device=dev, dtype=f32) if keep_u else None
+    u2 = torch.empty((d.N, d.H2), device=dev, dtype=f32) if keep_u else None
+    ws = None if keep_u else torch.empty(lib.b200gan_mlp_critic_bwd_workspace_floats(ctypes.byref(d)), device=dev,
+                                         dtype=f32)
+    _lib.check(lib.b200gan_mlp_critic_bwd(ctypes.byref(d), dout.data_ptr(), x.data_ptr(), w1.data_ptr(), w2.data_ptr(),
+                                          w3.data_ptr(), m1.data_ptr(), a1.data_ptr(), m2.data_ptr(), a2.data_ptr(),
+                                          *[_ptr(g) for g in grads], _ptr(u1), _ptr(u2), _ptr(ws), _stream()),
+               "mlp_critic_bwd")
+    return (*grads, u1, u2)
+
+
+def mlp_critic_dbwd(u, dout, u1, u2, m1, m2, w1, w2, w3, need):
+    """Double backward of the input gradient dx = U1 W1 for the gradient u [N, Din] arriving at dx.  need: 4 flags for
+    the gradients of (dout, W1, W2, W3).  Returns (ddout [N, 1], dW1, dW2, dW3), None where not needed; the gradients
+    w.r.t. x and the biases are exactly zero."""
+    u, dout, u1, u2, m1, m2, w1, w2, w3 = _f32("mlp_critic operand", u, dout, u1, u2, m1, m2, w1, w2, w3)
+    d = _mlp_critic_desc(u, w1, w2, w3, 0.0)
+    if dout.numel() != d.N or u1.shape != (d.N, d.H1) or u2.shape != (d.N, d.H2):
+        raise RuntimeError("b200gan mlp_critic_dbwd: operands do not match the layers")
+    lib, dev, f32 = _lib.load(), u.device, torch.float32
+    shapes = ((d.N, 1), tuple(w1.shape), tuple(w2.shape), tuple(w3.shape))
+    ddout, dw1, dw2, dw3 = [torch.empty(s_, device=dev, dtype=f32) if nd else None for s_, nd in zip(shapes, need)]
+    ws = torch.empty(lib.b200gan_mlp_critic_dbwd_workspace_floats(ctypes.byref(d)), device=dev, dtype=f32)
+    _lib.check(lib.b200gan_mlp_critic_dbwd(ctypes.byref(d), u.data_ptr(), dout.data_ptr(), u1.data_ptr(), u2.data_ptr(),
+                                           m1.data_ptr(), m2.data_ptr(), w1.data_ptr(), w2.data_ptr(), w3.data_ptr(),
+                                           _ptr(dw1), _ptr(dw2), _ptr(dw3), _ptr(ddout), ws.data_ptr(), _stream()),
+               "mlp_critic_dbwd")
+    return ddout, dw1, dw2, dw3
