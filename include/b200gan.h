@@ -55,7 +55,8 @@ enum {
   B200GAN_PACK_SIMT_FPROP = 0, /* [R][S][Cin][Cout]   : fprop (Conv2d and ConvTranspose2d), SIMT */
   B200GAN_PACK_SIMT_DGRAD = 1, /* [R][S][Cout][Cin]   : dgrad (Conv2d and ConvTranspose2d), SIMT */
   B200GAN_PACK_TC_FPROP = 2,   /* [R*S][Cout][Cin]    tf32-rounded, K-major, wgmma fprop      */
-  B200GAN_PACK_TC_DGRAD = 3,   /* [R*S][Cin][Cout]    tf32-rounded, taps flipped, dgrad       */
+  B200GAN_PACK_TC_DGRAD = 3,   /* [R*S][Cin][Cout]    tf32-rounded, taps in filter order (the
+                                  scatter form's tap offsets do the flip), dgrad               */
   B200GAN_PACK_TC_FPROP_UP2 = 4, /* [4 phases][4 taps][Cout][Cin]: 3x3 s1 p1 conv folded with a
                                     preceding nearest x2 upsample into four 2x2 phase filters  */
   B200GAN_PACK_TC_DGRAD_UP2 = 5  /* [4 phases][4 taps][Cin][Cout]: its data gradient           */

@@ -64,9 +64,13 @@ __device__ __forceinline__ void nb_update_running(const NbBn &bn, int C, int c, 
   rv[c] = v_run;
 }
 
+// every activation of the epilogue: the staged forward also runs b200gan_conv2d_fprop layers (nb_plain_fprop), whose
+// epilogue may end in Tanh or Sigmoid
 __device__ __forceinline__ float nb_act(float v, int act, float slope) {
   if (act == B200GAN_ACT_LRELU) return v > 0.f ? v : v * slope;
   if (act == B200GAN_ACT_RELU) return fmaxf(v, 0.f);
+  if (act == B200GAN_ACT_TANH) return tanhf(v);
+  if (act == B200GAN_ACT_SIGMOID) return 1.f / (1.f + expf(-v));
   return v;
 }
 __device__ __forceinline__ float nb_act_grad(float a, int act, float slope) {
