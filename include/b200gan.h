@@ -248,37 +248,7 @@ int b200gan_pad2d_bwd(const float *dy, float *dx, int32_t N, int32_t H, int32_t 
 int b200gan_act_fwd(const float *x, const float *mask, int32_t mask_per_channel, int32_t act,
                     float slope, int64_t n, int32_t C, int64_t HW, float *y, void *stream);
 
-/* ---- WGAN-GP critic: whole gradient-penalty double backward in one kernel --------------- */
-/* Critic D(x) = W3 lrelu(W2 lrelu(W1 x + b1) + b2) + b3  (wgan_gp.py:72-78), Din -> H1 -> H2 -> 1.
- * Computes, for interpolates xi[N][Din] (wgan_gp.py:124):
- *   gp = mean_n (||dD/dxi||_2 - 1)^2                                  (wgan_gp.py:128-137)
- * and, scaled by `lambda_gp` (wgan_gp.py:87,171), its gradient w.r.t. W1, W2, W3 -- the closed
- * form of autograd's double backward (SURVEY.md section 8a row a7); biases get zero gradient.
- * Outputs are OVERWRITTEN: gp[1], dW1[H1][Din], dW2[H2][H1], dW3[H2].
- * workspace: b200gan_gp_mlp_workspace_floats() floats. */
-typedef struct b200gan_gp_mlp_desc {
-  int32_t N, Din, H1, H2;
-  float slope;
-  float lambda_gp;
-} b200gan_gp_mlp_desc;
-size_t b200gan_gp_mlp_workspace_floats(const b200gan_gp_mlp_desc *d);
-int b200gan_gp_mlp_fwd_bwd(const b200gan_gp_mlp_desc *d, const float *xi, const float *W1,
-                           const float *b1, const float *W2, const float *b2, const float *W3,
-                           float *gp, float *dW1, float *dW2, float *dW3, float *workspace,
-                           void *stream);
-
-/* The whole critic iteration of wgan_gp.py:164-173 for the MLP critic in ONE cooperative kernel:
- *   losses[0] = -mean(D(real)) + mean(D(fake)) + lambda * gp,   losses[1] = lambda * gp,
- * with the interpolates alpha * real + (1 - alpha) * fake formed inside (alpha [N], wgan_gp.py:122-124), and the
- * gradient of losses[0] w.r.t. every parameter of D (all OVERWRITTEN): first-order backward of the real / fake passes and
- * the closed-form double backward of the penalty share their GEMMs (csrc/gp_mlp.cu).  real, fake: [N][Din]. */
-size_t b200gan_critic_step_workspace_floats(const b200gan_gp_mlp_desc *d);
-int b200gan_critic_step_mlp(const b200gan_gp_mlp_desc *d, const float *real, const float *fake, const float *alpha,
-                            const float *W1, const float *b1, const float *W2, const float *b2, const float *W3,
-                            const float *b3, float *losses, float *dW1, float *db1, float *dW2, float *db2, float *dW3,
-                            float *db3, float *workspace, void *stream);
-
-/* ---- MLP critic under autograd: forward, backward, double backward of the input gradient --- */
+/* ---- MLP critic: forward, backward, double backward of the input gradient; WGAN-GP critic step */
 /* The same critic D(x) = W3 lrelu(W2 lrelu(W1 x + b1) + b2) + b3, Din -> H1 -> H2 -> 1, one LeakyReLU
  * slope for both activations, as three generic passes with no penalty built in, so that a script's own
  * autograd.grad(create_graph=True) penalty (wgan_gp.py:125-137, wgan_div.py:143-163) runs every critic GEMM
@@ -321,6 +291,17 @@ int b200gan_mlp_critic_dbwd(const b200gan_mlp_critic_desc *d, const float *u, co
                             const float *U1, const float *U2, const float *m1, const float *m2,
                             const float *W1, const float *W2, const float *W3, float *dW1, float *dW2,
                             float *dW3, float *ddout, float *workspace, void *stream);
+/* The whole WGAN-GP critic iteration of wgan_gp.py:164-173 for this critic in ONE cooperative kernel:
+ *   losses[0] = -mean(D(real)) + mean(D(fake)) + lambda_gp * gp,   losses[1] = lambda_gp * gp,
+ *   gp = mean_n (||dD/dx_n||_2 - 1)^2 at the interpolates x = alpha * real + (1 - alpha) * fake, formed inside
+ * (alpha [N], wgan_gp.py:122-137), and the gradient of losses[0] w.r.t. every parameter of D (all OVERWRITTEN): the
+ * first-order backward of the real / fake passes and the closed-form double backward of the penalty share their GEMMs.
+ * real, fake: [N][Din].  workspace: b200gan_critic_step_workspace_floats() floats. */
+size_t b200gan_critic_step_workspace_floats(const b200gan_mlp_critic_desc *d);
+int b200gan_critic_step_mlp(const b200gan_mlp_critic_desc *d, float lambda_gp, const float *real, const float *fake,
+                            const float *alpha, const float *W1, const float *b1, const float *W2, const float *b2,
+                            const float *W3, const float *b3, float *losses, float *dW1, float *db1, float *dW2,
+                            float *db2, float *dW3, float *db3, float *workspace, void *stream);
 
 /* ---- flat-buffer Adam (torch.optim.Adam semantics: dcgan.py:134-135) --------------------- */
 /* p -= lr * mhat / (sqrt(vhat) + eps), bias-corrected with the step count read from the

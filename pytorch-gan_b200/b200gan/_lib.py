@@ -37,11 +37,6 @@ class NormDesc(ctypes.Structure):
                 ("momentum", c_f32), ("act", c_i32), ("slope", c_f32), ("round_tf32", c_i32)]
 
 
-class GpMlpDesc(ctypes.Structure):
-    _fields_ = [("N", c_i32), ("Din", c_i32), ("H1", c_i32), ("H2", c_i32), ("slope", c_f32),
-                ("lambda_gp", c_f32)]
-
-
 class MlpCriticDesc(ctypes.Structure):
     _fields_ = [("N", c_i32), ("Din", c_i32), ("H1", c_i32), ("H2", c_i32), ("slope", c_f32)]
 
@@ -96,15 +91,13 @@ SIGNATURES = {
     "b200gan_pad2d_fwd": (c_i32, [c_vp, c_vp] + [c_i32] * 10 + [c_vp]),
     "b200gan_pad2d_bwd": (c_i32, [c_vp, c_vp] + [c_i32] * 9 + [c_vp]),
     "b200gan_act_fwd": (c_i32, [c_vp, c_vp, c_i32, c_i32, c_f32, c_i64, c_i32, c_i64, c_vp, c_vp]),
-    "b200gan_gp_mlp_workspace_floats": (c_sz, [_P(GpMlpDesc)]),
-    "b200gan_gp_mlp_fwd_bwd": (c_i32, [_P(GpMlpDesc)] + [c_vp] * 12),
-    "b200gan_critic_step_workspace_floats": (c_sz, [_P(GpMlpDesc)]),
-    "b200gan_critic_step_mlp": (c_i32, [_P(GpMlpDesc)] + [c_vp] * 18),
     "b200gan_mlp_critic_fwd": (c_i32, [_P(MlpCriticDesc)] + [c_vp] * 13),
     "b200gan_mlp_critic_bwd_workspace_floats": (c_sz, [_P(MlpCriticDesc)]),
     "b200gan_mlp_critic_bwd": (c_i32, [_P(MlpCriticDesc)] + [c_vp] * 20),
     "b200gan_mlp_critic_dbwd_workspace_floats": (c_sz, [_P(MlpCriticDesc)]),
     "b200gan_mlp_critic_dbwd": (c_i32, [_P(MlpCriticDesc)] + [c_vp] * 15),
+    "b200gan_critic_step_workspace_floats": (c_sz, [_P(MlpCriticDesc)]),
+    "b200gan_critic_step_mlp": (c_i32, [_P(MlpCriticDesc), c_f32] + [c_vp] * 18),
     "b200gan_adam_step": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_i64, c_f64, c_f64, c_f64, c_f64, c_f32, c_vp, c_vp]),
     "b200gan_nb_supported": (c_i32, [_P(ConvGeom)]),
     "b200gan_nb_groups_supported": (c_i32, [_P(ConvGeom), c_i32]),

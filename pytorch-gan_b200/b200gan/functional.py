@@ -618,37 +618,6 @@ def norm_block(x, gamma, beta, stats, running_mean, running_var, nbt, spec):
     return NormFn.apply(x, gamma, beta, stats, running_mean, running_var, nbt, spec)
 
 
-class GradientPenaltyMLPFn(torch.autograd.Function):
-    """lambda * mean((||dD/dx||_2 - 1)^2) for the MLP critic D = L3(lrelu(L2(lrelu(L1 x)))) with the
-    gradient w.r.t. the weights produced in the same kernel (closed-form double backward)."""
-
-    @staticmethod
-    def forward(ctx, xi, w1, b1, w2, b2, w3, slope, lambda_gp):
-        gp, dw1, dw2, dw3 = ops.gp_mlp_fwd_bwd(xi.detach(), w1.detach().contiguous(), b1.detach().contiguous(),
-                                               w2.detach().contiguous(), b2.detach().contiguous(),
-                                               w3.detach().contiguous(), slope, lambda_gp)
-        ctx.save_for_backward(dw1, dw2, dw3)
-        return gp
-
-    @staticmethod
-    def backward(ctx, g):
-        dw1, dw2, dw3 = ctx.saved_tensors
-        # the penalty does not depend on the biases; the interpolates are constants (.data in the reference)
-        return None, g * dw1, None, g * dw2, None, g * dw3, None, None
-
-
-def gradient_penalty_mlp(critic_layers, xi, lambda_gp):
-    """critic_layers: the nn.Sequential(Linear, LeakyReLU, Linear, LeakyReLU, Linear) of wgan_gp.py:72-78."""
-    mods = list(critic_layers)
-    if not (len(mods) == 5 and all(isinstance(mods[i], torch.nn.Linear) for i in (0, 2, 4)) and
-            all(isinstance(mods[i], torch.nn.LeakyReLU) for i in (1, 3)) and mods[4].out_features == 1 and
-            mods[1].negative_slope == mods[3].negative_slope):
-        raise NotImplementedError("b200gan: fused gradient penalty expects Linear-LReLU-Linear-LReLU-Linear(->1)")
-    l1, l2, l3 = mods[0], mods[2], mods[4]
-    return GradientPenaltyMLPFn.apply(xi, l1.weight, l1.bias, l2.weight, l2.bias, l3.weight, float(mods[1].negative_slope),
-                                      float(lambda_gp))
-
-
 class CriticStepMLPFn(torch.autograd.Function):
     """d_loss = -mean(D(real)) + mean(D(fake)) + lambda * gp(D, interpolates) of wgan_gp.py:164-171 for the MLP critic,
     with every parameter gradient produced by the same kernel (first-order backward + closed-form double backward)."""
@@ -668,16 +637,17 @@ class CriticStepMLPFn(torch.autograd.Function):
 
 
 def critic_step_mlp(critic_layers, real, fake, alpha, lambda_gp):
-    """critic_layers: nn.Sequential(Linear, LeakyReLU, Linear, LeakyReLU, Linear(-> 1)) (wgan_gp.py:72-78).
-    Returns (d_loss, lambda * gradient penalty); d_loss.backward() fills the gradients of all six parameters."""
-    mods = list(critic_layers)
-    if not (len(mods) == 5 and all(isinstance(mods[i], torch.nn.Linear) for i in (0, 2, 4)) and
-            all(isinstance(mods[i], torch.nn.LeakyReLU) for i in (1, 3)) and mods[4].out_features == 1 and
-            mods[1].negative_slope == mods[3].negative_slope and all(mods[i].bias is not None for i in (0, 2, 4))):
-        raise NotImplementedError("b200gan: fused critic step expects Linear-LReLU-Linear-LReLU-Linear(->1) with biases")
-    l1, l2, l3 = mods[0], mods[2], mods[4]
-    return CriticStepMLPFn.apply(real, fake, alpha, l1.weight, l1.bias, l2.weight, l2.bias, l3.weight, l3.bias,
-                                 float(mods[1].negative_slope), float(lambda_gp))
+    """critic_layers: nn.Sequential(Linear, LeakyReLU, Linear, LeakyReLU, Linear(-> 1)) (wgan_gp.py:72-78), as
+    nn.mlp_critic_layers accepts it (no hooks).  Returns (d_loss, lambda * gradient penalty); d_loss.backward() fills the
+    gradients of all six parameters."""
+    from .nn import mlp_critic_layers  # nn imports this module
+    critic = mlp_critic_layers(list(critic_layers), real[0].numel())
+    if critic is None:
+        raise NotImplementedError("b200gan: fused critic step expects Linear-LReLU-Linear-LReLU-Linear(->1) with biases, "
+                                  "one slope, no hooks, taking the flattened images")
+    l1, l2, l3, slope = critic
+    return CriticStepMLPFn.apply(real, fake, alpha, l1.weight, l1.bias, l2.weight, l2.bias, l3.weight, l3.bias, slope,
+                                 float(lambda_gp))
 
 
 # ---- the MLP critic under autograd (csrc/mlp_critic.cu) ------------------------------------------------------------

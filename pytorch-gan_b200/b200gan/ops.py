@@ -12,7 +12,7 @@ import torch
 from . import _lib
 from ._lib import (ACT_NONE, ALGO_AUTO, ALGO_SIMT, ALGO_TC, PACK_SIMT_DGRAD, PACK_SIMT_FPROP, PACK_TC_DGRAD,
                    PACK_TC_DGRAD_UP2, PACK_TC_FPROP, PACK_TC_FPROP_UP2, PAD_REFLECT, PAD_ZERO, ConvGeom, Epilogue,
-                   GpMlpDesc, MlpCriticDesc, NbBn, NormDesc, TailDesc)
+                   MlpCriticDesc, NbBn, NormDesc, TailDesc)
 
 CL = torch.channels_last
 
@@ -537,52 +537,6 @@ def adam_step(p, g, m, v, lr, beta1, beta2, eps, grad_scale, step):
                                              beta1, beta2, eps, grad_scale, step.data_ptr(), _stream()), "adam_step")
 
 
-def gp_mlp_fwd_bwd(xi, w1, b1, w2, b2, w3, slope, lambda_gp):
-    """Gradient penalty of the 3-layer MLP critic and its weight gradients in one kernel
-    (wgan_gp.py:119-138 + the double backward at wgan_gp.py:173).  Returns (gp, dW1, dW2, dW3)."""
-    for t_ in (xi, w1, b1, w2, b2, w3):
-        _require_cuda(t_, "gp_mlp operand")
-    lib = _lib.load()
-    xi = xi.contiguous().view(xi.shape[0], -1)
-    d = GpMlpDesc()
-    d.N, d.Din, d.H1, d.H2 = xi.shape[0], xi.shape[1], w1.shape[0], w2.shape[0]
-    d.slope, d.lambda_gp = slope, lambda_gp
-    if w1.shape[1] != d.Din or w2.shape[1] != d.H1 or w3.numel() != d.H2:
-        raise RuntimeError("b200gan gp_mlp: layer shapes do not chain")
-    ws = torch.empty(lib.b200gan_gp_mlp_workspace_floats(ctypes.byref(d)), device=xi.device, dtype=torch.float32)
-    gp = torch.empty((), device=xi.device, dtype=torch.float32)
-    dw1, dw2, dw3 = torch.empty_like(w1), torch.empty_like(w2), torch.empty_like(w3)
-    _lib.check(lib.b200gan_gp_mlp_fwd_bwd(ctypes.byref(d), xi.data_ptr(), w1.data_ptr(), b1.data_ptr(), w2.data_ptr(),
-                                          b2.data_ptr(), w3.data_ptr(), gp.data_ptr(), dw1.data_ptr(), dw2.data_ptr(),
-                                          dw3.data_ptr(), ws.data_ptr(), _stream()), "gp_mlp_fwd_bwd")
-    return gp, dw1, dw2, dw3
-
-
-def critic_step_mlp(real, fake, alpha, w1, b1, w2, b2, w3, b3, slope, lambda_gp):
-    """wgan_gp.py:164-173 for the MLP critic in one kernel.  Returns (losses[2], dW1, db1, dW2, db2, dW3, db3)."""
-    for t_ in (real, fake, alpha, w1, b1, w2, b2, w3, b3):
-        _require_cuda(t_, "critic_step operand")
-    lib = _lib.load()
-    n = real.shape[0]
-    real, fake = real.contiguous().view(n, -1), fake.contiguous().view(n, -1)
-    alpha = alpha.contiguous().view(-1)
-    d = GpMlpDesc()
-    d.N, d.Din, d.H1, d.H2 = n, real.shape[1], w1.shape[0], w2.shape[0]
-    d.slope, d.lambda_gp = slope, lambda_gp
-    if (fake.shape != real.shape or alpha.numel() != n or w1.shape[1] != d.Din or w2.shape[1] != d.H1
-            or w3.numel() != d.H2):
-        raise RuntimeError("b200gan critic_step_mlp: shapes do not chain")
-    dev = real.device
-    ws = torch.empty(lib.b200gan_critic_step_workspace_floats(ctypes.byref(d)), device=dev, dtype=torch.float32)
-    losses = torch.empty(2, device=dev, dtype=torch.float32)
-    grads = [torch.empty_like(t_) for t_ in (w1, b1, w2, b2, w3, b3)]
-    _lib.check(lib.b200gan_critic_step_mlp(ctypes.byref(d), real.data_ptr(), fake.data_ptr(), alpha.data_ptr(),
-                                           w1.data_ptr(), b1.data_ptr(), w2.data_ptr(), b2.data_ptr(), w3.data_ptr(),
-                                           b3.data_ptr(), losses.data_ptr(), *[g.data_ptr() for g in grads],
-                                           ws.data_ptr(), _stream()), "critic_step_mlp")
-    return (losses, *grads)
-
-
 # ---- MLP critic under autograd: Linear -> LeakyReLU -> Linear -> LeakyReLU -> Linear(-> 1) (csrc/mlp_critic.cu) ------
 def _mlp_critic_desc(x, w1, w2, w3, slope):
     if x.dim() != 2 or w1.dim() != 2 or w2.dim() != 2:
@@ -659,3 +613,22 @@ def mlp_critic_dbwd(u, dout, u1, u2, m1, m2, w1, w2, w3, need):
                                            _ptr(dw1), _ptr(dw2), _ptr(dw3), _ptr(ddout), ws.data_ptr(), _stream()),
                "mlp_critic_dbwd")
     return ddout, dw1, dw2, dw3
+
+
+def critic_step_mlp(real, fake, alpha, w1, b1, w2, b2, w3, b3, slope, lambda_gp):
+    """wgan_gp.py:164-173 for the MLP critic in one kernel.  Returns (losses[2], dW1, db1, dW2, db2, dW3, db3)."""
+    real, fake, alpha, w1, b1, w2, b2, w3, b3 = _f32("critic_step operand", real, fake, alpha, w1, b1, w2, b2, w3, b3)
+    n = real.shape[0]
+    real, fake, alpha = real.view(n, -1), fake.view(n, -1), alpha.view(-1)
+    d = _mlp_critic_desc(real, w1, w2, w3, slope)
+    if fake.shape != real.shape or alpha.numel() != n or b1.numel() != d.H1 or b2.numel() != d.H2 or b3.numel() != 1:
+        raise RuntimeError("b200gan critic_step_mlp: fake, alpha or the biases do not match real and the layers")
+    lib, dev = _lib.load(), real.device
+    ws = torch.empty(lib.b200gan_critic_step_workspace_floats(ctypes.byref(d)), device=dev, dtype=torch.float32)
+    losses = torch.empty(2, device=dev, dtype=torch.float32)
+    grads = [torch.empty_like(t_) for t_ in (w1, b1, w2, b2, w3, b3)]
+    _lib.check(lib.b200gan_critic_step_mlp(ctypes.byref(d), float(lambda_gp), real.data_ptr(), fake.data_ptr(),
+                                           alpha.data_ptr(), w1.data_ptr(), b1.data_ptr(), w2.data_ptr(), b2.data_ptr(),
+                                           w3.data_ptr(), b3.data_ptr(), losses.data_ptr(),
+                                           *[g.data_ptr() for g in grads], ws.data_ptr(), _stream()), "critic_step_mlp")
+    return (losses, *grads)

@@ -94,16 +94,17 @@ def dcgan_step(generator, discriminator, opt_g, opt_d, real_imgs, z, loss=None, 
 def wgan_gp_critic_step(generator, discriminator, opt_d, real_imgs, z, alpha, lambda_gp=10.0, fused_gp=True,
                         reduce_d=None):
     """One critic iteration of implementations/wgan_gp/wgan_gp.py:155-174.  `alpha` [N,1,1,1] is the
-    interpolation weight the reference draws with numpy (wgan_gp.py:122).  With fused_gp the penalty and its
-    double backward run in the single gp_mlp kernel; otherwise through autograd exactly like the reference.
+    interpolation weight the reference draws with numpy (wgan_gp.py:122).  A truthy fused_gp (True or "step") runs
+    the whole iteration -- three critic passes, the penalty and the backward -- in one cooperative kernel
+    (functional.critic_step_mlp, MLP critic only); fused_gp=False builds the penalty with autograd exactly like the
+    reference, which on the drop-in modules runs on the fused critic kernels.
     The reference leaves fake_imgs attached (dead back-prop into G, whose grads are zeroed at :176); here the
     fakes are detached -- identical D update."""
     from . import functional as F
     opt_d.zero_grad()                                                     # :155
     with torch.no_grad():
         fake_imgs = generator(z)                                          # :161
-    if fused_gp == "step":
-        # the whole of :164-173 (three critic passes, penalty, backward) in one cooperative kernel
+    if fused_gp:
         d_loss, gp_term = F.critic_step_mlp(discriminator.model, real_imgs, fake_imgs, alpha, lambda_gp)
         d_loss.backward()
         _opt_step(opt_d, reduce_d)
@@ -112,15 +113,12 @@ def wgan_gp_critic_step(generator, discriminator, opt_d, real_imgs, z, alpha, la
     real_validity = discriminator(real_imgs)                              # :164
     fake_validity = discriminator(fake_imgs)                              # :166
     interpolates = alpha * real_imgs + (1 - alpha) * fake_imgs            # :124
-    if fused_gp:
-        gp_term = F.gradient_penalty_mlp(discriminator.model, interpolates, lambda_gp)
-    else:
-        interpolates = interpolates.requires_grad_(True)
-        d_int = discriminator(interpolates)                               # :125
-        grads = torch.autograd.grad(outputs=d_int, inputs=interpolates, grad_outputs=torch.ones_like(d_int),
-                                    create_graph=True, retain_graph=True, only_inputs=True)[0]   # :128-135
-        grads = grads.view(grads.size(0), -1)
-        gp_term = lambda_gp * ((grads.norm(2, dim=1) - 1) ** 2).mean()    # :137
+    interpolates = interpolates.requires_grad_(True)
+    d_int = discriminator(interpolates)                                   # :125
+    grads = torch.autograd.grad(outputs=d_int, inputs=interpolates, grad_outputs=torch.ones_like(d_int),
+                                create_graph=True, retain_graph=True, only_inputs=True)[0]   # :128-135
+    grads = grads.view(grads.size(0), -1)
+    gp_term = lambda_gp * ((grads.norm(2, dim=1) - 1) ** 2).mean()        # :137
     d_loss = -torch.mean(real_validity) + torch.mean(fake_validity) + gp_term   # :171
     d_loss.backward()                                                     # :173
     _opt_step(opt_d, reduce_d)                                            # :174

@@ -1,9 +1,9 @@
-// mlp_critic.cu -- autograd of the MLP critic (wgan_gp.py:72-78, wgan_div.py:72-78) as three cooperative kernels:
+// mlp_critic.cu -- the MLP critic (wgan_gp.py:72-78, wgan_div.py:72-78) as cooperative kernels:
 //   D(x) = W3 lrelu(W2 lrelu(W1 x + b1) + b2) + b3,      Din -> H1 -> H2 -> 1, one LeakyReLU slope.
-// Unlike gp_mlp.cu, no penalty is built in: the forward, the first-order backward for an arbitrary output gradient
-// dout, and the double backward of the input gradient for an arbitrary upstream gradient u = dL/d(dD/dx) are separate
-// entry points, so a script's own penalty arithmetic (||g|| - 1)^2, ||g||^p, ... stays in its autograd graph while every
-// critic GEMM runs here.
+// Its autograd is three kernels with no penalty built in: the forward, the first-order backward for an arbitrary output
+// gradient dout, and the double backward of the input gradient for an arbitrary upstream gradient u = dL/d(dD/dx) are
+// separate entry points, so a script's own penalty arithmetic (||g|| - 1)^2, ||g||^p, ... stays in its autograd graph
+// while every critic GEMM runs here.
 //   forward        h1 = x W1^T + b1, m1 = lrelu'(h1), a1 = h1 m1;   h2 = a1 W2^T + b2, m2 = lrelu'(h2), a2 = h2 m2
 //                  out = a2 W3^T + b3
 //   backward       U2 = dout W3 * m2;  U1 = (U2 W2) * m1;  dx = U1 W1
@@ -14,6 +14,7 @@
 // Each pass is ~0.1 GFLOP at the WGAN-GP size and latency bound, so each is ONE persistent cooperative launch whose
 // dependent phases are separated by grid.sync(); every phase spreads 32x32 fp32 FFMA output tiles (tile_gemm.cuh)
 // over the grid.  Column sums run one thread per column in a fixed order: the results are deterministic.
+// critic_step_kernel (below) is the whole WGAN-GP critic iteration, penalty included, in one such launch.
 #include "common.cuh"
 #include "tile_gemm.cuh"
 #include <cooperative_groups.h>
@@ -65,34 +66,31 @@ __device__ __forceinline__ void col_sums(const float *A, const float *wr, float 
   }
 }
 
+// one LeakyReLU layer over R rows: h = A W^T + b with A [R][K], W [J][K];  m = lrelu'(h), a = h m, both [R][J]
+__device__ __forceinline__ void lrelu_layer(const float *A, const float *W, const float *b, float slope, float *m,
+                                            float *a, int R, int K, int J, float (*As)[GT + 1], float (*Bs)[GT + 1]) {
+  for (int t = blockIdx.x; t < ntiles(R, J); t += gridDim.x)
+    tile_gemm(A, K, 1, W, 1, K, R, J, K, t,
+              [&](int r, int j, float acc) {
+                const float h = acc + b[j];
+                const float mk = h > 0.f ? 1.f : slope;
+                m[(size_t)r * J + j] = mk;
+                a[(size_t)r * J + j] = h * mk;
+              }, As, Bs);
+}
+
 __global__ void __launch_bounds__(256) mlp_critic_fwd_kernel(McFwdP p) {
   __shared__ float As[GT][GT + 1];
   __shared__ float Bs[GT][GT + 1];
   cg::grid_group grid = cg::this_grid();
-  const int N = p.N, Din = p.Din, H1 = p.H1, H2 = p.H2;
-  const int nb = gridDim.x, bid = blockIdx.x;
   // P1: h1 = x W1^T + b1
-  for (int t = bid; t < ntiles(N, H1); t += nb)
-    tile_gemm(p.x, Din, 1, p.W1, 1, Din, N, H1, Din, t,
-              [&](int n, int j, float acc) {
-                const float h = acc + p.b1[j];
-                const float m = h > 0.f ? 1.f : p.slope;
-                p.m1[(size_t)n * H1 + j] = m;
-                p.a1[(size_t)n * H1 + j] = h * m;
-              }, As, Bs);
+  lrelu_layer(p.x, p.W1, p.b1, p.slope, p.m1, p.a1, p.N, p.Din, p.H1, As, Bs);
   grid.sync();
   // P2: h2 = a1 W2^T + b2
-  for (int t = bid; t < ntiles(N, H2); t += nb)
-    tile_gemm(p.a1, H1, 1, p.W2, 1, H1, N, H2, H1, t,
-              [&](int n, int j, float acc) {
-                const float h = acc + p.b2[j];
-                const float m = h > 0.f ? 1.f : p.slope;
-                p.m2[(size_t)n * H2 + j] = m;
-                p.a2[(size_t)n * H2 + j] = h * m;
-              }, As, Bs);
+  lrelu_layer(p.a1, p.W2, p.b2, p.slope, p.m2, p.a2, p.N, p.H1, p.H2, As, Bs);
   grid.sync();
   // P3: out = a2 W3^T + b3
-  row_dots(p.a2, p.W3, p.b3, p.out, N, H2);
+  row_dots(p.a2, p.W3, p.b3, p.out, p.N, p.H2);
 }
 
 __global__ void __launch_bounds__(256) mlp_critic_bwd_kernel(McBwdP p) {
@@ -184,6 +182,148 @@ __global__ void __launch_bounds__(256) mlp_critic_dbwd_kernel(McDbwdP p) {
   if (p.ddout) row_dots(p.s, p.W3, nullptr, p.ddout, N, H2);
 }
 
+// ---- the whole critic iteration of wgan_gp.py:164-173 in ONE kernel -----------------------------------------------------------
+//   d_loss = -mean(D(real)) + mean(D(fake)) + lambda * gp(D, alpha * real + (1 - alpha) * fake)
+// and its gradient w.r.t. every parameter of D.  The three batches (real, fake, interpolates) are stacked into one 3N-row
+// problem; the first-order backward of the real/fake rows and the closed-form double backward of the penalty rows share
+// their GEMMs: with dout = (-1/N, +1/N, 1) per row group,
+//   U2 = dout * W3 * m2          rows < 2N: dL/dh2,        penalty rows: g2
+//   U1 = (U2 W2) * m1            rows < 2N: dL/dh1,        penalty rows: g1 (then scaled by coef -> g1s)
+//   X3 penalty rows <- gx = g1 W1 (the interpolates themselves are dead after layer 1)
+//   dW1 = U1^T X3                = dh1^T x  +  g1s^T gx
+//   A1 penalty rows <- t = coef * (gx W1^T) * m1;     dW2 = U2^T A1 = dh2^T a1 + g2^T t
+//   A2 penalty rows <- (t W2^T) * m2;                 dW3 = sum_r dout_r * A2_r
+// with gx = dD/dx, r_n = ||gx_n||_2, the penalty term lambda * mean((r - 1)^2) and coef_n = lambda * (2/N) (r_n - 1) / r_n
+// (the term's derivative w.r.t. r_n, over r_n).
+// Bias gradients come from the real/fake rows only (the penalty does not depend on the biases).
+struct CsP {
+  int N, Din, H1, H2;
+  float slope, lambda_gp;
+  const float *real, *fake, *alpha, *W1, *b1, *W2, *b2, *W3, *b3;
+  float *losses;  // [2]: d_loss, lambda * gp
+  float *dW1, *db1, *dW2, *db2, *dW3, *db3;
+  float *X3, *A1, *U1, *M1, *A2, *U2, *M2, *dout, *coef;
+};
+
+// The bound only caps ptxas at 64 registers; launch_coop still runs two blocks per SM.  Without it ptxas spills values
+// live across the division subroutine calls; under a two-block bound (128 registers) the kernel runs ~3% slower than
+// at 64 (206.5 vs 200.6 us per launch, N = 64, 1024 -> 512 -> 256, H100 80GB HBM3 at 700 W).
+__global__ void __launch_bounds__(256, 4) critic_step_kernel(CsP p) {
+  __shared__ float As[GT][GT + 1];
+  __shared__ float Bs[GT][GT + 1];
+  cg::grid_group grid = cg::this_grid();
+  const int N = p.N, Din = p.Din, H1 = p.H1, H2 = p.H2, R = 3 * p.N;
+  const int nb = gridDim.x, bid = blockIdx.x;
+  const int64_t gtid = (int64_t)bid * blockDim.x + threadIdx.x, gthreads = (int64_t)nb * blockDim.x;
+
+  // P0: stack the three batches, per-row output gradients
+  for (int64_t i = gtid; i < (int64_t)N * Din; i += gthreads) {
+    const int n = (int)(i / Din);
+    const float r = p.real[i], f = p.fake[i], a = p.alpha[n];
+    p.X3[i] = r;
+    p.X3[(int64_t)N * Din + i] = f;
+    p.X3[(int64_t)2 * N * Din + i] = a * r + (1.f - a) * f;
+  }
+  for (int64_t i = gtid; i < R; i += gthreads) p.dout[i] = i < N ? -1.f / (float)N : (i < 2 * N ? 1.f / (float)N : 1.f);
+  if (gtid < 2) p.losses[gtid] = 0.f;
+  grid.sync();
+  // P1: h1 = X3 W1^T + b1
+  lrelu_layer(p.X3, p.W1, p.b1, p.slope, p.M1, p.A1, R, Din, H1, As, Bs);
+  grid.sync();
+  // P2: h2 = a1 W2^T + b2; U2 = dout * W3 * m2
+  for (int t = bid; t < ntiles(R, H2); t += nb)
+    tile_gemm(p.A1, H1, 1, p.W2, 1, H1, R, H2, H1, t,
+              [&](int r, int j, float acc) {
+                const float h = acc + p.b2[j];
+                const float m = h > 0.f ? 1.f : p.slope;
+                p.M2[(size_t)r * H2 + j] = m;
+                p.A2[(size_t)r * H2 + j] = h * m;
+                p.U2[(size_t)r * H2 + j] = p.dout[r] * p.W3[j] * m;
+              }, As, Bs);
+  grid.sync();
+  // P3: critic outputs of the real / fake rows -> Wasserstein part of the loss;  U1 = (U2 W2) * m1
+  {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int r = bid * 8 + warp; r < 2 * N; r += nb * 8) {
+      float s = 0.f;
+      for (int j = lane; j < H2; j += 32) s = fmaf(p.A2[(size_t)r * H2 + j], p.W3[j], s);
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+      if (lane == 0) atomicAdd(p.losses, (s + p.b3[0]) * p.dout[r]);
+    }
+  }
+  for (int t = bid; t < ntiles(R, H1); t += nb)
+    tile_gemm(p.U2, H2, 1, p.W2, H1, 1, R, H1, H2, t,
+              [&](int r, int i, float acc) { p.U1[(size_t)r * H1 + i] = acc * p.M1[(size_t)r * H1 + i]; }, As, Bs);
+  grid.sync();
+  // P4: gx = g1 W1 over the penalty rows, written over the (dead) interpolates
+  for (int t = bid; t < ntiles(N, Din); t += nb)
+    tile_gemm(p.U1 + (size_t)2 * N * H1, H1, 1, p.W1, Din, 1, N, Din, H1, t,
+              [&](int n, int d, float acc) { p.X3[(size_t)(2 * N + n) * Din + d] = acc; }, As, Bs);
+  grid.sync();
+  // P5: per-sample gradient norm, penalty, coefficient; g1 -> g1s = coef * g1
+  {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int n = bid * 8 + warp; n < N; n += nb * 8) {
+      const float *gx = p.X3 + (size_t)(2 * N + n) * Din;
+      float s = 0.f;
+      for (int d = lane; d < Din; d += 32) s = fmaf(gx[d], gx[d], s);
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+      const float r = sqrtf(s);
+      const float c = p.lambda_gp * (2.f / (float)N) * (r - 1.f) / r;
+      if (lane == 0) {
+        p.coef[n] = c;
+        const float term = p.lambda_gp * (r - 1.f) * (r - 1.f) / (float)N;
+        atomicAdd(p.losses, term);
+        atomicAdd(p.losses + 1, term);
+      }
+      float *g1 = p.U1 + (size_t)(2 * N + n) * H1;
+      for (int i = lane; i < H1; i += 32) g1[i] *= c;
+    }
+  }
+  grid.sync();
+  // P6: dW1 = U1^T X3;  t = coef * (gx W1^T) * m1 over the (dead) a1 of the penalty rows;  db1
+  {
+    const int ta = ntiles(H1, Din), tb = ntiles(N, H1);
+    for (int t = bid; t < ta + tb; t += nb) {
+      if (t < ta)
+        tile_gemm(p.U1, 1, H1, p.X3, Din, 1, H1, Din, R, t,
+                  [&](int i, int d, float acc) { p.dW1[(size_t)i * Din + d] = acc; }, As, Bs);
+      else
+        tile_gemm(p.X3 + (size_t)2 * N * Din, Din, 1, p.W1, 1, Din, N, H1, Din, t - ta,
+                  [&](int n, int i, float acc) {
+                    p.A1[(size_t)(2 * N + n) * H1 + i] = acc * p.coef[n] * p.M1[(size_t)(2 * N + n) * H1 + i];
+                  }, As, Bs);
+    }
+    col_sums(p.U1, nullptr, p.db1, 2 * N, H1);
+  }
+  grid.sync();
+  // P7: dW2 = U2^T A1;  A2 penalty rows <- (t W2^T) * m2;  db2
+  {
+    const int ta = ntiles(H2, H1), tb = ntiles(N, H2);
+    for (int t = bid; t < ta + tb; t += nb) {
+      if (t < ta)
+        tile_gemm(p.U2, 1, H2, p.A1, H1, 1, H2, H1, R, t,
+                  [&](int j, int i, float acc) { p.dW2[(size_t)j * H1 + i] = acc; }, As, Bs);
+      else
+        tile_gemm(p.A1 + (size_t)2 * N * H1, H1, 1, p.W2, 1, H1, N, H2, H1, t - ta,
+                  [&](int n, int j, float acc) {
+                    p.A2[(size_t)(2 * N + n) * H2 + j] = acc * p.M2[(size_t)(2 * N + n) * H2 + j];
+                  }, As, Bs);
+    }
+    col_sums(p.U2, nullptr, p.db2, 2 * N, H2);
+  }
+  grid.sync();
+  // P8: dW3 = sum_r dout_r * A2_r;  db3 = sum over the real / fake rows of dout
+  col_sums(p.A2, p.dout, p.dW3, R, H2);
+  if (gtid == 0) {
+    float s = 0.f;
+    for (int r = 0; r < 2 * N; ++r) s += p.dout[r];
+    p.db3[0] = s;
+  }
+}
+
 // one persistent cooperative launch, grid sized to the device's SMs (at most two blocks per SM)
 template <class P>
 static int launch_coop(void (*kernel)(P), P &p, void *stream, const char *what) {
@@ -263,4 +403,32 @@ extern "C" int b200gan_mlp_critic_dbwd(const b200gan_mlp_critic_desc *d, const f
   p.t = workspace;
   p.s = workspace + (size_t)d->N * d->H1;
   return launch_coop(mlp_critic_dbwd_kernel, p, stream, "mlp_critic_dbwd");
+}
+
+extern "C" size_t b200gan_critic_step_workspace_floats(const b200gan_mlp_critic_desc *d) {
+  if (!d) return 0;
+  const size_t R = (size_t)3 * d->N;
+  return R * ((size_t)d->Din + 3 * (size_t)d->H1 + 3 * (size_t)d->H2 + 1) + d->N + 64;
+}
+
+extern "C" int b200gan_critic_step_mlp(const b200gan_mlp_critic_desc *d, float lambda_gp, const float *real,
+                                       const float *fake, const float *alpha, const float *W1, const float *b1,
+                                       const float *W2, const float *b2, const float *W3, const float *b3,
+                                       float *losses, float *dW1, float *db1, float *dW2, float *db2, float *dW3,
+                                       float *db3, float *workspace, void *stream) {
+  B2_CHECK_ARG(d && real && fake && alpha && W1 && b1 && W2 && b2 && W3 && b3 && losses && dW1 && db1 && dW2 && db2 &&
+                   dW3 && db3 && workspace, "critic_step_mlp: null pointer");
+  B2_CHECK_ARG(dims_ok(d), "critic_step_mlp: bad dims");
+  CsP p;
+  p.N = d->N; p.Din = d->Din; p.H1 = d->H1; p.H2 = d->H2; p.slope = d->slope; p.lambda_gp = lambda_gp;
+  p.real = real; p.fake = fake; p.alpha = alpha; p.W1 = W1; p.b1 = b1; p.W2 = W2; p.b2 = b2; p.W3 = W3; p.b3 = b3;
+  p.losses = losses; p.dW1 = dW1; p.db1 = db1; p.dW2 = dW2; p.db2 = db2; p.dW3 = dW3; p.db3 = db3;
+  const size_t R = (size_t)3 * d->N;
+  float *w = workspace;
+  p.X3 = w; w += R * d->Din;
+  p.A1 = w; w += R * d->H1; p.U1 = w; w += R * d->H1; p.M1 = w; w += R * d->H1;
+  p.A2 = w; w += R * d->H2; p.U2 = w; w += R * d->H2; p.M2 = w; w += R * d->H2;
+  p.dout = w; w += R;
+  p.coef = w;
+  return launch_coop(critic_step_kernel, p, stream, "critic_step_mlp");
 }

@@ -1,4 +1,4 @@
-// tile_gemm.cuh -- the 32x32 fp32 FFMA tile GEMM shared by the cooperative MLP-critic kernels (gp_mlp.cu, mlp_critic.cu).
+// tile_gemm.cuh -- the 32x32 fp32 FFMA tile GEMM of the cooperative MLP-critic kernels (mlp_critic.cu).
 // Each phase of those kernels spreads the 32x32 output tiles of one or two small GEMMs over a persistent grid.
 #pragma once
 #include <cuda_runtime.h>

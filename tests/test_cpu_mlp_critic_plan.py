@@ -51,3 +51,22 @@ def test_rejects_hooked_layers_and_has_no_side_effects():
     assert bnn.mlp_critic_layers(mods, DIN) is not None
     for k, v in torch.nn.Sequential(*mods).state_dict().items():
         assert torch.equal(v, state[k]) and v.grad is None, k
+
+
+def test_fused_critic_step_refuses_what_the_plan_rejects(monkeypatch):
+    """functional.critic_step_mlp (the one-kernel WGAN-GP critic iteration) accepts exactly what mlp_critic_layers
+    accepts: a hooked critic, whose hooks the kernel would skip, and a non-critic are refused before any launch."""
+    from b200gan import functional as F, ops
+
+    def launched(*a, **kw):
+        raise AssertionError("critic_step_mlp launched")
+    monkeypatch.setattr(ops, "critic_step_mlp", launched)
+    real = fake = torch.zeros(2, 1, 28, 28)
+    alpha = torch.zeros(2, 1, 1, 1)
+    hooked = _critic(bnn)
+    hooked[0].register_forward_hook(lambda m, a, out: None)
+    for what, mods in {"hooked": hooked, "trailing sigmoid": _critic(bnn) + [bnn.Sigmoid()]}.items():
+        with pytest.raises(NotImplementedError):
+            F.critic_step_mlp(bnn.Sequential(*mods), real, fake, alpha, 10.0)
+    with pytest.raises(AssertionError, match="launched"):  # the same critic without the hook goes to the kernel
+        F.critic_step_mlp(bnn.Sequential(*_critic(bnn)), real, fake, alpha, 10.0)

@@ -90,12 +90,12 @@ def test_library_loads_and_exports_every_declared_symbol():
     assert lib.b200gan_version() == 100
 
 
-def test_struct_layouts_match_the_header():
+def test_abi_struct_sizes_match_the_header():
     from b200gan import _lib
     assert ctypes.sizeof(_lib.ConvGeom) == 17 * 4
     assert ctypes.sizeof(_lib.Epilogue) == 40
     assert ctypes.sizeof(_lib.NormDesc) == 9 * 4
-    assert ctypes.sizeof(_lib.GpMlpDesc) == 6 * 4
+    assert ctypes.sizeof(_lib.MlpCriticDesc) == 5 * 4
     assert ctypes.sizeof(_lib.TailDesc) == 8 * 4
     assert ctypes.sizeof(_lib.NbBn) == 48 and ctypes.sizeof(_lib.AdamTensor) == 40
     assert ctypes.sizeof(_lib.PackJob) == 16 + 17 * 4 + 4
