@@ -6,9 +6,9 @@ gridDim.z = phases x ksplit; weight gradient: gridDim.x = pixel splits), whether
 same bits, and the partial sums `s` that are added outside one accumulation chain (k-splits, pixel splits, folded
 jobs).  Each case names the edge it exists for.
 
-The table is written from the eligibility predicates (tc_supported, wg_plan, fewk_ok, nb_plain_*_ok, nb_wgrad_ok
-and the kernel choice in simt_gather_gemm / simt_wgrad), not from a run.  Tile widths and split counts assume a
-132-SM H100 SXM; tests/test_gpu_conv_conformance.py checks the grids only on such a device.
+The table is written from the eligibility predicates (tc_supported, wg_plan, fewk_ok, nb_plain_*_ok, nb_wgrad_ok),
+not from a run.  Tile widths and split counts assume a 132-SM H100 SXM; tests/test_gpu_conv_conformance.py checks the
+grids only on such a device.
 
 tests/test_cpu_conv_case_table.py checks it against b200gan_conv2d_supported and against the kernels declared in the
 sources; tests/test_gpu_conv_conformance.py runs every case.
@@ -204,27 +204,27 @@ SIMT = [
        deterministic=False, s=528, why="5x5: neither TC (no 128-channel operand) nor staged: conv_wgrad_kernel"),
     _c("simt_5x5", 2, 32, 64, 8, 8, 5, 5, pads=P2, algo="SIMT", epi=("bias",), kernels=("conv_gather_gemm_kernel",),
        why="5x5 forward forced onto the generic gather GEMM"),
-    _c("smallk_gather", 2, 33, 3, 8, 8, 3, 3, pads=P1, epi=("bias",), kernels=("conv_gather_smallk_kernel<4>",),
-       why="K <= 4 with C = 33 (not a multiple of 4): one warp per pixel"),
+    _c("smallk_gather", 2, 33, 3, 8, 8, 3, 3, pads=P1, epi=("bias",), kernels=("conv_gather_gemm_kernel",),
+       why="K = 3 with C = 33 (not fewk): 3 of the tile's 64 output columns, a reduction that is not a multiple of 16"),
     _c("smallk_vec", 2, 64, 1, 8, 8, 4, 4, stride=2, pads=P1, epi=("bias", "sigmoid"),
-       kernels=("conv_smallk_vec_kernel<16, 4>",), why="K = 1, stride 2 (not fewk): float4 lanes over 64 channels"),
-    _c("smallc", 2, 3, 12, 8, 8, 4, 4, stride=2, pads=P1, epi=("bias",), kernels=("conv_smallc_kernel",),
-       why="C = 3, K = 12 (not a multiple of 16, so not staged)"),
-    _c("s3_smallc", 2, 3, 8, 8, 8, 3, 3, pads=P1, epi=("bias", "lrelu"), kernels=("conv3x3s1_smallc_kernel<3>",),
-       why="3x3 s1 p1 with C = 3, K = 8"),
-    _c("s3_smallk", 2, 16, 2, 8, 8, 3, 3, pads=P1, epi=("bias",), kernels=("conv3x3s1_smallk_kernel<4, 2>",),
+       kernels=("conv_gather_gemm_kernel",), why="K = 1, stride 2 (not fewk): one output column of the tile"),
+    _c("smallc", 2, 3, 12, 8, 8, 4, 4, stride=2, pads=P1, epi=("bias",), kernels=("conv_gather_gemm_kernel",),
+       why="C = 3, K = 12 (not a multiple of 16, so not staged): 12 of the tile's 64 output columns"),
+    _c("s3_smallc", 2, 3, 8, 8, 8, 3, 3, pads=P1, epi=("bias", "lrelu"), kernels=("conv_gather_gemm_kernel",),
+       why="3x3 s1 p1 with C = 3, K = 8: a 27-long reduction, its second 16-wide slice partly empty"),
+    _c("s3_smallk", 2, 16, 2, 8, 8, 3, 3, pads=P1, epi=("bias",), kernels=("conv_gather_gemm_kernel",),
        why="3x3 s1 p1 with K = 2, C = 16 (too few channels for fewk)"),
     _c("smallcd", 2, 64, 2, 8, 8, 5, 5, stride=2, pads=P2, pas=WGRAD,
-       kernels=("conv_wgrad_smallcd_kernel", "colsum_kernel"), deterministic=False, s=1056,
-       why="wgrad with 2 output channels, 5x5 s2: block partials and atomics"),
+       kernels=("conv_wgrad_kernel", "colsum_kernel"), deterministic=False, s=528,
+       why="wgrad with 2 output channels, 5x5 s2: 2 of the tile's 64 dense columns"),
     _c("tr_cd1", 2, 1, 16, 8, 8, 3, 3, pads=P1, transposed=True, pas=WGRAD,
-       kernels=("conv3x3s1_wgrad_cd1_kernel<4>", "colsum_kernel"), deterministic=False, s=528,
-       why="ConvTranspose2d(1, 16, 3, 1, 1) wgrad: the single dense-channel 3x3 kernel"),
+       kernels=("conv_wgrad_kernel", "colsum_kernel"), deterministic=False, s=528,
+       why="ConvTranspose2d(1, 16, 3, 1, 1) wgrad: one dense channel, gathered over dy"),
     _c("tr_simt_s2", 2, 32, 64, 4, 4, 4, 4, stride=2, pads=P1, transposed=True, algo="SIMT",
        epi=("bias",), kernels=("conv_gather_gemm_kernel",), grid=(1, 1, 4),
        why="transposed stride-2 fprop forced onto SIMT: parity classes"),
     _c("tr_simt_s2", 2, 64, 3, 4, 4, 4, 4, stride=2, pads=P1, transposed=True, pas=DGRAD,
-       kernels=("conv_smallc_kernel",), why="transposed dgrad with 3 output channels: SIMT gather over dy"),
+       kernels=("conv_gather_gemm_kernel",), why="transposed dgrad with 3 output channels: SIMT gather over dy"),
     _c("tr_simt_s2", 2, 64, 3, 4, 4, 4, 4, stride=2, pads=P1, transposed=True, pas=WGRAD,
        kernels=("conv_wgrad_kernel", "colsum_kernel"), deterministic=False, s=528, why="transposed SIMT wgrad"),
     _c("virt_up2_reflect", 2, 32, 16, 4, 4, 3, 3, pads=P1, pad_mode=REFLECT, up=2, pas=DGRAD,
@@ -283,7 +283,7 @@ STAGED = [
     _c("nb_asym", 2, 3, 64, 16, 16, 4, 4, stride=2, pads=(2, 2, 1, 1), epi=("bias",), kernels=("nbk_fprop2_kernel",),
        why="ZeroPad2d((1,0,1,0)) + Conv2d(3, 64, 4, 2, 1): asymmetric padding, allowed by nb_plain_fprop_ok"),
     _c("nb_asym", 2, 3, 64, 16, 16, 4, 4, stride=2, pads=(2, 2, 1, 1), pas=DGRAD,
-       kernels=("conv_smallk_vec_kernel<16, 4>",), why="asymmetric padding is not staged in dgrad: SIMT gather"),
+       kernels=("conv_gather_gemm_kernel",), why="asymmetric padding is not staged in dgrad: SIMT gather"),
     _c("nb_asym", 2, 3, 64, 16, 16, 4, 4, stride=2, pads=(2, 2, 1, 1), pas=WGRAD,
        kernels=("conv_wgrad_kernel", "colsum_kernel"), deterministic=False, s=528,
        why="asymmetric padding is not staged in wgrad: SIMT"),
@@ -330,7 +330,7 @@ def _epilogue_cases():
             name = base.name + "-" + ("all" if opts == _ALL else opts[0])
             ks = kern
             if fewk and ("chan_scale" in epi or "round_tf32" in epi):
-                ks = ("conv3x3s1_smallk_kernel<8, 3>",)  # fewk takes neither option: the SIMT 3x3 kernel does
+                ks = ("conv_gather_gemm_kernel",)  # fewk takes neither option: the SIMT gather GEMM does
             stats = [o for o in epi if o.startswith("stats")]
             deferred = stats and not (fuses and (stats[0] == "stats_c" or per_sample_fused))
             if deferred:
