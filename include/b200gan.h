@@ -190,8 +190,9 @@ int b200gan_norm_finalize(const b200gan_norm_desc *d, double *stats, const float
 /* y = act(x * scale + shift); may run in place (y == x). */
 int b200gan_norm_apply(const b200gan_norm_desc *d, const float *x, const float *scale_shift,
                        float *y, void *stream);
-/* Backward.  Inputs: dy, saved input x, mean_rstd, gamma (or NULL), and for a fused activation EITHER scale_shift
- * (LeakyReLU / ReLU: the mask is recomputed from x, nothing else has to be kept) OR the saved output y.
+/* Backward.  Inputs: dy, saved input x, mean_rstd, gamma (or NULL), and scale_shift (or NULL).  With scale_shift
+ * a LeakyReLU / ReLU mask is recomputed from x; the saved output y is required only for Tanh / Sigmoid, or for
+ * LeakyReLU / ReLU when scale_shift is NULL (otherwise y may be NULL).
  * sums[2][G] fp64 workspace: zero on entry, handed back zeroed.
  * Outputs: dx; dgamma_dbeta[2][G] (only meaningful for per_sample == 0 with affine; may be NULL). */
 int b200gan_norm_bwd(const b200gan_norm_desc *d, const float *dy, const float *x, const float *y,

@@ -204,8 +204,8 @@ def bias_grad(dy, y, chan_scale, act, slope):
 
 
 # ---- normalisation -----------------------------------------------------------------------------
-def _norm_desc(x, per_sample, eps, momentum, act, slope, round_tf32):
-    n, c, h, w = x.shape
+def _norm_desc(shape, per_sample, eps, momentum, act, slope, round_tf32):
+    n, c, h, w = shape
     d = NormDesc()
     d.N, d.HW, d.C, d.per_sample = n, h * w, c, int(per_sample)
     d.eps, d.momentum, d.act, d.slope, d.round_tf32 = eps, momentum, act, slope, int(round_tf32)
@@ -241,21 +241,14 @@ def new_stats(x, per_sample):
 def norm_forward(x, gamma, beta, running_mean, running_var, nbt, per_sample, eps, momentum, act=ACT_NONE, slope=0.0,
                  stats=None, round_tf32=False, return_scale_shift=False):
     """Training-mode BatchNorm2d / InstanceNorm2d.  Returns (y, mean_rstd)."""
-    lib = _lib.load()
-    d = _norm_desc(x, per_sample, eps, momentum, act, slope, round_tf32)
-    st = _stream()
     if stats is None:
-        stats = new_stats(x, per_sample)
-        _lib.check(lib.b200gan_norm_stats(ctypes.byref(d), x.data_ptr(), stats.data_ptr(), st), "norm_stats")
-    groups = stats.numel() // 2
-    mean_rstd = torch.empty(2 * groups, device=x.device, dtype=torch.float32)
-    scale_shift = torch.empty(2 * groups, device=x.device, dtype=torch.float32)
-    _lib.check(lib.b200gan_norm_finalize(ctypes.byref(d), stats.data_ptr(), _ptr(gamma), _ptr(beta),
-                                         mean_rstd.data_ptr(), scale_shift.data_ptr(), _ptr(running_mean),
-                                         _ptr(running_var), _ptr(nbt), st), "norm_finalize")
+        stats = norm_stats(x, per_sample)
+    mean_rstd, scale_shift = norm_finalize(x.shape, stats, gamma, beta, running_mean, running_var, nbt, per_sample, eps,
+                                           momentum, x.device)
+    d = _norm_desc(x.shape, per_sample, eps, momentum, act, slope, round_tf32)
     y = torch.empty_like(x, memory_format=CL)
-    _lib.check(lib.b200gan_norm_apply(ctypes.byref(d), x.data_ptr(), scale_shift.data_ptr(), y.data_ptr(), st),
-               "norm_apply")
+    _lib.check(_lib.load().b200gan_norm_apply(ctypes.byref(d), x.data_ptr(), scale_shift.data_ptr(), y.data_ptr(),
+                                              _stream()), "norm_apply")
     if return_scale_shift:
         return y, mean_rstd, scale_shift
     return y, mean_rstd
@@ -263,10 +256,7 @@ def norm_forward(x, gamma, beta, running_mean, running_var, nbt, per_sample, eps
 
 def norm_finalize(x_shape, stats, gamma, beta, running_mean, running_var, nbt, per_sample, eps, momentum, device):
     """Batch statistics -> (mean_rstd, scale_shift); updates the running statistics.  `stats` is consumed (zeroed)."""
-    n, c, h, w = x_shape
-    d = NormDesc()
-    d.N, d.HW, d.C, d.per_sample = n, h * w, c, int(per_sample)
-    d.eps, d.momentum, d.act, d.slope, d.round_tf32 = eps, momentum, ACT_NONE, 0.0, 0
+    d = _norm_desc(x_shape, per_sample, eps, momentum, ACT_NONE, 0.0, False)
     groups = stats.numel() // 2
     mean_rstd = torch.empty(2 * groups, device=device, dtype=torch.float32)
     scale_shift = torch.empty(2 * groups, device=device, dtype=torch.float32)
@@ -277,7 +267,7 @@ def norm_finalize(x_shape, stats, gamma, beta, running_mean, running_var, nbt, p
 
 
 def norm_stats(x, per_sample):
-    d = _norm_desc(x, per_sample, 0.0, 0.0, ACT_NONE, 0.0, False)
+    d = _norm_desc(x.shape, per_sample, 0.0, 0.0, ACT_NONE, 0.0, False)
     stats = new_stats(x, per_sample)
     _lib.check(_lib.load().b200gan_norm_stats(ctypes.byref(d), x.data_ptr(), stats.data_ptr(), _stream()), "norm_stats")
     return stats
@@ -321,7 +311,7 @@ def tail_bwd(d, a, mean_rstd, scale_shift, w, g, need_affine, need_bias, round_t
 
 def norm_apply_affine(x, scale_shift, per_sample, act=ACT_NONE, slope=0.0):
     """y = act(x * scale + shift) with precomputed per-group scale/shift (eval-mode BatchNorm)."""
-    d = _norm_desc(x, per_sample, 0.0, 0.0, act, slope, False)
+    d = _norm_desc(x.shape, per_sample, 0.0, 0.0, act, slope, False)
     y = torch.empty_like(x, memory_format=CL)
     _lib.check(_lib.load().b200gan_norm_apply(ctypes.byref(d), x.data_ptr(), scale_shift.data_ptr(), y.data_ptr(),
                                               _stream()), "norm_apply")
@@ -331,7 +321,7 @@ def norm_apply_affine(x, scale_shift, per_sample, act=ACT_NONE, slope=0.0):
 def norm_backward(dy, x, y, mean_rstd, gamma, per_sample, eps, act=ACT_NONE, slope=0.0, need_params=False,
                   round_tf32=False, scale_shift=None):
     lib = _lib.load()
-    d = _norm_desc(x, per_sample, eps, 0.0, act, slope, round_tf32)
+    d = _norm_desc(x.shape, per_sample, eps, 0.0, act, slope, round_tf32)
     groups = mean_rstd.numel() // 2
     sums = zero_scratch(x.device, 2 * groups)
     dx = torch.empty_like(x, memory_format=CL)
