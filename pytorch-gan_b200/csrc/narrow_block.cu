@@ -988,6 +988,24 @@ extern "C" int b200gan_nb_supported(const b200gan_conv_geom *g) {
 }
 
 namespace b200gan {
+// the (KT, PT) instances of the staged kernels; nb_plan may name others (only through its tuning hook), which the
+// launchers refuse before they write anything
+#define NB_FPROP_INSTANCES(X) X(16, 1) X(16, 2) X(16, 4) X(8, 1) X(8, 2) X(8, 4) X(4, 1) X(4, 2) X(4, 4)
+#define NB_DGRAD_INSTANCES(X)                                                                                \
+  X(16, 1) X(16, 2) X(16, 4) X(8, 1) X(8, 2) X(8, 4) X(4, 1) X(4, 2) X(4, 4) X(6, 1) X(6, 2) X(6, 4) X(3, 1) \
+  X(3, 2) X(3, 4) X(1, 1)
+#define NB_IS_INSTANCE(KT_, PT_) if (pl.KT == KT_ && pl.PT == PT_) return true;
+static bool nb_fprop_instance(const NbPlan &pl) {
+  NB_FPROP_INSTANCES(NB_IS_INSTANCE)
+  return false;
+}
+static bool nb_dgrad_instance(const NbPlan &pl) {
+  NB_DGRAD_INSTANCES(NB_IS_INSTANCE)
+  return false;
+}
+#undef NB_IS_INSTANCE
+
+// out_stats [groups][2][K] (may be null) is zeroed here, once the call is known to launch
 static int nb_fprop2_launch(const b200gan_conv_geom *g, const NbBn &in_bn, float *rm, float *rv, long long *nbt,
                             float momentum, const float *x, const float *packed, const float *bias, int act, float slope,
                             const float *chan_scale, float *y, double *out_stats, int reflect, int rtf, int groups,
@@ -995,6 +1013,8 @@ static int nb_fprop2_launch(const b200gan_conv_geom *g, const NbBn &in_bn, float
   B2_CHECK_ARG(groups >= 1 && groups <= NB_MAX_GROUPS && g->N % groups == 0, "nb_fprop: bad statistics group count");
   const NbPlan pl = nb_plan_fprop(g, groups);
   B2_CHECK_ARG(pl.ok, "nb_fprop: no tile plan fits in shared memory");
+  B2_CHECK_ARG(nb_fprop_instance(pl), "nb_fprop: no kernel instance for KT=%d PT=%d", pl.KT, pl.PT);
+  if (out_stats) B2_CUDA(cudaMemsetAsync(out_stats, 0, (size_t)groups * 2 * g->K * sizeof(double), st));
   NbFprop2 q;
   q.x = x; q.wp = packed; q.bias = bias; q.cs = chan_scale; q.y = y; q.out_stats = out_stats;
   q.in_bn = in_bn; q.rm = rm; q.rv = rv; q.nbt = nbt; q.momentum = momentum;
@@ -1014,9 +1034,7 @@ static int nb_fprop2_launch(const b200gan_conv_geom *g, const NbBn &in_bn, float
     if (int e = ensure_dynamic_smem(nbk_fprop2_kernel<KT_, PT_>, (int)NB_SMEM_MAX, done)) return e;          \
     nbk_fprop2_kernel<KT_, PT_><<<grid, 256, pl.smem, st>>>(q);                                              \
   }
-  NB_FPROP_CASE(16, 1) NB_FPROP_CASE(16, 2) NB_FPROP_CASE(16, 4)
-  NB_FPROP_CASE(8, 1) NB_FPROP_CASE(8, 2) NB_FPROP_CASE(8, 4)
-  NB_FPROP_CASE(4, 1) NB_FPROP_CASE(4, 2) NB_FPROP_CASE(4, 4)
+  NB_FPROP_INSTANCES(NB_FPROP_CASE)
 #undef NB_FPROP_CASE
   B2_LAUNCH_CHECK();
   return B200GAN_OK;
@@ -1054,8 +1072,10 @@ extern "C" int b200gan_nb_fprop(const b200gan_conv_geom *g, const b200gan_nb_bn 
   B2_CHECK_ARG(x && packed && y, "nb_fprop: null pointer");
   B2_CHECK_ARG((((uintptr_t)x | (uintptr_t)packed | (uintptr_t)y) & 15) == 0, "nb_fprop: pointers must be 16-byte aligned");
   cudaStream_t st = as_stream(stream);
-  if (out_stats) B2_CUDA(cudaMemsetAsync(out_stats, 0, (size_t)groups * 2 * g->K * sizeof(double), st));
-  if ((int64_t)g->N * g->P * g->Q == 0) return B200GAN_OK;
+  if ((int64_t)g->N * g->P * g->Q == 0) {
+    if (out_stats) B2_CUDA(cudaMemsetAsync(out_stats, 0, (size_t)groups * 2 * g->K * sizeof(double), st));
+    return B200GAN_OK;
+  }
   return nb_fprop2_launch(g, to_bn(in_bn), running_mean, running_var, reinterpret_cast<long long *>(num_batches_tracked),
                           momentum, x, packed, bias, act, slope, chan_scale, y, out_stats, 0, 0, groups, st);
 }
@@ -1226,6 +1246,7 @@ int b200gan::nb_wgrad_reduce(const float *ws, float *dw, int elems, int nslabs, 
 }
 
 namespace b200gan {
+// sums [groups][2][C] (may be null) is zeroed here, once the call is known to launch
 static int nb_dgrad2_launch(const b200gan_conv_geom *g, const float *dz, const float *packed, const NbBn &in_bn,
                             const float *a_prev, float *g_out, double *sums, cudaStream_t st) {
   const int st_ = g->stride;
@@ -1233,6 +1254,8 @@ static int nb_dgrad2_launch(const b200gan_conv_geom *g, const float *dz, const f
   B2_CHECK_ARG(groups <= NB_MAX_GROUPS && g->N % groups == 0, "nb_dgrad: bad statistics group count");
   const NbPlan pl = nb_plan_dgrad(g, groups);
   B2_CHECK_ARG(pl.ok, "nb_dgrad: no tile plan fits in shared memory");
+  B2_CHECK_ARG(nb_dgrad_instance(pl), "nb_dgrad: no kernel instance for KT=%d PT=%d", pl.KT, pl.PT);
+  if (sums) B2_CUDA(cudaMemsetAsync(sums, 0, (size_t)groups * 2 * g->C * sizeof(double), st));
   NbDgrad2 q;
   q.dz = dz; q.wp = packed; q.a_prev = a_prev; q.g_out = g_out; q.sums = sums; q.in_bn = in_bn;
   q.N = g->N; q.H = g->H; q.W = g->W; q.C = g->C; q.P = g->P; q.Q = g->Q; q.K = g->K; q.R = g->R; q.S = g->S;
@@ -1251,12 +1274,7 @@ static int nb_dgrad2_launch(const b200gan_conv_geom *g, const float *dz, const f
     if (int e = ensure_dynamic_smem(nbk_dgrad2_kernel<KT_, PT_>, (int)NB_SMEM_MAX, done)) return e;          \
     nbk_dgrad2_kernel<KT_, PT_><<<grid, 256, pl.smem, st>>>(q);                                              \
   }
-  NB_DGRAD_CASE(16, 1) NB_DGRAD_CASE(16, 2) NB_DGRAD_CASE(16, 4)
-  NB_DGRAD_CASE(8, 1) NB_DGRAD_CASE(8, 2) NB_DGRAD_CASE(8, 4)
-  NB_DGRAD_CASE(4, 1) NB_DGRAD_CASE(4, 2) NB_DGRAD_CASE(4, 4)
-  NB_DGRAD_CASE(6, 1) NB_DGRAD_CASE(6, 2) NB_DGRAD_CASE(6, 4)
-  NB_DGRAD_CASE(3, 1) NB_DGRAD_CASE(3, 2) NB_DGRAD_CASE(3, 4)
-  NB_DGRAD_CASE(1, 1)
+  NB_DGRAD_INSTANCES(NB_DGRAD_CASE)
 #undef NB_DGRAD_CASE
   B2_LAUNCH_CHECK();
   return B200GAN_OK;
@@ -1287,9 +1305,11 @@ extern "C" int b200gan_nb_dgrad(const b200gan_conv_geom *g, const float *dz, con
   B2_CHECK_ARG(dz && packed && g_out, "nb_dgrad: null pointer");
   B2_CHECK_ARG(!sums || (in_bn && in_bn->stats && a_prev), "nb_dgrad: sums need the upstream BatchNorm and its input");
   cudaStream_t st = as_stream(stream);
-  const int dgroups = (in_bn && in_bn->stats && in_bn->groups > 1) ? in_bn->groups : 1;
-  if (sums) B2_CUDA(cudaMemsetAsync(sums, 0, (size_t)dgroups * 2 * g->C * sizeof(double), st));
-  if ((int64_t)g->N * g->H * g->W == 0) return B200GAN_OK;
+  if ((int64_t)g->N * g->H * g->W == 0) {
+    const int dgroups = (in_bn && in_bn->stats && in_bn->groups > 1) ? in_bn->groups : 1;
+    if (sums) B2_CUDA(cudaMemsetAsync(sums, 0, (size_t)dgroups * 2 * g->C * sizeof(double), st));
+    return B200GAN_OK;
+  }
   return nb_dgrad2_launch(g, dz, packed, to_bn(in_bn), a_prev, g_out, sums, st);
 }
 
