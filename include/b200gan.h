@@ -304,16 +304,6 @@ int b200gan_critic_step_mlp(const b200gan_mlp_critic_desc *d, float lambda_gp, c
                             const float *W3, const float *b3, float *losses, float *dW1, float *db1, float *dW2,
                             float *db2, float *dW3, float *db3, float *workspace, void *stream);
 
-/* ---- flat-buffer Adam (torch.optim.Adam semantics: dcgan.py:134-135) --------------------- */
-/* p -= lr * mhat / (sqrt(vhat) + eps), bias-corrected with the step count read from the
- * device (step[0] is incremented by the kernel -> CUDA-graph capturable).  lr, betas and eps
- * are doubles like torch's Python-side hyper-parameters: torch forms 1 - beta, 1 - beta^t and
- * lr / (1 - beta1^t) in double and casts them to fp32 where they meet a tensor.
- * grad_scale multiplies g first (1/world_size after an all-reduce sum). */
-int b200gan_adam_step(float *p, const float *g, float *m, float *v, int64_t n, double lr,
-                      double beta1, double beta2, double eps, float grad_scale, float *step,
-                      void *stream);
-
 /* ---- Discriminator conv blocks as a fused chain (csrc/narrow_block.cu) -------------------------------------------- */
 /* Replaces, for the narrow strided layers of dcgan.py:77-88
  *     [nn.Conv2d(in, out, 3, 2, 1), nn.LeakyReLU(0.2, inplace=True), nn.Dropout2d(0.25), nn.BatchNorm2d(out, 0.8)] x 4
@@ -383,9 +373,14 @@ int b200gan_linear1_bwd(const float *x, const float *w, const float *y, const fl
 int b200gan_bce_fwd(const float *v, const float *t, float *loss, int64_t n, void *stream);
 int b200gan_bce_bwd(const float *v, const float *t, const float *gout, float *dv, int64_t n, void *stream);
 
-/* Multi-tensor form: every parameter tensor of one optimizer in ONE launch (the table travels as a kernel argument;
- * `g` is whatever tensor autograd left in param.grad).  step: TWO floats on the device, zero-initialised by the caller:
- * step[0] = number of steps taken (advanced by the last block of the launch), step[1] = internal ticket counter. */
+/* ---- Adam (torch.optim.Adam semantics: dcgan.py:134-135) ---------------------------------------------------------- */
+/* p -= lr * mhat / (sqrt(vhat) + eps), bias-corrected with the step count read from the device.  lr, betas and eps are
+ * doubles like torch's Python-side hyper-parameters: torch forms 1 - beta, 1 - beta^t and lr / (1 - beta1^t) in double
+ * and casts them to fp32 where they meet a tensor.  grad_scale multiplies g first (1/world_size after an all-reduce
+ * sum).  Every parameter tensor of one optimizer in ONE launch per 48 tensors (the table travels as a kernel argument;
+ * `g` is whatever tensor autograd left in param.grad; n > 0).  step: TWO floats on the device, zero-initialised by the
+ * caller: step[0] = number of steps taken (advanced once per call, by the last block of the last launch -> CUDA-graph
+ * capturable; count 0 only advances it), step[1] = internal ticket counter. */
 typedef struct b200gan_adam_tensor {
   float *p;
   const float *g;

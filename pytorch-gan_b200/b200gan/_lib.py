@@ -98,7 +98,6 @@ SIGNATURES = {
     "b200gan_mlp_critic_dbwd": (c_i32, [_P(MlpCriticDesc)] + [c_vp] * 15),
     "b200gan_critic_step_workspace_floats": (c_sz, [_P(MlpCriticDesc)]),
     "b200gan_critic_step_mlp": (c_i32, [_P(MlpCriticDesc), c_f32] + [c_vp] * 18),
-    "b200gan_adam_step": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_i64, c_f64, c_f64, c_f64, c_f64, c_f32, c_vp, c_vp]),
     "b200gan_nb_supported": (c_i32, [_P(ConvGeom)]),
     "b200gan_nb_groups_supported": (c_i32, [_P(ConvGeom), c_i32]),
     "b200gan_nb_fprop": (c_i32, [_P(ConvGeom), _P(NbBn), c_vp, c_vp, c_vp, c_f32, c_vp, c_vp, c_vp, c_i32, c_f32, c_vp,

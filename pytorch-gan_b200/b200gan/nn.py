@@ -34,6 +34,10 @@ def _pair_same(v, what):
 
 def _act_of(m):
     if isinstance(m, _T["LeakyReLU"]):
+        if m.negative_slope < 0:
+            # the fused backward kernels recover the derivative from the sign of the output y, which a negative
+            # slope makes positive on the negative side as well
+            raise NotImplementedError(f"b200gan: {m} (negative_slope < 0)")
         return ACT_LRELU, float(m.negative_slope)
     if isinstance(m, _T["ReLU"]):
         return ACT_RELU, 0.0

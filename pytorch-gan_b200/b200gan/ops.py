@@ -522,11 +522,6 @@ def bce_bwd(v, t, gout):
     return dv
 
 
-def adam_step(p, g, m, v, lr, beta1, beta2, eps, grad_scale, step):
-    _lib.check(_lib.load().b200gan_adam_step(p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), p.numel(), lr,
-                                             beta1, beta2, eps, grad_scale, step.data_ptr(), _stream()), "adam_step")
-
-
 # ---- MLP critic under autograd: Linear -> LeakyReLU -> Linear -> LeakyReLU -> Linear(-> 1) (csrc/mlp_critic.cu) ------
 def _mlp_critic_desc(x, w1, w2, w3, slope):
     if x.dim() != 2 or w1.dim() != 2 or w2.dim() != 2:

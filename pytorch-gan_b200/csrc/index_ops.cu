@@ -267,28 +267,9 @@ bias_grad_kernel(const float *__restrict__ dy, const float *__restrict__ y, cons
 // meet a tensor -- (float)(1 - 0.999) is not 1.f - 0.999f (1.3e-5 apart), so they arrive here as doubles too.
 //   m = b1 m + (1-b1) g;  v = b2 v + (1-b2) g^2;  p -= step_size * m / (sqrt(v) / sqrt(1 - b2^t) + eps)
 // The step count lives on the device (CUDA-graph capturable).
-__global__ void adam_kernel(float *__restrict__ p, const float *__restrict__ g, float *__restrict__ m,
-                            float *__restrict__ v, int64_t n, double lr, double b1, double b2, double eps,
-                            float gscale, const float *__restrict__ step) {
-  const double t = (double)*step + 1.0;
-  const float neg_step_size = (float)(-(lr / (1.0 - pow(b1, t))));
-  const float bc2_sqrt = (float)sqrt(1.0 - pow(b2, t));
-  const float b1f = (float)b1, omb1 = (float)(1.0 - b1), b2f = (float)b2, omb2 = (float)(1.0 - b2);
-  const float epsf = (float)eps;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n;
-       i += (int64_t)gridDim.x * blockDim.x) {
-    float gi = g[i] * gscale;
-    float mi = b1f * m[i] + omb1 * gi;
-    float vi = b2f * v[i] + omb2 * gi * gi;
-    m[i] = mi;
-    v[i] = vi;
-    float denom = sqrtf(vi) / bc2_sqrt + epsf;
-    p[i] += neg_step_size * (mi / denom);
-  }
-}
 __global__ void adam_step_inc_kernel(float *step) { *step += 1.f; }
 
-// Multi-tensor form: ONE launch updates every parameter tensor of an optimizer.  The tensor table travels as a kernel
+// ONE launch updates every parameter tensor of an optimizer.  The tensor table travels as a kernel
 // argument (no device-side table to maintain; addresses are whatever autograd produced this step, or the fixed
 // addresses of a captured CUDA graph).  Block b works on chunk (b - block_begin[t]) of tensor t; the last block to
 // finish (atomicInc ticket, self-resetting) advances the device-side step count, so there is no second launch.
@@ -408,6 +389,8 @@ extern "C" int b200gan_pad2d_bwd(const float *dy, float *dx, int32_t N, int32_t 
                                  int32_t pad_t, int32_t pad_l, int32_t pad_b, int32_t pad_r, int32_t mode,
                                  void *stream) {
   B2_CHECK_ARG(dy && dx, "pad2d_bwd: null pointer");
+  B2_CHECK_ARG(mode != B200GAN_PAD_REFLECT || (pad_t < H && pad_b < H && pad_l < W && pad_r < W),
+               "pad2d_bwd: reflection pad must be smaller than the input");
   int Ho = H + pad_t + pad_b, Wo = W + pad_l + pad_r;
   int64_t total = (int64_t)N * H * W * C;
   if (total == 0) return B200GAN_OK;
@@ -446,23 +429,14 @@ extern "C" int b200gan_epilogue_bwd(const float *dy, const float *y, const float
   return B200GAN_OK;
 }
 
-extern "C" int b200gan_adam_step(float *p, const float *g, float *m, float *v, int64_t n, double lr,
-                                 double beta1, double beta2, double eps, float grad_scale, float *step,
-                                 void *stream) {
-  B2_CHECK_ARG(p && g && m && v && step, "adam_step: null pointer");
-  if (n > 0) {
-    adam_kernel<<<stream_blocks(n), 256, 0, as_stream(stream)>>>(p, g, m, v, n, lr, beta1, beta2, eps,
-                                                                 grad_scale, step);
-    B2_LAUNCH_CHECK();
-  }
-  adam_step_inc_kernel<<<1, 1, 0, as_stream(stream)>>>(step);
-  B2_LAUNCH_CHECK();
-  return B200GAN_OK;
-}
-
 extern "C" int b200gan_adam_multi(const b200gan_adam_tensor *tensors, int32_t count, double lr, double beta1,
                                   double beta2, double eps, float grad_scale, float *step, void *stream) {
   B2_CHECK_ARG(step != nullptr && (count == 0 || tensors != nullptr) && count >= 0, "adam_multi: bad arguments");
+  // the whole table before the first launch: a refused call updates no tensor
+  for (int i = 0; i < count; ++i) {
+    const b200gan_adam_tensor &t = tensors[i];
+    B2_CHECK_ARG(t.p && t.g && t.m && t.v && t.n > 0, "adam_multi: tensor %d has a null pointer or no elements", i);
+  }
   cudaStream_t st = as_stream(stream);
   if (count == 0) {
     adam_step_inc_kernel<<<1, 1, 0, st>>>(step);
@@ -475,7 +449,6 @@ extern "C" int b200gan_adam_multi(const b200gan_adam_tensor *tensors, int32_t co
     int blocks = 0;
     for (int i = 0; i < c; ++i) {
       const b200gan_adam_tensor &t = tensors[base + i];
-      B2_CHECK_ARG(t.p && t.g && t.m && t.v && t.n > 0, "adam_multi: tensor %d has a null pointer or no elements", base + i);
       tb.p[i] = t.p; tb.g[i] = t.g; tb.m[i] = t.m; tb.v[i] = t.v; tb.n[i] = t.n;
       tb.block_begin[i] = blocks;
       blocks += (int)ceil_div64(t.n, ADAM_CHUNK);

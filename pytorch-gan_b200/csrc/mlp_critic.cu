@@ -194,7 +194,7 @@ __global__ void __launch_bounds__(256) mlp_critic_dbwd_kernel(McDbwdP p) {
 //   A1 penalty rows <- t = coef * (gx W1^T) * m1;     dW2 = U2^T A1 = dh2^T a1 + g2^T t
 //   A2 penalty rows <- (t W2^T) * m2;                 dW3 = sum_r dout_r * A2_r
 // with gx = dD/dx, r_n = ||gx_n||_2, the penalty term lambda * mean((r - 1)^2) and coef_n = lambda * (2/N) (r_n - 1) / r_n
-// (the term's derivative w.r.t. r_n, over r_n).
+// (the term's derivative w.r.t. r_n, over r_n), and coef_n = 0 where r_n = 0.
 // Bias gradients come from the real/fake rows only (the penalty does not depend on the biases).
 struct CsP {
   int N, Din, H1, H2;
@@ -271,7 +271,8 @@ __global__ void __launch_bounds__(256, 4) critic_step_kernel(CsP p) {
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
       const float r = sqrtf(s);
-      const float c = p.lambda_gp * (2.f / (float)N) * (r - 1.f) / r;
+      // r = 0 (a zero input gradient): torch's norm backward passes 0 there, and 0 * (-inf) would be NaN
+      const float c = r == 0.f ? 0.f : p.lambda_gp * (2.f / (float)N) * (r - 1.f) / r;
       if (lane == 0) {
         p.coef[n] = c;
         const float term = p.lambda_gp * (r - 1.f) * (r - 1.f) / (float)N;

@@ -194,3 +194,13 @@ def test_grouped_discriminator_pass_eligibility_is_decided_on_the_host():
     g2, _ = ops.make_geom((8, 64, 8, 8), (128, 64, 3, 3), 2, (1, 1, 1, 1))
     assert lib.b200gan_nb_groups_supported(ctypes.byref(g2), 2) == 1
     assert lib.b200gan_nb_groups_supported(ctypes.byref(g2), 5) == 0  # more groups than the kernels take
+
+
+def test_negative_leaky_relu_slope_is_refused():
+    """the fused backward kernels take LeakyReLU's derivative from the sign of its output y: with a negative slope y is
+    positive on the negative side too, so such a module is refused rather than given the derivative 1 there"""
+    from b200gan import nn as bnn
+    with pytest.raises(NotImplementedError):
+        bnn._act_of(torch.nn.LeakyReLU(-0.1))
+    assert bnn._act_of(torch.nn.LeakyReLU(0.2)) == (bnn.ACT_LRELU, 0.2)
+    assert bnn._act_of(torch.nn.LeakyReLU(0.0)) == (bnn.ACT_LRELU, 0.0)

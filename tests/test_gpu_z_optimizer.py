@@ -1,5 +1,5 @@
-"""GPU parity of the flat-buffer Adam entry point (b200gan_adam_step) against torch.optim.Adam with the reference's
-hyper-parameters (dcgan.py:134-135: lr 2e-4, betas (0.5, 0.999), eps 1e-8, no weight decay, no amsgrad)."""
+"""GPU parity of b200gan.optim.Adam (b200gan_adam_multi) against torch.optim.Adam with the reference's hyper-parameters
+(dcgan.py:134-135: lr 2e-4, betas (0.5, 0.999), eps 1e-8, no weight decay, no amsgrad)."""
 import itertools
 
 import pytest
@@ -11,8 +11,9 @@ pytestmark = pytest.mark.gpu
 
 
 @pytest.mark.parametrize("n", [1, 1000, 100003])
-def test_flat_adam_matches_torch_adam(n):
-    from b200gan import ops
+def test_one_tensor_adam_matches_torch_adam(n):
+    """one parameter tensor of n elements through optim.Adam, five steps"""
+    from b200gan import optim
     torch.manual_seed(5)
     p0 = torch.randn(n, device="cuda")
     grads = [torch.randn(n, device="cuda") * (0.1 + i) for i in range(5)]
@@ -23,35 +24,38 @@ def test_flat_adam_matches_torch_adam(n):
         pr.grad = g.clone()
         opt.step()
 
-    p, m, v = p0.clone(), torch.zeros(n, device="cuda"), torch.zeros(n, device="cuda")
-    step = torch.zeros(1, device="cuda")
+    p = torch.nn.Parameter(p0.clone())
+    ours = optim.Adam([p], lr=2e-4, betas=(0.5, 0.999), eps=1e-8)
     for g in grads:
-        ops.adam_step(p, g, m, v, 2e-4, 0.5, 0.999, 1e-8, 1.0, step)
-    assert step.item() == 5.0  # the step count lives on the device (CUDA-graph capturable)
-    st = opt.state[pr]
-    assert rel_err(m, st["exp_avg"]) < 1e-6
-    assert rel_err(v, st["exp_avg_sq"]) < 1e-6
+        p.grad = g.clone()
+        ours.step()
+    so, st = ours.state[p], opt.state[pr]
+    assert so["step"].item() == 5.0  # the step count lives on the device (CUDA-graph capturable)
+    assert rel_err(so["exp_avg"], st["exp_avg"]) < 1e-6
+    assert rel_err(so["exp_avg_sq"], st["exp_avg_sq"]) < 1e-6
     # parameters: within 5 fp32 ulps / 1e-8 of torch's after five steps (the two differ only in FMA contraction of the
     # moment updates, i.e. by at most one rounding of p per step)
-    assert torch.allclose(p, pr.detach(), rtol=6e-7, atol=1e-8)
+    assert torch.allclose(p.detach(), pr.detach(), rtol=6e-7, atol=1e-8)
     # and the accumulated update itself (~1e-3 of |p|, so one ulp of p is ~1e-4 of it): 4 significant digits over
     # the whole vector; an fp32 CPU emulation of the kernel's arithmetic sits at 2.5e-6
     if n >= 1000:
-        assert rel_err(p - p0, pr.detach() - p0) < 2e-4
+        assert rel_err(p.detach() - p0, pr.detach() - p0) < 2e-4
 
 
-def test_flat_adam_grad_scale_is_the_all_reduce_average():
+def test_adam_grad_scale_is_the_all_reduce_average():
     """grad_scale = 1/world_size folds the averaging of an all-reduce(sum) into the update (b200gan/ddp.py)."""
-    from b200gan import ops
+    from b200gan import optim
     torch.manual_seed(6)
     n = 4097
     p0, g = torch.randn(n, device="cuda"), torch.randn(n, device="cuda")
     outs = []
     for grad, scale in ((g * 4.0, 0.25), (g, 1.0)):
-        p, m, v = p0.clone(), torch.zeros(n, device="cuda"), torch.zeros(n, device="cuda")
-        step = torch.zeros(1, device="cuda")
-        ops.adam_step(p, grad, m, v, 2e-4, 0.5, 0.999, 1e-8, scale, step)
-        outs.append((p, m, v))
+        p = torch.nn.Parameter(p0.clone())
+        ours = optim.Adam([p], lr=2e-4, betas=(0.5, 0.999))
+        ours.grad_scale = scale
+        p.grad = grad.clone()
+        ours.step()
+        outs.append((p.detach(), ours.state[p]["exp_avg"], ours.state[p]["exp_avg_sq"]))
     for a, b in zip(*outs):
         assert torch.equal(a, b)  # x4 and x0.25 are exact in binary floating point
 
