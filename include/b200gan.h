@@ -304,6 +304,56 @@ int b200gan_critic_step_mlp(const b200gan_mlp_critic_desc *d, float lambda_gp, c
                             const float *W3, const float *b3, float *losses, float *dW1, float *db1, float *dW2,
                             float *db2, float *dW3, float *db3, float *workspace, void *stream);
 
+/* ---- MLP generator: forward and backward (csrc/mlp_generator/mlp_generator.cu) ------------------------------------ */
+/* The MLP generator of wgan_gp.py:42-65 / gan.py:38-61 (Linear weights W[l][width[l+1]][width[l]], biases b[l]):
+ *   a_{-1} = z [N][width[0]]
+ *   h_l = a_{l-1} W_l^T + b_l;  y_l = BatchNorm1d_l(h_l) when has_norm[l], else h_l;  a_l = lrelu(y_l)     l < L - 1
+ *   out = tanh(a_{L-2} W_{L-1}^T + b_{L-1})                                                  [N][width[L]]
+ * BatchNorm1d in training mode: batch mean and biased variance, y = gamma (h - mean) / sqrt(var + eps) + beta; the
+ * running statistics (when the three pointers are non-NULL) are updated on the device with torch's rule,
+ *   running_mean = (1 - momentum) running_mean + momentum mean,
+ *   running_var  = (1 - momentum) running_var  + momentum var N / (N - 1),   num_batches_tracked += 1,
+ * so a call can be captured in a CUDA graph.  One LeakyReLU slope >= 0, one eps and one momentum for every layer.
+ * Each call is ONE cooperative launch of 32 x 32 fp32 FFMA tiles; every output element and column sum is formed in a
+ * fixed order, so results are bit-identical from call to call and do not depend on the grid size.
+ * Limits: 1 <= L <= B200GAN_MLP_GEN_MAX_LAYERS; 1 <= width <= B200GAN_MLP_GEN_MAX_WIDTH; 1 <= N <=
+ * B200GAN_MLP_GEN_MAX_N, and N >= 2 when a layer has a norm (torch refuses one value per channel in training).  The
+ * column statistics run one thread per column over all N rows, which bounds N; the reference sizes are N 64 with
+ * widths 100 -> 128 -> 256 -> 512 -> 1024 -> 1024 (wgan_gp.py, 32 x 32) or -> 784 (gan.py, 28 x 28). */
+#define B200GAN_MLP_GEN_MAX_LAYERS 8
+#define B200GAN_MLP_GEN_MAX_WIDTH 8192
+#define B200GAN_MLP_GEN_MAX_N 8192
+typedef struct b200gan_mlp_gen_desc {
+  int32_t L, N;
+  int32_t width[B200GAN_MLP_GEN_MAX_LAYERS + 1];
+  int32_t has_norm[B200GAN_MLP_GEN_MAX_LAYERS];    /* only l < L - 1 may be set */
+  float slope, eps, momentum;
+  const float *W[B200GAN_MLP_GEN_MAX_LAYERS], *b[B200GAN_MLP_GEN_MAX_LAYERS];
+  const float *gamma[B200GAN_MLP_GEN_MAX_LAYERS], *beta[B200GAN_MLP_GEN_MAX_LAYERS];  /* norm layers: non-NULL */
+  float *running_mean[B200GAN_MLP_GEN_MAX_LAYERS], *running_var[B200GAN_MLP_GEN_MAX_LAYERS];
+  int64_t *num_batches_tracked[B200GAN_MLP_GEN_MAX_LAYERS];
+} b200gan_mlp_gen_desc;
+/* Gradients of the backward, all OVERWRITTEN; each may be NULL and is then not computed (norm layers only for dgamma
+ * and dbeta). */
+typedef struct b200gan_mlp_gen_grads {
+  float *dW[B200GAN_MLP_GEN_MAX_LAYERS], *db[B200GAN_MLP_GEN_MAX_LAYERS];
+  float *dgamma[B200GAN_MLP_GEN_MAX_LAYERS], *dbeta[B200GAN_MLP_GEN_MAX_LAYERS];
+} b200gan_mlp_gen_grads;
+/* What the backward reads from the forward, in this order: a_l [N][width[l+1]] for l < L - 1, then for each norm layer
+ * xhat_l = (h_l - mean) / sqrt(var + eps) [N][width[l+1]], then for each norm layer 1 / sqrt(var + eps) [width[l+1]]. */
+size_t b200gan_mlp_gen_saved_floats(const b200gan_mlp_gen_desc *d);
+/* Scratch of both passes: 3 N max(width[1..L]) floats. */
+size_t b200gan_mlp_gen_workspace_floats(const b200gan_mlp_gen_desc *d);
+/* out [N][width[L]].  saved: b200gan_mlp_gen_saved_floats() floats for a later backward, or NULL (a forward under
+ * torch.no_grad(): only out and the running statistics are written). */
+int b200gan_mlp_gen_fwd(const b200gan_mlp_gen_desc *d, const float *z, float *out, float *saved, float *workspace,
+                        void *stream);
+/* Backward for the output gradient dout [N][width[L]], from z, the forward's out and saved; dz [N][width[0]] may be
+ * NULL. */
+int b200gan_mlp_gen_bwd(const b200gan_mlp_gen_desc *d, const float *dout, const float *z, const float *out,
+                        const float *saved, float *dz, const b200gan_mlp_gen_grads *grads, float *workspace,
+                        void *stream);
+
 /* ---- Discriminator conv blocks as a fused chain (csrc/narrow_block.cu) -------------------------------------------- */
 /* Replaces, for the narrow strided layers of dcgan.py:77-88
  *     [nn.Conv2d(in, out, 3, 2, 1), nn.LeakyReLU(0.2, inplace=True), nn.Dropout2d(0.25), nn.BatchNorm2d(out, 0.8)] x 4

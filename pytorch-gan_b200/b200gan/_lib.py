@@ -41,6 +41,20 @@ class MlpCriticDesc(ctypes.Structure):
     _fields_ = [("N", c_i32), ("Din", c_i32), ("H1", c_i32), ("H2", c_i32), ("slope", c_f32)]
 
 
+MLP_GEN_MAX_LAYERS, MLP_GEN_MAX_WIDTH, MLP_GEN_MAX_N = 8, 8192, 8192
+
+
+class MlpGenDesc(ctypes.Structure):
+    _fields_ = [("L", c_i32), ("N", c_i32), ("width", c_i32 * (MLP_GEN_MAX_LAYERS + 1)),
+                ("has_norm", c_i32 * MLP_GEN_MAX_LAYERS), ("slope", c_f32), ("eps", c_f32), ("momentum", c_f32)] + [
+        (n, c_vp * MLP_GEN_MAX_LAYERS)
+        for n in ("W", "b", "gamma", "beta", "running_mean", "running_var", "num_batches_tracked")]
+
+
+class MlpGenGrads(ctypes.Structure):
+    _fields_ = [(n, c_vp * MLP_GEN_MAX_LAYERS) for n in ("dW", "db", "dgamma", "dbeta")]
+
+
 class PackJob(ctypes.Structure):
     _fields_ = [("w", c_vp), ("packed", c_vp), ("geom", ConvGeom), ("pack", c_i32)]
 
@@ -98,6 +112,10 @@ SIGNATURES = {
     "b200gan_mlp_critic_dbwd": (c_i32, [_P(MlpCriticDesc)] + [c_vp] * 15),
     "b200gan_critic_step_workspace_floats": (c_sz, [_P(MlpCriticDesc)]),
     "b200gan_critic_step_mlp": (c_i32, [_P(MlpCriticDesc), c_f32] + [c_vp] * 18),
+    "b200gan_mlp_gen_saved_floats": (c_sz, [_P(MlpGenDesc)]),
+    "b200gan_mlp_gen_workspace_floats": (c_sz, [_P(MlpGenDesc)]),
+    "b200gan_mlp_gen_fwd": (c_i32, [_P(MlpGenDesc)] + [c_vp] * 5),
+    "b200gan_mlp_gen_bwd": (c_i32, [_P(MlpGenDesc)] + [c_vp] * 5 + [_P(MlpGenGrads), c_vp, c_vp]),
     "b200gan_nb_supported": (c_i32, [_P(ConvGeom)]),
     "b200gan_nb_groups_supported": (c_i32, [_P(ConvGeom), c_i32]),
     "b200gan_nb_fprop": (c_i32, [_P(ConvGeom), _P(NbBn), c_vp, c_vp, c_vp, c_f32, c_vp, c_vp, c_vp, c_i32, c_f32, c_vp,

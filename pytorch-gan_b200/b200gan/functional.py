@@ -708,3 +708,78 @@ class MlpCriticGradFn(torch.autograd.Function):
 def mlp_critic(x, l1, l2, l3, slope):
     """Linear l1 -> LeakyReLU(slope) -> Linear l2 -> LeakyReLU(slope) -> Linear l3 (-> 1) on x [N, Din] as MlpCriticFn."""
     return MlpCriticFn.apply(x, l1.weight, l1.bias, l2.weight, l2.bias, l3.weight, l3.bias, float(slope))
+
+
+# ---- the MLP generator under autograd (csrc/mlp_generator) --------------------------------------------------------
+class MlpGenSpec:
+    """The non-tensor half of a generator call: per layer whether a BatchNorm1d follows its Linear and that norm's
+    running-statistics buffers (updated in place by the forward), and the slope, eps and momentum shared by all."""
+
+    def __init__(self, norms, slope, eps, momentum):
+        self.norms = norms          # per layer: (running_mean, running_var, num_batches_tracked) or None
+        self.slope, self.eps, self.momentum = float(slope), float(eps), float(momentum)
+
+    def layers(self, params):
+        """[(W, b, norm)] for ops.mlp_gen_*, from the flat parameter list W0, b0, [gamma0, beta0], W1, ..."""
+        out, i = [], 0
+        for norm in self.norms:
+            w, b = params[i], params[i + 1]
+            i += 2
+            if norm is not None:
+                out.append((w, b, (params[i], params[i + 1], *norm)))
+                i += 2
+            else:
+                out.append((w, b, None))
+        return out
+
+
+class MlpGeneratorFn(torch.autograd.Function):
+    """G(z) = tanh(W_L ... lrelu(BatchNorm1d(W_1 lrelu(W_0 z + b_0) + b_1)) ... + b_L) (wgan_gp.py:42-65, gan.py:38-61):
+    one launch forward, one launch backward.  Inputs: z, the spec, then W, b (and gamma, beta after a norm) per layer."""
+
+    @staticmethod
+    def forward(ctx, z, spec, *params):
+        out, saved = ops.mlp_gen_fwd(z.detach(), spec.layers([p.detach() for p in params]), spec.slope, spec.eps,
+                                     spec.momentum, keep=True)
+        ctx.spec = spec
+        ctx.save_for_backward(z, out, saved, *params)
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        if torch.is_grad_enabled():
+            raise NotImplementedError("b200gan: the fused MLP generator is not twice differentiable (create_graph=True)")
+        z, out, saved, *params = ctx.saved_tensors
+        spec = ctx.spec
+        nig = ctx.needs_input_grad
+        need, i = [], 2
+        for norm in spec.norms:
+            k = 4 if norm is not None else 2
+            need.append(tuple(nig[i:i + k]) + (False,) * (4 - k))
+            i += k
+        dz, grads = ops.mlp_gen_bwd(dout.contiguous(), z.detach(), out, saved, spec.layers([p.detach() for p in params]),
+                                    spec.slope, spec.eps, spec.momentum, nig[0], need)
+        flat = []
+        for norm, g in zip(spec.norms, grads):
+            flat += list(g if norm is not None else g[:2])
+        return (dz, None, *flat)
+
+
+def mlp_generator(z, layers, slope):
+    """layers: [(Linear, BatchNorm1d or None)] (nn.mlp_generator_layers) on z [N, width[0]]: Linear -> (norm) ->
+    LeakyReLU(slope) blocks, the last Linear -> Tanh.  Without autograd (torch.no_grad(), nothing requiring grad) the
+    forward keeps nothing for a backward."""
+    params, norms, eps, momentum = [], [], 0.0, 0.0
+    for lin, bn in layers:
+        params += [lin.weight, lin.bias]
+        if bn is not None:
+            params += [bn.weight, bn.bias]
+            norms.append((bn.running_mean, bn.running_var, bn.num_batches_tracked))
+            eps, momentum = bn.eps, bn.momentum
+        else:
+            norms.append(None)
+    spec = MlpGenSpec(norms, slope, eps, momentum)
+    if torch.is_grad_enabled() and (z.requires_grad or any(p.requires_grad for p in params)):
+        return MlpGeneratorFn.apply(z, spec, *params)
+    return ops.mlp_gen_fwd(z, spec.layers([p.detach() for p in params]), spec.slope, spec.eps, spec.momentum,
+                           keep=False)[0]

@@ -12,6 +12,7 @@ There is no CPU / cuDNN fallback for the conv and norm modules: CPU tensors rais
 import torch
 import torch.nn as tnn
 
+from . import _lib
 from . import functional as F
 from . import ops
 from ._lib import (ACT_LRELU, ACT_NONE, ACT_RELU, ACT_SIGMOID, ACT_TANH, PAD_REFLECT, PAD_ZERO)
@@ -20,7 +21,8 @@ from .functional import ConvSpec, NormSpec, PackCache
 _T = {  # the stock classes, captured before any patching
     n: getattr(tnn, n) for n in (
         "Conv2d", "ConvTranspose2d", "BatchNorm2d", "InstanceNorm2d", "LeakyReLU", "ReLU", "Tanh", "Sigmoid",
-        "Upsample", "ZeroPad2d", "ReflectionPad2d", "Dropout", "Dropout2d", "Sequential", "Linear", "BCELoss")
+        "Upsample", "ZeroPad2d", "ReflectionPad2d", "Dropout", "Dropout2d", "Sequential", "Linear", "BCELoss",
+        "BatchNorm1d")
 }
 
 
@@ -286,6 +288,12 @@ class Linear(_T["Linear"]):
         return super().forward(x)
 
 
+class BatchNorm1d(_T["BatchNorm1d"]):
+    """nn.BatchNorm1d, same state_dict.  Inside the MLP generator pattern of a Sequential (mlp_generator_layers,
+    wgan_gp.py:42-65, gan.py:38-61) it runs in the fused generator kernels; anywhere else, and on the CPU, it is the stock
+    module."""
+
+
 class BCELoss(_T["BCELoss"]):
     def forward(self, input, target):
         if (input.is_cuda and input.dtype == torch.float32 and self.reduction == "mean" and self.weight is None
@@ -544,6 +552,54 @@ def mlp_critic_layers(mods, in_features):
     return l1, l2, l3, float(mods[1].negative_slope)
 
 
+def mlp_generator_layers(mods, in_features):
+    """([(Linear, BatchNorm1d or None)], slope) if the module list `mods` is the MLP generator of wgan_gp.py:42-65 /
+    gan.py:38-61 -- [Linear -> (BatchNorm1d)? -> LeakyReLU(s)] x (L - 1), Linear -> Tanh, at most 8 Linears of at most
+    8192 features, all with biases, chained widths from in_features, one slope >= 0 -- which runs as
+    functional.MlpGeneratorFn; else None.  Every BatchNorm1d is in training mode, affine, with tracked running statistics and a momentum (not None), all with
+    one eps and one momentum: what the kernels compute.  A last Linear with one output stays with the Linear(K, 1) + Tanh
+    head kernel.  Stock or drop-in classes only, without hooks.  No side effects."""
+    def plain(m, name):  # the stock class or its drop-in, with no hooks that calling the module would run
+        return (type(m) in (_T[name], REPLACEMENTS[name]) and not m._forward_hooks and not m._forward_pre_hooks
+                and not m._backward_hooks)
+
+    layers, slopes, norms, i, width = [], set(), [], 0, in_features
+    while i < len(mods):
+        lin = mods[i]
+        if not plain(lin, "Linear") or lin.bias is None or lin.in_features != width:
+            return None
+        width, i = lin.out_features, i + 1
+        if i + 1 == len(mods):  # the output layer
+            if not plain(mods[i], "Tanh") or width == 1:
+                return None
+            layers.append((lin, None))
+            break
+        bn = None
+        if i < len(mods) and plain(mods[i], "BatchNorm1d"):
+            bn = mods[i]
+            if not (bn.training and bn.affine and bn.track_running_stats and bn.running_mean is not None
+                    and bn.momentum is not None and bn.num_features == width):
+                return None
+            norms.append((bn.eps, bn.momentum))
+            i += 1
+        if i >= len(mods) or not plain(mods[i], "LeakyReLU"):
+            return None
+        slopes.add(mods[i].negative_slope)
+        layers.append((lin, bn))
+        i += 1
+    else:
+        return None
+    widths = [in_features] + [lin.out_features for lin, _ in layers]
+    if len(layers) > _lib.MLP_GEN_MAX_LAYERS or max(widths) > _lib.MLP_GEN_MAX_WIDTH:
+        return None
+    if len(slopes) > 1 or len(set(norms)) > 1:
+        return None
+    slope = slopes.pop() if slopes else 0.0
+    if slope < 0:
+        return None
+    return layers, float(slope)
+
+
 class Sequential(_T["Sequential"]):
     def _plan(self):
         mods = list(self._modules.values())
@@ -618,6 +674,11 @@ class Sequential(_T["Sequential"]):
         critic = mlp_critic_layers(mods, x.shape[1])
         if critic is not None and x.shape[0] >= 1:
             return F.mlp_critic(x, *critic)
+        gen = mlp_generator_layers(mods, x.shape[1])
+        # one row with a norm: the stock BatchNorm1d raises torch's own ValueError on the leaf-by-leaf path below
+        if gen is not None and (x.shape[0] >= 2 or all(bn is None for _, bn in gen[0])) \
+                and x.shape[0] <= _lib.MLP_GEN_MAX_N:
+            return F.mlp_generator(x, *gen)
         i = 0
         while i < len(mods):
             m = mods[i]
@@ -709,7 +770,7 @@ REPLACEMENTS = {
     "Conv2d": Conv2d, "ConvTranspose2d": ConvTranspose2d, "BatchNorm2d": BatchNorm2d,
     "InstanceNorm2d": InstanceNorm2d, "LeakyReLU": LeakyReLU, "ReLU": ReLU, "Tanh": Tanh, "Sigmoid": Sigmoid,
     "Upsample": Upsample, "ZeroPad2d": ZeroPad2d, "ReflectionPad2d": ReflectionPad2d, "Dropout": Dropout,
-    "Dropout2d": Dropout2d, "Sequential": Sequential, "Linear": Linear, "BCELoss": BCELoss,
+    "Dropout2d": Dropout2d, "Sequential": Sequential, "Linear": Linear, "BCELoss": BCELoss, "BatchNorm1d": BatchNorm1d,
 }
 for _n, _c in REPLACEMENTS.items():
     _c.__name__ = _n

@@ -12,7 +12,7 @@ import torch
 from . import _lib
 from ._lib import (ACT_NONE, ALGO_AUTO, ALGO_SIMT, ALGO_TC, PACK_SIMT_DGRAD, PACK_SIMT_FPROP, PACK_TC_DGRAD,
                    PACK_TC_DGRAD_UP2, PACK_TC_FPROP, PACK_TC_FPROP_UP2, PAD_REFLECT, PAD_ZERO, ConvGeom, Epilogue,
-                   MlpCriticDesc, NbBn, NormDesc, TailDesc)
+                   MlpCriticDesc, MlpGenDesc, MlpGenGrads, NbBn, NormDesc, TailDesc)
 
 CL = torch.channels_last
 
@@ -617,3 +617,70 @@ def critic_step_mlp(real, fake, alpha, w1, b1, w2, b2, w3, b3, slope, lambda_gp)
                                            w3.data_ptr(), b3.data_ptr(), losses.data_ptr(),
                                            *[g.data_ptr() for g in grads], ws.data_ptr(), _stream()), "critic_step_mlp")
     return (losses, *grads)
+
+
+# ---- MLP generator: [Linear -> (BatchNorm1d)? -> LeakyReLU] x (L - 1), Linear -> Tanh (csrc/mlp_generator) ----------
+def _mlp_gen_desc(z, layers, slope, eps, momentum):
+    """layers: [(W, b, norm)] with norm = (gamma, beta, running_mean, running_var, num_batches_tracked) or None; the
+    running statistics may be None (not tracked)."""
+    if z.dim() != 2 or not 1 <= len(layers) <= _lib.MLP_GEN_MAX_LAYERS:
+        raise RuntimeError(f"b200gan mlp_gen: z must be a matrix and 1 <= layers <= {_lib.MLP_GEN_MAX_LAYERS}")
+    d = MlpGenDesc()
+    d.L, d.N = len(layers), z.shape[0]
+    d.width[0] = z.shape[1]
+    d.slope, d.eps, d.momentum = float(slope), float(eps), float(momentum)
+    for l, (w, b, norm) in enumerate(layers):
+        if w.dim() != 2 or w.shape[1] != d.width[l] or (b is not None and b.numel() != w.shape[0]):
+            raise RuntimeError(f"b200gan mlp_gen: layer {l}: W {tuple(w.shape)} does not chain from width {d.width[l]}")
+        d.width[l + 1] = w.shape[0]
+        d.W[l], d.b[l] = w.data_ptr(), _ptr(b)
+        if norm is not None:
+            d.has_norm[l] = 1
+            for name, t_ in zip(("gamma", "beta", "running_mean", "running_var", "num_batches_tracked"), norm):
+                getattr(d, name)[l] = _ptr(t_)
+    return d
+
+
+def mlp_gen_fwd(z, layers, slope, eps, momentum, keep):
+    """The generator's forward in one launch; updates the running statistics in place.  Returns (out [N, width[L]],
+    saved): saved is what mlp_gen_bwd reads (see b200gan_mlp_gen_saved_floats in include/b200gan.h) when keep, else
+    None."""
+    z = _f32("mlp_gen operand", z)[0]
+    layers = [(*_f32("mlp_gen operand", w, b), None if n is None else (*_f32("mlp_gen operand", *n[:4]), n[4]))
+              for w, b, n in layers]
+    d = _mlp_gen_desc(z, layers, slope, eps, momentum)
+    lib, dev = _lib.load(), z.device
+    out = torch.empty((d.N, d.width[d.L]), device=dev, dtype=torch.float32)
+    saved = torch.empty(lib.b200gan_mlp_gen_saved_floats(ctypes.byref(d)), device=dev, dtype=torch.float32) if keep \
+        else None
+    ws = torch.empty(lib.b200gan_mlp_gen_workspace_floats(ctypes.byref(d)), device=dev, dtype=torch.float32)
+    _lib.check(lib.b200gan_mlp_gen_fwd(ctypes.byref(d), z.data_ptr(), out.data_ptr(), _ptr(saved), ws.data_ptr(),
+                                       _stream()), "mlp_gen_fwd")
+    return out, saved
+
+
+def mlp_gen_bwd(dout, z, out, saved, layers, slope, eps, momentum, need_dz, need):
+    """Backward of mlp_gen_fwd for the output gradient dout.  need: per layer 4 flags for (dW, db, dgamma, dbeta).
+    Returns (dz or None, [(dW, db, dgamma, dbeta)] with None where not needed or where the layer has no norm)."""
+    dout, z, out = _f32("mlp_gen operand", dout, z, out)
+    layers = [(*_f32("mlp_gen operand", w), None, None if n is None else (*_f32("mlp_gen operand", *n[:2]),
+                                                                          None, None, None))
+              for w, _, n in layers]
+    d = _mlp_gen_desc(z, layers, slope, eps, momentum)
+    if dout.shape != (d.N, d.width[d.L]) or out.shape != dout.shape:
+        raise RuntimeError("b200gan mlp_gen_bwd: dout / out do not match the layers")
+    lib, dev, f32 = _lib.load(), z.device, torch.float32
+    gr = MlpGenGrads()
+    grads = []
+    for l, ((w, _, norm), flags) in enumerate(zip(layers, need)):
+        shapes = (tuple(w.shape), (w.shape[0],), (w.shape[0],), (w.shape[0],))
+        row = [torch.empty(s_, device=dev, dtype=f32) if f and (k < 2 or norm is not None) else None
+               for k, (s_, f) in enumerate(zip(shapes, flags))]
+        for name, t_ in zip(("dW", "db", "dgamma", "dbeta"), row):
+            getattr(gr, name)[l] = _ptr(t_)
+        grads.append(tuple(row))
+    dz = torch.empty_like(z) if need_dz else None
+    ws = torch.empty(lib.b200gan_mlp_gen_workspace_floats(ctypes.byref(d)), device=dev, dtype=f32)
+    _lib.check(lib.b200gan_mlp_gen_bwd(ctypes.byref(d), dout.data_ptr(), z.data_ptr(), out.data_ptr(), _ptr(saved),
+                                       _ptr(dz), ctypes.byref(gr), ws.data_ptr(), _stream()), "mlp_gen_bwd")
+    return dz, grads

@@ -24,13 +24,21 @@ FLAGS = [
 ]
 
 
+def _files():
+    """Every file under csrc/, at any depth, as a path relative to it."""
+    out = []
+    for d, _, names in os.walk(CSRC):
+        out += [os.path.relpath(os.path.join(d, n), CSRC) for n in names]
+    return sorted(out)
+
+
 def sources():
-    return sorted(f for f in os.listdir(CSRC) if f.endswith(".cu"))
+    return [f for f in _files() if f.endswith(".cu")]
 
 
 def digest():
     h = hashlib.sha256()
-    for f in sorted(os.listdir(CSRC)) + ["../../include/b200gan.h"]:
+    for f in _files() + ["../../include/b200gan.h"]:
         with open(os.path.join(CSRC, f), "rb") as fh:
             h.update(f.encode())
             h.update(fh.read())
@@ -50,7 +58,7 @@ def build(force=False, verbose=False):
         raise RuntimeError("nvcc not found and no prebuilt libb200gan.so")
 
     def compile_one(src):
-        obj = os.path.join(OBJ, src.replace(".cu", ".o"))
+        obj = os.path.join(OBJ, src.replace(os.sep, "_").replace(".cu", ".o"))
         cmd = [NVCC, *FLAGS, "-c", os.path.join(CSRC, src), "-o", obj]
         if verbose:
             cmd.insert(1, "-Xptxas=-v")

@@ -1,4 +1,5 @@
-// tile_gemm.cuh -- the 32x32 fp32 FFMA tile GEMM of the cooperative MLP-critic kernels (mlp_critic.cu).
+// tile_gemm.cuh -- the 32x32 fp32 FFMA tile GEMM of the cooperative MLP kernels (mlp_critic.cu,
+// mlp_generator/mlp_generator.cu).
 // Each phase of those kernels spreads the 32x32 output tiles of one or two small GEMMs over a persistent grid.
 #pragma once
 #include <cuda_runtime.h>
