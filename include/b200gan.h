@@ -149,6 +149,10 @@ int b200gan_conv2d_dgrad(const b200gan_conv_geom *g, const float *dy, const floa
 size_t b200gan_conv2d_wgrad_workspace_floats(const b200gan_conv_geom *g, int algo);
 int b200gan_conv2d_wgrad(const b200gan_conv_geom *g, const float *x, const float *dy, float *dw,
                          float *db, float *workspace, int algo, void *stream);
+/* The same, except that on the tensor-core route of a Conv2d db is summed by the weight-gradient kernel from the dy
+ * values it already holds, instead of by a separate pass over dy (the other routes and ConvTranspose2d: as above). */
+int b200gan_conv2d_wgrad_fused_bias(const b200gan_conv_geom *g, const float *x, const float *dy, float *dw,
+                                    float *db, float *workspace, int algo, void *stream);
 
 /* dz = dy * act'(y) * chan_scale  -- backward of the fused fprop epilogue, from the saved
  * output y (LeakyReLU/ReLU sign and Tanh/Sigmoid derivative are functions of y).
@@ -198,6 +202,23 @@ int b200gan_norm_apply(const b200gan_norm_desc *d, const float *x, const float *
 int b200gan_norm_bwd(const b200gan_norm_desc *d, const float *dy, const float *x, const float *y,
                      const float *mean_rstd, const float *scale_shift, const float *gamma, double *sums, float *dx,
                      float *dgamma_dbeta, void *stream);
+
+/* ---- BatchNorm2d [-> LeakyReLU / ReLU] [-> Upsample x2] -> Conv2d backward (dcgan.py:53-55,56-59) ------------------ */
+/* The conv's data gradient dx as b200gan_conv2d_dgrad (ALGO_TC, packed PACK_TC_DGRAD[_UP2]) writes it, bit for bit, and
+ * in the same epilogue the sums the norm backward needs: sums[0..C) += sum dy', sums[C..2C) += sum dy' * xhat, with
+ * dy' = dx * act'(x * scale + shift) and xhat = (x - mean) * rstd.  x: the norm input [N][H][W][C] (the conv's input
+ * grid); d: the norm (per_sample 0, act NONE / LRELU / RELU); mean_rstd, scale_shift from b200gan_norm_finalize.  sums:
+ * fp64 [2][C], zero on entry.  B200GAN_E_UNSUPPORTED unless b200gan_conv2d_dgrad_norm_supported(g): Conv2d, stride 1,
+ * zero padding, up 1 or 2, a tensor-core data gradient whose contraction is not split over CTAs. */
+int b200gan_conv2d_dgrad_norm_supported(const b200gan_conv_geom *g);
+int b200gan_conv2d_dgrad_norm(const b200gan_conv_geom *g, const b200gan_norm_desc *d, const float *dy,
+                              const float *packed, const float *x, const float *mean_rstd, const float *scale_shift,
+                              double *sums, float *dx, void *stream);
+/* The rest of b200gan_norm_bwd once `sums` holds what its reduction would have produced (b200gan_conv2d_dgrad_norm):
+ * dx and dgamma_dbeta; act NONE, or LRELU / RELU with scale_shift.  sums is handed back zeroed. */
+int b200gan_norm_bwd_from_sums(const b200gan_norm_desc *d, const float *dy, const float *x, const float *mean_rstd,
+                               const float *scale_shift, const float *gamma, double *sums, float *dx,
+                               float *dgamma_dbeta, void *stream);
 
 /* ---- Generator tail: BatchNorm2d -> LeakyReLU/ReLU -> Conv2d(C, K<=3, 3, 1, 1) -> Tanh, fused -------------- */
 /* Replaces the module run dcgan.py:60-63

@@ -88,12 +88,16 @@ SIGNATURES = {
     "b200gan_conv2d_dgrad": (c_i32, [_P(ConvGeom), c_vp, c_vp, c_vp, c_vp, c_i32, c_vp]),
     "b200gan_conv2d_wgrad_workspace_floats": (c_sz, [_P(ConvGeom), c_i32]),
     "b200gan_conv2d_wgrad": (c_i32, [_P(ConvGeom), c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_vp]),
+    "b200gan_conv2d_wgrad_fused_bias": (c_i32, [_P(ConvGeom), c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_vp]),
     "b200gan_epilogue_bwd": (c_i32, [c_vp, c_vp, c_vp, c_i32, c_f32, c_i64, c_i32, c_i64, c_i32, c_vp, c_vp]),
     "b200gan_bias_grad": (c_i32, [c_vp, c_vp, c_vp, c_i32, c_f32, c_i64, c_i32, c_i64, c_vp, c_vp]),
     "b200gan_norm_stats": (c_i32, [_P(NormDesc), c_vp, c_vp, c_vp]),
     "b200gan_norm_finalize": (c_i32, [_P(NormDesc), c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "b200gan_norm_apply": (c_i32, [_P(NormDesc), c_vp, c_vp, c_vp, c_vp]),
     "b200gan_norm_bwd": (c_i32, [_P(NormDesc), c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "b200gan_conv2d_dgrad_norm_supported": (c_i32, [_P(ConvGeom)]),
+    "b200gan_conv2d_dgrad_norm": (c_i32, [_P(ConvGeom), _P(NormDesc)] + [c_vp] * 8),
+    "b200gan_norm_bwd_from_sums": (c_i32, [_P(NormDesc)] + [c_vp] * 9),
     "b200gan_tail_supported": (c_i32, [_P(TailDesc)]),
     "b200gan_tail_fprop": (c_i32, [_P(TailDesc), c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "b200gan_tail_bwd_workspace_bytes": (c_sz, [_P(TailDesc)]),

@@ -276,6 +276,80 @@ class NormFn(torch.autograd.Function):
         return dx, dgamma, dbeta, None, None, None, None, None
 
 
+class NormConvFn(torch.autograd.Function):
+    """Training-mode BatchNorm2d [-> LeakyReLU/ReLU] [-> Upsample x2] -> Conv2d (dcgan.py:53-55, 56-59): the forward
+    is NormFn's and ConvFn's, the backward reads no tensor twice for the norm -- its sums come out of the conv's
+    data-gradient epilogue (ops.conv_dgrad_norm) -- and takes the bias gradient from the weight-gradient kernel.
+    Only for geometries with ops.conv_dgrad_norm_supported (nn.Sequential checks)."""
+
+    @staticmethod
+    def forward(ctx, x, gamma, beta, stats, running_mean, running_var, nbt, weight, bias, chan_scale, nspec: NormSpec,
+                cspec: ConvSpec, cache: PackCache):
+        ops._require_cuda(x, "norm input")
+        ops._require_cuda(weight, "conv weight")
+        x = _as_cl(x)
+        a, mean_rstd, scale_shift = ops.norm_forward(
+            x, None if gamma is None else gamma.detach(), None if beta is None else beta.detach(), running_mean,
+            running_var, nbt, False, nspec.eps, nspec.momentum, nspec.act, nspec.slope, stats, nspec.rtf_out,
+            return_scale_shift=True)
+        g, _ = ops.make_geom(tuple(a.shape), tuple(weight.shape), cspec.stride, cspec.pads, cspec.pad_mode, cspec.up)
+        algo, kind = ops.conv_plan(g, 0, chan_scale)
+        packed = cache.get(g, weight.detach(), kind)
+        out_stats = None
+        if cspec.stats is not None:
+            out_stats = ops.zero_scratch(x.device, 2 * (g.N * g.K if cspec.stats else g.K))
+        y = ops.conv_fprop(g, a, packed, algo, bias=None if bias is None else bias.detach(), act=cspec.act,
+                           slope=cspec.slope, chan_scale=chan_scale, stats=out_stats,
+                           stats_per_sample=bool(cspec.stats), round_tf32=cspec.rtf_out)
+        ctx.nspec, ctx.cspec, ctx.cache, ctx.g = nspec, cspec, cache, g
+        ctx.has_bias = bias is not None
+        # the norm output `a` is the conv's weight-gradient operand; the conv's output is kept only for its activation
+        ctx.save_for_backward(x, mean_rstd, scale_shift, gamma, a, weight, y if cspec.act != ACT_NONE else None,
+                              chan_scale)
+        if out_stats is not None:
+            ctx.mark_non_differentiable(out_stats)
+            ctx.set_materialize_grads(False)
+            return y, out_stats
+        return y
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, dy, *unused):
+        x, mean_rstd, scale_shift, gamma, a, weight, y, chan_scale = ctx.saved_tensors
+        nspec, cspec, g = ctx.nspec, ctx.cspec, ctx.g
+        dy = _as_cl(dy)
+        if cspec.act != ACT_NONE or chan_scale is not None:
+            dz = ops.epilogue_bwd(dy, y, chan_scale, cspec.act, cspec.slope, cspec.rtf_dz)
+        else:
+            dz = dy
+        nig = ctx.needs_input_grad
+        dx = dgamma = dbeta = dw = db = None
+        need_params = gamma is not None and (nig[1] or nig[2])
+        if nig[0] or need_params:
+            algo, kind = ops.conv_plan(g, 1)
+            da, sums = ops.conv_dgrad_norm(g, dz, ctx.cache.get(g, weight.detach(), kind), x, mean_rstd, scale_shift,
+                                           nspec.act, nspec.slope)
+            dx, dgb = ops.norm_backward_from_sums(da, x, mean_rstd, None if gamma is None else gamma.detach(), sums,
+                                                  nspec.eps, nspec.act, nspec.slope, need_params, nspec.rtf_dx,
+                                                  scale_shift)
+            if need_params:
+                c = x.shape[1]
+                dgamma, dbeta = dgb[:c], dgb[c:]
+            if not nig[0]:
+                dx = None
+        want_db = ctx.has_bias and nig[8]
+        if want_db and dz is not dy and cspec.rtf_dz:
+            # as in ConvFn: the bias gradient of a rounded dz comes from the unrounded values
+            db = ops.bias_grad(dy, y, chan_scale, cspec.act, cspec.slope)
+            want_db = False
+        if nig[7] or want_db:
+            dw, db2 = ops.conv_wgrad(g, a, dz, tuple(weight.shape), want_db, ops.conv_plan(g, 2)[0])
+            db = db2 if want_db else db
+            if not nig[7]:
+                dw = None
+        return dx, dgamma, dbeta, None, None, None, None, dw, db, None, None, None, None
+
+
 @dataclass(frozen=True)
 class TailSpec:
     eps: float = 1e-5

@@ -113,6 +113,14 @@ def _dropout2d_scale(x_shape, p, device):
     return noise.bernoulli_(1.0 - p).div_(1.0 - p).view(n, c)
 
 
+def _conv_cache(conv):
+    cache = conv.__dict__.get("_b200_cache")
+    if cache is None:
+        cache = PackCache()
+        conv.__dict__["_b200_cache"] = cache
+    return cache
+
+
 def _run_conv(conv, x, up=1, extra_pads=(0, 0, 0, 0), pad_mode=PAD_ZERO, act=ACT_NONE, slope=0.0, chan_scale=None,
               stats=None, rtf_out=False, rtf_dz=False):
     if not _conv_ok(conv):
@@ -129,11 +137,20 @@ def _run_conv(conv, x, up=1, extra_pads=(0, 0, 0, 0), pad_mode=PAD_ZERO, act=ACT
     pads = tuple(e + pad for e in extra_pads)
     spec = ConvSpec(stride=int(conv.stride[0]), pads=pads, pad_mode=pad_mode, up=up, transposed=transposed, act=act,
                     slope=slope, stats=stats, rtf_out=rtf_out, rtf_dz=rtf_dz)
-    cache = conv.__dict__.get("_b200_cache")
-    if cache is None:
-        cache = PackCache()
-        conv.__dict__["_b200_cache"] = cache
-    return F.conv_block(x, conv.weight, conv.bias, chan_scale, spec, cache)
+    return F.conv_block(x, conv.weight, conv.bias, chan_scale, spec, _conv_cache(conv))
+
+
+def _batch_norm_spec(norm, per_sample, act, slope, rtf_out, rtf_dx):
+    """(NormSpec, running_mean, running_var, num_batches_tracked) of a norm that normalises with batch statistics."""
+    rm = rv = nbt = None
+    momentum = 0.0
+    if not per_sample and norm.training and norm.track_running_stats:
+        if norm.momentum is None:
+            raise NotImplementedError("b200gan: BatchNorm2d(momentum=None)")
+        rm, rv, nbt, momentum = norm.running_mean, norm.running_var, norm.num_batches_tracked, float(norm.momentum)
+    spec = NormSpec(per_sample=per_sample, eps=float(norm.eps), momentum=momentum, act=act, slope=slope,
+                    rtf_out=rtf_out, rtf_dx=rtf_dx)
+    return spec, rm, rv, nbt
 
 
 def _run_norm(norm, x, act=ACT_NONE, slope=0.0, stats=None, rtf_out=False, rtf_dx=False):
@@ -148,14 +165,7 @@ def _run_norm(norm, x, act=ACT_NONE, slope=0.0, stats=None, rtf_out=False, rtf_d
     if use_batch_stats and not per_sample:
         _no_groups("a stand-alone BatchNorm2d")
     if use_batch_stats:
-        rm = rv = nbt = None
-        momentum = 0.0
-        if not per_sample and norm.training and norm.track_running_stats:
-            if norm.momentum is None:
-                raise NotImplementedError("b200gan: BatchNorm2d(momentum=None)")
-            rm, rv, nbt, momentum = norm.running_mean, norm.running_var, norm.num_batches_tracked, float(norm.momentum)
-        spec = NormSpec(per_sample=per_sample, eps=float(norm.eps), momentum=momentum, act=act, slope=slope,
-                        rtf_out=rtf_out, rtf_dx=rtf_dx)
+        spec, rm, rv, nbt = _batch_norm_spec(norm, per_sample, act, slope, rtf_out, rtf_dx)
         return F.norm_block(x, norm.weight, norm.bias, stats, rm, rv, nbt, spec)
     # eval-mode BatchNorm2d: constant per-channel affine
     rstd = torch.rsqrt(norm.running_var + norm.eps)
@@ -335,6 +345,32 @@ class _TailStep:
 
     def __init__(self, norm_step, conv_step):
         self.norm_step, self.conv_step = norm_step, conv_step
+
+
+def _no_hooks(m):
+    return not (m._forward_hooks or m._forward_pre_hooks or m._backward_hooks)
+
+
+def _norm_conv_fused(ns, cs, x_shape):
+    """True if a norm step and the conv step after it run as functional.NormConvFn at this input shape: BatchNorm2d
+    [-> LeakyReLU/ReLU] with batch statistics (training mode) [-> Upsample x2] -> Conv2d, stride 1, zero padding, no
+    hooks, and a geometry whose data gradient can carry the norm's sums (dcgan.py:53-55, 56-59).  No side effects."""
+    if not (isinstance(ns, _NormStep) and isinstance(cs, _ConvStep)):
+        return False
+    norm, conv = ns.norm, cs.conv
+    if not isinstance(norm, _T["BatchNorm2d"]) or ns.act not in (ACT_NONE, ACT_LRELU, ACT_RELU):
+        return False
+    if isinstance(conv, _T["ConvTranspose2d"]) or cs.pad_mode != PAD_ZERO or tuple(conv.stride) != (1, 1):
+        return False
+    if not (_no_hooks(norm) and _no_hooks(conv) and norm.training and ops.bn_groups.active <= 1):
+        return False
+    if norm.track_running_stats and norm.momentum is None:
+        return False
+    if not (len(x_shape) == 4 and x_shape[1] == norm.num_features == conv.in_channels):
+        return False
+    pads = tuple(e + int(conv.padding[0]) for e in cs.extra_pads)
+    g, _ = ops.make_geom(tuple(x_shape), tuple(conv.weight.shape), 1, pads, PAD_ZERO, cs.up)
+    return ops.conv_dgrad_norm_supported(g)
 
 
 def _chain_plan(chain, shape):
@@ -738,6 +774,21 @@ class Sequential(_T["Sequential"]):
                     stats = None
                 else:
                     queue[0:0] = [ns, cs]
+                continue
+            if queue and _norm_conv_fused(s, queue[0], tuple(x.shape)):
+                # one node whose backward takes the norm's sums from the conv's data-gradient epilogue
+                ns, cs = s, queue.pop(0)
+                scale = None
+                if cs.dropout2d is not None and cs.dropout2d.training and cs.dropout2d.p > 0.0:
+                    scale = _dropout2d_scale((x.shape[0], cs.conv.out_channels), cs.dropout2d.p, x.device)
+                want = cs.stats if (cs.next_norm is not None and _uses_batch_stats(cs.next_norm)) else None
+                norm, conv = ns.norm, cs.conv
+                nspec, rm, rv, nbt = _batch_norm_spec(norm, False, ns.act, ns.slope, ns.rtf_out, ns.rtf_dx)
+                cspec = ConvSpec(stride=1, pads=tuple(e + int(conv.padding[0]) for e in cs.extra_pads), up=cs.up,
+                                 act=cs.act, slope=cs.slope, stats=want, rtf_out=cs.rtf_out, rtf_dz=cs.rtf_dz)
+                out = F.NormConvFn.apply(x, norm.weight, norm.bias, stats if ns.takes_stats else None, rm, rv, nbt,
+                                         conv.weight, conv.bias, scale, nspec, cspec, _conv_cache(conv))
+                x, stats = out if want is not None else (out, None)
                 continue
             if isinstance(s, _ConvStep):
                 cs = None

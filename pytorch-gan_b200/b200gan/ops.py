@@ -181,8 +181,8 @@ def conv_wgrad(g, x, dy, weight_shape, need_bias, algo):
     db = torch.empty(g.K, device=x.device, dtype=torch.float32) if need_bias else None
     nws = lib.b200gan_conv2d_wgrad_workspace_floats(ctypes.byref(g), algo)
     ws = torch.empty(nws, device=x.device, dtype=torch.float32) if nws else None
-    _lib.check(lib.b200gan_conv2d_wgrad(ctypes.byref(g), x.data_ptr(), dy.data_ptr(), dw.data_ptr(), _ptr(db),
-                                        _ptr(ws), algo, _stream()), "conv2d_wgrad")
+    _lib.check(lib.b200gan_conv2d_wgrad_fused_bias(ctypes.byref(g), x.data_ptr(), dy.data_ptr(), dw.data_ptr(),
+                                                   _ptr(db), _ptr(ws), algo, _stream()), "conv2d_wgrad")
     return dw, db
 
 
@@ -329,6 +329,37 @@ def norm_backward(dy, x, y, mean_rstd, gamma, per_sample, eps, act=ACT_NONE, slo
     _lib.check(lib.b200gan_norm_bwd(ctypes.byref(d), dy.data_ptr(), x.data_ptr(), _ptr(y), mean_rstd.data_ptr(),
                                     _ptr(scale_shift), _ptr(gamma), sums.data_ptr(), dx.data_ptr(), _ptr(dgb), _stream()),
                "norm_bwd")
+    return dx, dgb
+
+
+# ---- BatchNorm2d [act] [Upsample x2] Conv2d backward: the norm's sums from the conv's data-gradient epilogue ----------
+def conv_dgrad_norm_supported(g):
+    if Config.algo == "simt":
+        return False
+    return bool(_lib.load().b200gan_conv2d_dgrad_norm_supported(ctypes.byref(g)))
+
+
+def conv_dgrad_norm(g, dy, packed, x, mean_rstd, scale_shift, act, slope):
+    """(dx, sums): the conv's data gradient (tensor cores) and, from the same epilogue, the fp64 [2][C] sums the
+    BatchNorm backward of its input x needs.  `sums` is a zero_scratch buffer for norm_backward_from_sums to consume."""
+    d = _norm_desc(x.shape, False, 0.0, 0.0, act, slope, False)
+    sums = zero_scratch(x.device, 2 * g.C)
+    dx = empty_cl(g.N, g.C, g.H, g.W, dy.device)
+    _lib.check(_lib.load().b200gan_conv2d_dgrad_norm(ctypes.byref(g), ctypes.byref(d), dy.data_ptr(), packed.data_ptr(),
+                                                     x.data_ptr(), mean_rstd.data_ptr(), scale_shift.data_ptr(),
+                                                     sums.data_ptr(), dx.data_ptr(), _stream()), "conv2d_dgrad_norm")
+    return dx, sums
+
+
+def norm_backward_from_sums(dy, x, mean_rstd, gamma, sums, eps, act=ACT_NONE, slope=0.0, need_params=False,
+                            round_tf32=False, scale_shift=None):
+    """norm_backward (batch statistics) given the sums conv_dgrad_norm produced; hands `sums` back zeroed."""
+    d = _norm_desc(x.shape, False, eps, 0.0, act, slope, round_tf32)
+    dx = torch.empty_like(x, memory_format=CL)
+    dgb = torch.empty(sums.numel(), device=x.device, dtype=torch.float32) if need_params else None
+    _lib.check(_lib.load().b200gan_norm_bwd_from_sums(ctypes.byref(d), dy.data_ptr(), x.data_ptr(), mean_rstd.data_ptr(),
+                                                      _ptr(scale_shift), _ptr(gamma), sums.data_ptr(), dx.data_ptr(),
+                                                      _ptr(dgb), _stream()), "norm_bwd_from_sums")
     return dx, dgb
 
 

@@ -40,10 +40,11 @@ size_t fewk_wgrad_workspace_floats(const b200gan_conv_geom *g);
 int tc_supported(const b200gan_conv_geom *g, int pass);
 int tc_fprop(const b200gan_conv_geom *g, const b200gan_epilogue *ep, const float *x,
              const float *packed, float *y, cudaStream_t st);
-int tc_dgrad(const b200gan_conv_geom *g, const float *dy, const float *packed, float *dx,
+struct TcNormBwd;
+int tc_dgrad(const b200gan_conv_geom *g, const float *dy, const float *packed, float *dx, const TcNormBwd *nb,
              cudaStream_t st);
 size_t tc_wgrad_workspace_floats(const b200gan_conv_geom *g);
-int tc_wgrad(const b200gan_conv_geom *g, const float *x, const float *dy, float *dw, float *ws,
+int tc_wgrad(const b200gan_conv_geom *g, const float *x, const float *dy, float *dw, float *db, float *ws,
              cudaStream_t st);
 
 static thread_local char g_err[512] = "";
@@ -411,7 +412,7 @@ extern "C" int b200gan_conv2d_dgrad(const b200gan_conv_geom *g, const float *dy,
   switch (dgrad_route(g, algo)) {
     case DgradRoute::Tc:
       if (!tc_supported(g, 1)) B2_UNSUPPORTED("conv2d_dgrad: geometry not supported by the tensor-core path");
-      return tc_dgrad(g, dy, packed, dx, st);
+      return tc_dgrad(g, dy, packed, dx, nullptr, st);
     case DgradRoute::Transposed:
       // dx[n,ih,iw,c] = sum_{r,s,k} dy[n, ih*stride - pad + r, iw*stride - pad + s, k] * w[c,k,r,s]
       return simt_gather_gemm(g->N, g->P, g->Q, g->K, g->H, g->W, g->C, g->R, g->S, g->stride, g->pad_t, g->pad_l,
@@ -473,8 +474,9 @@ extern "C" size_t b200gan_conv2d_wgrad_workspace_floats(const b200gan_conv_geom 
   return 0;
 }
 
-extern "C" int b200gan_conv2d_wgrad(const b200gan_conv_geom *g, const float *x, const float *dy, float *dw,
-                                    float *db, float *workspace, int algo, void *stream) {
+// fuse_db: a Conv2d bias gradient on the tensor-core route comes out of the weight-gradient kernel itself
+static int conv2d_wgrad(const b200gan_conv_geom *g, const float *x, const float *dy, float *dw, float *db,
+                        float *workspace, int algo, bool fuse_db, void *stream) {
   if (int e = validate_geom(g)) return e;
   B2_CHECK_ARG(x && dy && dw, "conv2d_wgrad: null pointer");
   cudaStream_t st = as_stream(stream);
@@ -482,7 +484,8 @@ extern "C" int b200gan_conv2d_wgrad(const b200gan_conv_geom *g, const float *x, 
   switch (wgrad_route(g, algo)) {
     case WgradRoute::Tc:
       if (!tc_supported(g, 2)) B2_UNSUPPORTED("conv2d_wgrad: geometry not supported by the tensor-core path");
-      rc = tc_wgrad(g, x, dy, dw, workspace, st);
+      if (fuse_db && !g->transposed) return tc_wgrad(g, x, dy, dw, db, workspace, st);  // db from the same pass
+      rc = tc_wgrad(g, x, dy, dw, nullptr, workspace, st);
       break;
     case WgradRoute::Fewk:
       rc = fewk_wgrad(g, x, dy, dw, workspace, st);
@@ -502,4 +505,14 @@ extern "C" int b200gan_conv2d_wgrad(const b200gan_conv_geom *g, const float *x, 
   if (rc) return rc;
   if (db) return simt_colsum(dy, db, (int64_t)g->N * g->P * g->Q, g->K, st);
   return B200GAN_OK;
+}
+
+extern "C" int b200gan_conv2d_wgrad(const b200gan_conv_geom *g, const float *x, const float *dy, float *dw,
+                                    float *db, float *workspace, int algo, void *stream) {
+  return conv2d_wgrad(g, x, dy, dw, db, workspace, algo, false, stream);
+}
+
+extern "C" int b200gan_conv2d_wgrad_fused_bias(const b200gan_conv_geom *g, const float *x, const float *dy, float *dw,
+                                               float *db, float *workspace, int algo, void *stream) {
+  return conv2d_wgrad(g, x, dy, dw, db, workspace, algo, true, stream);
 }

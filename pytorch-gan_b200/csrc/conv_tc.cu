@@ -109,7 +109,23 @@ struct TcParams {
                      // TMA out-of-bounds fill (cyclegan/models.py:82, Conv2d(64, 3, 7)): direct stores, no TMA store
   int32_t ksplit;    // > 1: the (tap, k-chunk) loop is split over `ksplit` CTAs; raw partial tiles are added into a zeroed
                      // output with TMA reduce-stores (layers with few output pixels: pix2pix/models.py:62-73 at 1x1..8x8)
+  // Norm-backward sums (data gradient of a conv fed by a batch-statistics BatchNorm2d [+ LeakyReLU / ReLU]): nb_x is
+  // the norm input on the output grid, or nullptr.  Then `stats` receives sum dy' and sum dy' * xhat per channel
+  // instead of sum y and sum y^2, with dy' = y * act'(x * scale + shift) and xhat = (x - mean) * rstd.
+  const float *nb_x;
+  const float *nb_mean_rstd;   // [2][ldk]
+  const float *nb_scale_shift; // [2][ldk]
+  int32_t nb_act;
+  float nb_slope;
   long long *trace;  // bring-up: per-CTA clock64 timeline (64 slots per CTA) or nullptr
+};
+
+// host-side description of the norm-backward epilogue of a data gradient (see TcParams::nb_x)
+struct TcNormBwd {
+  const float *x, *mean_rstd, *scale_shift;
+  int32_t act;
+  float slope;
+  double *sums;  // [2][C]
 };
 
 #define TC_TRACE(slot)                                                   \
@@ -197,6 +213,44 @@ __device__ __forceinline__ void epilogue_chunk(float (&v)[32], const float *bias
   if (rtf) {
 #pragma unroll
     for (int j = 0; j < 32; ++j) v[j] = round_tf32(v[j]);
+  }
+}
+
+// The two norm-backward summands of 32 channels of one pixel, from the data gradient v of the norm's output:
+// v <- dy' = v * act'(x * scale + shift), s2 <- dy' * (x - mean) * rstd, both zero for a pixel outside the output
+// (xrow == nullptr).  The mask is taken from x as norm_bwd_reduce_kernel takes it; 8 channels at a time, so that x and
+// the per-channel parameters of the whole chunk are never live at once.
+__device__ __forceinline__ void norm_bwd_terms(float (&v)[32], float (&s2)[32], const float *xrow, const float *mean_rstd,
+                                               const float *scale_shift, int ldk, int act, float slope) {
+  const bool masked = act != B200GAN_ACT_NONE;
+  const float lo = act == B200GAN_ACT_LRELU ? slope : 0.f;
+#pragma unroll
+  for (int g = 0; g < 4; ++g) {
+    float xx[8], mean[8], rstd[8], sc[8], sh[8];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int o = 2 * g + h;
+      const float4 a = xrow ? __ldg(reinterpret_cast<const float4 *>(xrow) + o) : make_float4(0.f, 0.f, 0.f, 0.f);
+      const float4 m = __ldg(reinterpret_cast<const float4 *>(mean_rstd) + o);
+      const float4 r = __ldg(reinterpret_cast<const float4 *>(mean_rstd + ldk) + o);
+      const float4 s = __ldg(reinterpret_cast<const float4 *>(scale_shift) + o);
+      const float4 t = __ldg(reinterpret_cast<const float4 *>(scale_shift + ldk) + o);
+      xx[4 * h] = a.x; xx[4 * h + 1] = a.y; xx[4 * h + 2] = a.z; xx[4 * h + 3] = a.w;
+      mean[4 * h] = m.x; mean[4 * h + 1] = m.y; mean[4 * h + 2] = m.z; mean[4 * h + 3] = m.w;
+      rstd[4 * h] = r.x; rstd[4 * h + 1] = r.y; rstd[4 * h + 2] = r.z; rstd[4 * h + 3] = r.w;
+      sc[4 * h] = s.x; sc[4 * h + 1] = s.y; sc[4 * h + 2] = s.z; sc[4 * h + 3] = s.w;
+      sh[4 * h] = t.x; sh[4 * h + 1] = t.y; sh[4 * h + 2] = t.z; sh[4 * h + 3] = t.w;
+    }
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const int j = 8 * g + e;
+      float dz = v[j];
+      if (masked && !(fmaf(xx[e], sc[e], sh[e]) > 0.f)) dz *= lo;
+      dz = xrow ? dz : 0.f;
+      v[j] = dz;
+      s2[j] = dz * ((xx[e] - mean[e]) * rstd[e]);
+    }
+    asm volatile("" ::: "memory");  // keeps the next group's loads behind this group's arithmetic
   }
 }
 
@@ -338,10 +392,17 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
       if (p.stats) {
         float s2[32];
+        // not in the 256-wide instance, where it would spill (the host never asks for it there)
+        if (BN < 256 && p.nb_x) {
+          const int ch = ntile * BN + c;
+          norm_bwd_terms(v, s2, valid ? p.nb_x + ((int64_t)(on * p.Ho + oh) * p.Wo + ow) * p.ldk + ch : nullptr,
+                         p.nb_mean_rstd + ch, p.nb_scale_shift + ch, p.ldk, p.nb_act, p.nb_slope);
+        } else {
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          v[j] = valid ? v[j] : 0.f;
-          s2[j] = v[j] * v[j];
+          for (int j = 0; j < 32; ++j) {
+            v[j] = valid ? v[j] : 0.f;
+            s2[j] = v[j] * v[j];
+          }
         }
         float cs1 = warp_colsum32(v, lane);
         float cs2 = warp_colsum32(s2, lane);
@@ -661,13 +722,43 @@ static int ilog2_ceil(int v) {
 // Set-up shared by run_tc and run_up2_allphase: the 128-pixel tile of an N x Ho x Wo grid per phase (BW x BH pixels
 // of BNn images; returns BNn), the epilogue and the trace.  Per-sample sums fuse only when a tile is one image;
 // otherwise *deferred takes the statistics buffer and the caller runs conv_stats_pass after the conv.
+// box of the 128-pixel tile: BW = 2^bwl x BH = 2^bhl pixels of BNn images
+static int tc_tile_shape(int Ho, int Wo, int &bwl, int &bhl) {
+  bwl = ilog2_ceil(Wo);
+  if (bwl > 7) bwl = 7;
+  bhl = ilog2_ceil(Ho);
+  if (bhl > 7 - bwl) bhl = 7 - bwl;
+  return TC_BM / ((1 << bwl) * (1 << bhl));
+}
+
+// pixel tiles of one phase of an N x Ho x Wo output grid
+static int64_t tc_tiles(int N, int Ho, int Wo) {
+  int bwl, bhl;
+  const int BNn = tc_tile_shape(Ho, Wo, bwl, bhl);
+  return (int64_t)ceil_div(Wo, 1 << bwl) * ceil_div(Ho, 1 << bhl) * ceil_div(N, BNn);
+}
+
+// output channels per CTA.  256-wide tiles (A 16 KB + B 32 KB per stage feed 2 x 4 x M64 N256 K8: the 128-channel A
+// box is fetched half as often per output channel) when the layer still gives every SM a CTA
+static int tc_block_n(int Kout, int64_t tiles) {
+  if (Kout % 256 == 0 && tiles * (Kout / 256) >= num_sms()) return 256;
+  return (Kout % 128 == 0) ? 128 : (Kout % 64 == 0 ? 64 : 32);
+}
+
+// few output tiles (deep U-Net layers at 1x1 .. 16x16 pixels): the number of CTAs the contraction of a plain
+// (epilogue-free) conv is split over so that the machine is used; 1 = no split
+static int tc_ksplit(int64_t ctas, int min_iters) {
+  if (ctas >= num_sms() || min_iters < 16) return 1;
+  int ks = (int)((2 * num_sms() + ctas - 1) / ctas);
+  if (ks > min_iters / 8) ks = min_iters / 8;
+  if (ks > 32) ks = 32;
+  return ks >= 2 ? ks : 1;
+}
+
 template <class Params>
 static int tc_setup(Params &p, int N, int Ho, int Wo, int ldk, const b200gan_epilogue *ep, double **deferred) {
-  int bwl = ilog2_ceil(Wo);
-  if (bwl > 7) bwl = 7;
-  int bhl = ilog2_ceil(Ho);
-  if (bhl > 7 - bwl) bhl = 7 - bwl;
-  const int BNn = TC_BM / ((1 << bwl) * (1 << bhl));
+  int bwl, bhl;
+  const int BNn = tc_tile_shape(Ho, Wo, bwl, bhl);
   p.bw_log2 = bwl;
   p.bh_log2 = bhl;
   p.tiles_w = ceil_div(Wo, 1 << bwl);
@@ -754,14 +845,14 @@ int tc_supported(const b200gan_conv_geom *g, int pass) {
 //  btaps   : number of tap blocks in the packed weight matrix (rows = btaps * Kout)
 //  out     : N x Ho x Wo pixels per phase.  phase_out: 1 -> y is the full-resolution tensor [N][2Ho][2Wo][ldk]
 //            addressed through the phase view {2*ldk, Wo, 2, Ho, N}; phase z writes (out_dc[z], out_da[z]).
+//  nb      : norm-backward sums in the epilogue (plain output, unsplit), or nullptr
 static int run_tc(const float *in, int N, int Hi, int Wi, int Cc, bool phase_in, const float *packedB, int Kout,
                   int btaps, int nphase, const int *tap_begin, const TcTap *taps, int Ho, int Wo, bool phase_out,
-                  const int *out_dc, const int *out_da, int ldk, const b200gan_epilogue *ep, float *y,
-                  cudaStream_t st) {
+                  const int *out_dc, const int *out_da, int ldk, const b200gan_epilogue *ep, const TcNormBwd *nb,
+                  float *y, cudaStream_t st) {
   const int narrow_k = Kout < 32 ? Kout : 0;
   const int Kreal = Kout;
   if (narrow_k) Kout = 32;  // MMA N = 32; rows >= Kreal of every B box are TMA out-of-bounds zeros
-  int BN = (Kout % 128 == 0) ? 128 : (Kout % 64 == 0 ? 64 : 32);
   TcParams p;
   memset(&p, 0, sizeof(p));
   const int total_taps = tap_begin[nphase];
@@ -772,12 +863,8 @@ static int run_tc(const float *in, int N, int Hi, int Wi, int Cc, bool phase_in,
   double *deferred_stats;
   const int BNn = tc_setup(p, N, Ho, Wo, ldk, ep, &deferred_stats);
   const int BW = 1 << p.bw_log2, BH = 1 << p.bh_log2;
-  {
-    // 256-wide tiles (A 16 KB + B 32 KB per stage feed 2 x 4 x M64 N256 K8: the 128-channel A box is fetched half as
-    // often per output channel) when the layer still gives every SM a CTA
-    const int64_t tiles = (int64_t)p.tiles_w * p.tiles_h * ceil_div(N, BNn) * nphase;
-    if (Kout % 256 == 0 && tiles * (Kout / 256) >= num_sms()) BN = 256;
-  }
+  const int64_t tiles = (int64_t)p.tiles_w * p.tiles_h * ceil_div(N, BNn) * nphase;
+  const int BN = tc_block_n(Kout, tiles);
   for (int i = 0; i < 4; ++i) {
     p.out_dc[i] = i < nphase ? out_dc[i] : 0;
     p.out_da[i] = i < nphase ? out_da[i] : 0;
@@ -794,26 +881,33 @@ static int run_tc(const float *in, int N, int Hi, int Wi, int Cc, bool phase_in,
     p.stats = nullptr;
   }
   {
-    // few output tiles (deep U-Net layers at 1x1 .. 16x16 pixels): split the contraction so that the machine is used
     const bool plain = !p.bias && !p.chan_scale && p.act == B200GAN_ACT_NONE && !p.rtf;
-    const int64_t ctas = (int64_t)p.tiles_w * p.tiles_h * ceil_div(N, BNn) * (Kout / BN) * nphase;
     int min_iters = 1 << 30;
     for (int z = 0; z < nphase; ++z) {
       const int it = (tap_begin[z + 1] - tap_begin[z]) * p.kchunks;
       if (it < min_iters) min_iters = it;
     }
-    if (plain && !narrow_k && ctas < num_sms() && min_iters >= 16) {
-      int ks = (int)((2 * num_sms() + ctas - 1) / ctas);
-      if (ks > min_iters / 8) ks = min_iters / 8;
-      if (ks > 32) ks = 32;
-      if (ks >= 2) {
-        p.ksplit = ks;
-        if (p.stats) {  // partial tiles cannot carry the norm statistics: one extra pass over the (small) output
-          deferred_stats = p.stats;
-          p.stats = nullptr;
-        }
+    const int ks = plain && !narrow_k ? tc_ksplit(tiles * (Kout / BN), min_iters) : 1;
+    if (ks >= 2) {
+      if (nb) B2_UNSUPPORTED("tensor-core dgrad with norm sums: the contraction of this geometry is split");
+      p.ksplit = ks;
+      if (p.stats) {  // partial tiles cannot carry the norm statistics: one extra pass over the (small) output
+        deferred_stats = p.stats;
+        p.stats = nullptr;
       }
     }
+  }
+  if (nb) {
+    B2_CHECK_ARG(!narrow_k && !phase_out && nphase == 1 && !p.stats && !deferred_stats,
+                 "tensor-core dgrad with norm sums: plain output without other statistics only");
+    p.stats = nb->sums;
+    p.stats_per_sample = 0;
+    p.stats_groups = ldk;
+    p.nb_x = nb->x;
+    p.nb_mean_rstd = nb->mean_rstd;
+    p.nb_scale_shift = nb->scale_shift;
+    p.nb_act = nb->act;
+    p.nb_slope = nb->slope;
   }
   B2_CHECK_ARG(((uintptr_t)in % 16 == 0) && ((uintptr_t)packedB % 16 == 0) && ((uintptr_t)y % 16 == 0),
                "tensor-core conv: pointers must be 16-byte aligned");
@@ -950,13 +1044,13 @@ static int tc_gather(const float *in, int N, int Hi, int Wi, int Cc, int R, int 
     }
   tap_begin[1] = nt;
   return run_tc(in, N, Hi, Wi, Cc, stride == 2, packedB, Kout, R * S, 1, tap_begin, taps, Po, Qo, false, out_dc, out_da,
-                Kout, ep, out, st);
+                Kout, ep, nullptr, out, st);
 }
 
 // scatter form.  in: [N][Pi][Qi][Cc]; out: [N][Ho][Wo][Kout] (full resolution); B: [R*S][Kout][Cc]
 static int tc_scatter(const float *in, int N, int Pi, int Qi, int Cc, int R, int S, int stride, int pad_t, int pad_l,
-                      const float *packedB, int Kout, int Ho, int Wo, const b200gan_epilogue *ep, float *out,
-                      cudaStream_t st) {
+                      const float *packedB, int Kout, int Ho, int Wo, const b200gan_epilogue *ep, const TcNormBwd *nb,
+                      float *out, cudaStream_t st) {
   TcTap taps[TC_MAX_TAPS];
   memset(taps, 0, sizeof(taps));
   int tap_begin[5] = {0, 0, 0, 0, 0};
@@ -971,7 +1065,7 @@ static int tc_scatter(const float *in, int N, int Pi, int Qi, int Cc, int R, int
       }
     tap_begin[1] = nt;
     return run_tc(in, N, Pi, Qi, Cc, false, packedB, Kout, R * S, 1, tap_begin, taps, Ho, Wo, false, out_dc, out_da, Kout,
-                  ep, out, st);
+                  ep, nb, out, st);
   }
   int nt = 0;
   for (int ph = 0; ph < 4; ++ph) {
@@ -993,7 +1087,7 @@ static int tc_scatter(const float *in, int N, int Pi, int Qi, int Cc, int R, int
   }
   tap_begin[4] = nt;
   return run_tc(in, N, Pi, Qi, Cc, false, packedB, Kout, R * S, 4, tap_begin, taps, Ho / 2, Wo / 2, true, out_dc, out_da,
-                Kout, ep, out, st);
+                Kout, ep, nb, out, st);
 }
 
 int tc_fprop(const b200gan_conv_geom *g, const b200gan_epilogue *ep, const float *x, const float *packed, float *y,
@@ -1021,15 +1115,29 @@ int tc_fprop(const b200gan_conv_geom *g, const b200gan_epilogue *ep, const float
       out_da[ph] = a;
     }
     return run_tc(x, g->N, g->H, g->W, g->C, false, packed, g->K, 16, 4, tap_begin, taps, g->H, g->W, true, out_dc, out_da,
-                  g->K, e, y, st);
+                  g->K, e, nullptr, y, st);
   }
   if (g->transposed)  // ConvTranspose2d forward: scatter x into the (stride x larger) output
-    return tc_scatter(x, g->N, g->H, g->W, g->C, g->R, g->S, g->stride, g->pad_t, g->pad_l, packed, g->K, g->P, g->Q, e, y,
-                      st);
+    return tc_scatter(x, g->N, g->H, g->W, g->C, g->R, g->S, g->stride, g->pad_t, g->pad_l, packed, g->K, g->P, g->Q, e,
+                      nullptr, y, st);
   return tc_gather(x, g->N, g->H, g->W, g->C, g->R, g->S, g->stride, g->pad_t, g->pad_l, packed, g->K, g->P, g->Q, e, y, st);
 }
 
-int tc_dgrad(const b200gan_conv_geom *g, const float *dy, const float *packed, float *dx, cudaStream_t st) {
+// The data gradients that can carry the norm-backward sums (TcNormBwd): Conv2d, stride 1, zero padding, up 1 or 2 --
+// the gradient is written on the input grid without a phase view -- with at most 128 channels per CTA and a
+// contraction that run_tc does not split.
+int tc_dgrad_norm_supported(const b200gan_conv_geom *g) {
+  if (!tc_supported(g, 1) || g->transposed || g->stride != 1 || g->pad_mode != B200GAN_PAD_ZERO) return 0;
+  const int64_t tiles = tc_tiles(g->N, g->H, g->W);
+  const int taps = g->up == 2 ? 16 : g->R * g->S;
+  const int bn = tc_block_n(g->C, tiles);
+  return bn <= 128 && tc_ksplit(tiles * (g->C / bn), taps * (g->K / TC_BK)) == 1;
+}
+
+// nb: norm-backward sums in the epilogue (tc_dgrad_norm_supported geometries), or nullptr
+int tc_dgrad(const b200gan_conv_geom *g, const float *dy, const float *packed, float *dx, const TcNormBwd *nb,
+             cudaStream_t st) {
+  if (nb && !tc_dgrad_norm_supported(g)) B2_UNSUPPORTED("tensor-core dgrad with norm sums: geometry not supported");
   if (g->up == 2) {
     // dx[i][j] = sum_{a,b,dr,ds} dy[2(i-(a-1+dr))+a][2(j-(b-1+ds))+b] * Wf[a][b][dr][ds]^T
     TcTap taps[TC_MAX_TAPS];
@@ -1046,13 +1154,37 @@ int tc_dgrad(const b200gan_conv_geom *g, const float *dy, const float *packed, f
       }
     }
     return run_tc(dy, g->N, g->P, g->Q, g->K, true, packed, g->C, 16, 1, tap_begin, taps, g->H, g->W, false, out_dc, out_da,
-                  g->C, nullptr, dx, st);
+                  g->C, nullptr, nb, dx, st);
   }
   if (g->transposed)  // dx[ih] = sum dy[stride*ih - pad + r] w: gather over dy
     return tc_gather(dy, g->N, g->P, g->Q, g->K, g->R, g->S, g->stride, g->pad_t, g->pad_l, packed, g->C, g->H, g->W, nullptr,
                      dx, st);
   return tc_scatter(dy, g->N, g->P, g->Q, g->K, g->R, g->S, g->stride, g->pad_t, g->pad_l, packed, g->C, g->H, g->W, nullptr,
-                    dx, st);
+                    nb, dx, st);
 }
 
 }  // namespace b200gan
+
+// The C ABI of the data gradient with norm sums lives here, next to TcNormBwd (b200gan_norm_bwd_from_sums: norm.cu).
+using namespace b200gan;
+
+extern "C" int b200gan_conv2d_dgrad_norm_supported(const b200gan_conv_geom *g) {
+  if (validate_geom(g) != B200GAN_OK) return 0;
+  return tc_dgrad_norm_supported(g);
+}
+
+extern "C" int b200gan_conv2d_dgrad_norm(const b200gan_conv_geom *g, const b200gan_norm_desc *d, const float *dy,
+                                         const float *packed, const float *x, const float *mean_rstd,
+                                         const float *scale_shift, double *sums, float *dx, void *stream) {
+  if (int e = validate_geom(g)) return e;
+  B2_CHECK_ARG(d && dy && packed && x && mean_rstd && sums && dx, "conv2d_dgrad_norm: null pointer");
+  if (d->per_sample) B2_UNSUPPORTED("conv2d_dgrad_norm: batch statistics only (per-sample norms are not supported)");
+  B2_CHECK_ARG(d->C == g->C && d->N == g->N && d->HW == g->H * g->W, "conv2d_dgrad_norm: norm and conv input differ");
+  B2_CHECK_ARG(d->act == B200GAN_ACT_NONE || d->act == B200GAN_ACT_LRELU || d->act == B200GAN_ACT_RELU,
+               "conv2d_dgrad_norm: the norm's activation must be none, LeakyReLU or ReLU");
+  B2_CHECK_ARG(scale_shift != nullptr, "conv2d_dgrad_norm: scale_shift required");
+  B2_CHECK_ARG(((uintptr_t)x | (uintptr_t)mean_rstd | (uintptr_t)scale_shift) % 16 == 0,
+               "conv2d_dgrad_norm: pointers must be 16-byte aligned");
+  const TcNormBwd nb{x, mean_rstd, scale_shift, d->act, d->slope, sums};
+  return tc_dgrad(g, dy, packed, dx, &nb, as_stream(stream));
+}

@@ -318,6 +318,21 @@ static int check_desc(const b200gan_norm_desc *d) {
   return B200GAN_OK;
 }
 
+// passes 2 and 3 of the backward, once `sums` holds sum dy' and sum dy' * xhat (hands the workspace back zeroed)
+static int norm_bwd_apply_params(const b200gan_norm_desc *d, const float *dy, const float *x, const float *y,
+                                 const float *mean_rstd, const float *scale_shift, const float *gamma, double *sums,
+                                 float *dx, float *dgamma_dbeta, int vec, dim3 grid, int64_t rows, cudaStream_t st) {
+  const int G = d->per_sample ? d->N * d->C : d->C;
+  const float inv = (float)(1.0 / (d->per_sample ? (double)d->HW : (double)d->N * (double)d->HW));
+  auto apply = vec == 4 ? norm_bwd_apply_kernel<4> : norm_bwd_apply_kernel<1>;
+  apply<<<grid, 256, 0, st>>>(dy, x, y, mean_rstd, scale_shift, gamma, sums, dx, rows, d->C, G, inv, d->act, d->slope,
+                              d->round_tf32);
+  B2_LAUNCH_CHECK();
+  norm_bwd_params_kernel<<<ceil_div(G, 128), 128, 0, st>>>(sums, dgamma_dbeta, G);
+  B2_LAUNCH_CHECK();
+  return B200GAN_OK;
+}
+
 }  // namespace b200gan
 
 using namespace b200gan;
@@ -385,12 +400,19 @@ extern "C" int b200gan_norm_bwd(const b200gan_norm_desc *d, const float *dy, con
   auto reduce = vec == 4 ? norm_bwd_reduce_kernel<4> : norm_bwd_reduce_kernel<1>;
   reduce<<<grid, 256, 0, st>>>(dy, x, yy, mean_rstd, scale_shift, sums, rows, d->C, G, d->act, d->slope);
   B2_LAUNCH_CHECK();
-  const float inv = (float)(1.0 / (d->per_sample ? (double)d->HW : (double)d->N * (double)d->HW));
-  auto apply = vec == 4 ? norm_bwd_apply_kernel<4> : norm_bwd_apply_kernel<1>;
-  apply<<<grid, 256, 0, st>>>(dy, x, yy, mean_rstd, scale_shift, gamma, sums, dx, rows, d->C, G, inv, d->act, d->slope,
-                              d->round_tf32);
-  B2_LAUNCH_CHECK();
-  norm_bwd_params_kernel<<<ceil_div(G, 128), 128, 0, st>>>(sums, dgamma_dbeta, G);
-  B2_LAUNCH_CHECK();
-  return B200GAN_OK;
+  return norm_bwd_apply_params(d, dy, x, yy, mean_rstd, scale_shift, gamma, sums, dx, dgamma_dbeta, vec, grid, rows, st);
+}
+
+extern "C" int b200gan_norm_bwd_from_sums(const b200gan_norm_desc *d, const float *dy, const float *x,
+                                          const float *mean_rstd, const float *scale_shift, const float *gamma,
+                                          double *sums, float *dx, float *dgamma_dbeta, void *stream) {
+  if (int e = check_desc(d)) return e;
+  B2_CHECK_ARG(dy && x && mean_rstd && sums && dx, "norm_bwd_from_sums: null pointer");
+  B2_CHECK_ARG(d->act == B200GAN_ACT_NONE || ((d->act == B200GAN_ACT_LRELU || d->act == B200GAN_ACT_RELU) && scale_shift),
+               "norm_bwd_from_sums: activation must be none, or LeakyReLU / ReLU with scale_shift");
+  const int vec = vec_width(d->C, {dy, x, dx});
+  int64_t rows;
+  const dim3 grid = slice_grid(d, vec, rows);
+  return norm_bwd_apply_params(d, dy, x, x, mean_rstd, scale_shift, gamma, sums, dx, dgamma_dbeta, vec, grid, rows,
+                               as_stream(stream));
 }

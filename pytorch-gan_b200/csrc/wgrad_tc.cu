@@ -34,6 +34,8 @@ struct WgJob {
   int16_t s_dc, d_dc;  // channel base in the parity / phase view
   int8_t s_da, d_da;   // row-parity coordinate in the view
   int8_t s_dw, s_dh;   // shift of S in (view) pixels
+  int8_t db;           // 1: this job's D pixels are summed into the bias gradient (each dy pixel is read by one such job)
+  int8_t pad_;
 };
 
 struct WgParams {
@@ -48,6 +50,7 @@ struct WgParams {
   int32_t ldn;                    // N' total (row length of a partial matrix)
   int32_t mtotal;                 // M' total
   float *partial;                 // [job][M'][N'], zeroed by the host; splits accumulate with TMA reduce-add
+  float *db;                      // Conv2d bias gradient: [K] per-channel sums of D = dy (zeroed by the host), or nullptr
 };
 
 // shared memory: TMA ring | two K-major B buffers; after the last MMA the front is the staging tile
@@ -155,6 +158,16 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
         (uint32_t)(abase + 128 + ((((ac >> 2)) ^ (ap + 1)) << 4)),      // a2: channel ac,     pixel ap + 1
         (uint32_t)(abase + 128 + ((((ac >> 2) + 2) ^ (ap + 1)) << 4))}; // a3: channel ac + 8, pixel ap + 1
     float acc[NB / 2];                  // the first MMA overwrites it (scale_d = 0)
+    // bias gradient: the D = dy values this thread passes on are summed where they already sit in registers -- as A
+    // fragments (channels ac, ac + 8 of its warp; by the CTAs of N-tile 0) or as the B transpose's float4 (channels
+    // tq * 4 + i of every chunk; by the CTAs of M-tile 0; B = D only has NB <= 64)
+    const bool db_job = p.db != nullptr && p.jobs[job].db;
+    const bool dbA = db_job && !p.s_is_a && nt == 0;
+    const bool dbB = db_job && p.s_is_a && mt == 0;
+    float dsa0 = 0.f, dsa1 = 0.f;
+    float dsb[NB <= 64 ? NB / 8 : 1];
+#pragma unroll
+    for (int i = 0; i < (NB <= 64 ? NB / 8 : 1); ++i) dsb[i] = 0.f;
     int stage = 0;
     uint32_t phase = 0;
     // stage `it` -> A fragments fa and the K-major B tile of buffer it & 1; the ring slot is released afterwards
@@ -167,11 +180,24 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
       for (int k = 0; k < WG_PIX / 8; ++k)
 #pragma unroll
         for (int j = 0; j < 4; ++j) fa[4 * k + j] = *reinterpret_cast<const uint32_t *>(src + aoff[j] + k * 1024);
+      if (dbA) {
+#pragma unroll
+        for (int k = 0; k < WG_PIX / 8; ++k) {
+          dsa0 += __uint_as_float(fa[4 * k]) + __uint_as_float(fa[4 * k + 2]);
+          dsa1 += __uint_as_float(fa[4 * k + 1]) + __uint_as_float(fa[4 * k + 3]);
+        }
+      }
 #pragma unroll
       for (int c = 0; c < NB / 32; ++c) {
         const float4 v = *reinterpret_cast<const float4 *>(src + L::A_BYTES + c * WG_CHUNK_BYTES + tp * 128 +
                                                            ((tq ^ (tp & 7)) << 4));
         const float e[4] = {v.x, v.y, v.z, v.w};
+        if constexpr (NB <= 64) {
+          if (dbB) {
+#pragma unroll
+            for (int i = 0; i < 4; ++i) dsb[4 * c + i] += e[i];
+          }
+        }
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
           const int r = c * 32 + tq * 4 + i;
@@ -211,6 +237,28 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
     }
     wgmma_wait<0>();
     wgmma_fence_regs<NB / 2>(acc);
+    if (dbA) {  // the four lanes l % 4 of a fragment row hold different pixels of the same two channels
+      dsa0 += __shfl_xor_sync(0xffffffffu, dsa0, 1);
+      dsa1 += __shfl_xor_sync(0xffffffffu, dsa1, 1);
+      dsa0 += __shfl_xor_sync(0xffffffffu, dsa0, 2);
+      dsa1 += __shfl_xor_sync(0xffffffffu, dsa1, 2);
+      if ((lane & 3) == 0) {
+        const int ch = (mt * 4 + 2 * half + (wq >> 1)) * 32 + ac;
+        atomicAdd(p.db + ch, dsa0);
+        atomicAdd(p.db + ch + 8, dsa1);
+      }
+    }
+    if constexpr (NB <= 64) {
+      if (dbB) {  // lane = pixel row tp of the stage
+#pragma unroll
+        for (int i = 0; i < NB / 8; ++i) {
+          float s = dsb[i];
+#pragma unroll
+          for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+          if (lane == 0) atomicAdd(p.db + nt * NB + (i >> 2) * 32 + tq * 4 + (i & 3), s);
+        }
+      }
+    }
     wg_consumers_sync();  // every MMA has retired: ring and operand buffers are free for the staging tile
     // registers -> 128B-swizzled staging tile -> TMA reduce-add of the partial tile into partial[job][m'][n']
     store_acc_sw128<NB>(smem, acc, half * 64);
@@ -419,10 +467,13 @@ static int launch_wg(const CUtensorMap &tmX, const CUtensorMap &tmY, const CUten
   return B200GAN_OK;
 }
 
-int tc_wgrad(const b200gan_conv_geom *g, const float *x, const float *dy, float *dw, float *ws, cudaStream_t st) {
+// db: the Conv2d bias gradient (sum of dy over the pixels) from the same pass, or nullptr (ConvTranspose2d: nullptr)
+int tc_wgrad(const b200gan_conv_geom *g, const float *x, const float *dy, float *dw, float *db, float *ws,
+             cudaStream_t st) {
   WgPlan pl;
   if (!wg_plan(g, pl)) B2_UNSUPPORTED("tensor-core wgrad: geometry not supported");
   B2_CHECK_ARG(ws != nullptr, "tensor-core wgrad: workspace required");
+  B2_CHECK_ARG(!(db && g->transposed), "tensor-core wgrad: bias gradient of a ConvTranspose2d is not fused");
   B2_CHECK_ARG(((uintptr_t)x % 16 == 0) && ((uintptr_t)dy % 16 == 0) && ((uintptr_t)ws % 16 == 0),
                "tensor-core wgrad: pointers must be 16-byte aligned");
   const bool up2 = g->up == 2;
@@ -437,8 +488,10 @@ int tc_wgrad(const b200gan_conv_geom *g, const float *x, const float *dy, float 
         int a = ph >> 1, b = ph & 1, dr = tp >> 1, ds = tp & 1;
         WgJob &j = p.jobs[ph * 4 + tp];
         j.d_dc = (int16_t)(b * g->K); j.d_da = (int8_t)a; j.s_dh = (int8_t)(a - 1 + dr); j.s_dw = (int8_t)(b - 1 + ds);
+        j.db = tp == 0;  // the four phases read disjoint quarters of dy; the taps of one phase the same quarter
       }
   } else {
+    p.jobs[0].db = 1;    // every tap reads all of dy
     for (int r = 0; r < g->R; ++r)
       for (int s2 = 0; s2 < g->S; ++s2) {
         WgJob &j = p.jobs[r * g->S + s2];
@@ -456,6 +509,7 @@ int tc_wgrad(const b200gan_conv_geom *g, const float *x, const float *dy, float 
   p.tiles_total = pl.tiles_total; p.tiles_per_split = pl.tps;
   p.s_is_a = pl.s_is_a; p.mtiles = pl.mtiles; p.ntiles = pl.ntiles; p.ldn = pl.ldn; p.mtotal = pl.mtotal;
   p.partial = ws;
+  p.db = db;
 
   // operand tensors: Conv2d: S = x [N][H][W][C], D = dy [N][P][Q][K]; ConvTranspose2d: S = dy, D = x
   const float *sptr = g->transposed ? dy : x, *dptr = g->transposed ? x : dy;
@@ -493,6 +547,7 @@ int tc_wgrad(const b200gan_conv_geom *g, const float *x, const float *dy, float 
     if (int e = make_tmap_f32(&tmP, ws, 2, dims, strides, pbox)) return e;
   }
   B2_CUDA(cudaMemsetAsync(ws, 0, (size_t)pl.njobs * pl.mtotal * pl.ldn * sizeof(float), st));
+  if (db) B2_CUDA(cudaMemsetAsync(db, 0, (size_t)g->K * sizeof(float), st));  // per-CTA sums are added atomically
   dim3 grid((unsigned)pl.nsplits, (unsigned)pl.njobs, (unsigned)(pl.mtiles * pl.ntiles));
   int rc = pl.NB == 256 ? launch_wg<256, 3>(tmX, tmY, tmP, p, grid, st)
            : pl.NB == 128 ? launch_wg<128, 6>(tmX, tmY, tmP, p, grid, st)
