@@ -203,6 +203,16 @@ int b200gan_norm_bwd(const b200gan_norm_desc *d, const float *dy, const float *x
                      const float *mean_rstd, const float *scale_shift, const float *gamma, double *sums, float *dx,
                      float *dgamma_dbeta, void *stream);
 
+/* Double backward of b200gan_norm_bwd (gradient penalties through a training-mode norm): given u = dL/d(dx) and
+ * ugamma_ubeta[2][C] = dL/d(dgamma), dL/d(dbeta) per channel (NULL = 0), writes gx = dL/dx, gdy = dL/d(dy) and
+ * ggamma_per_group[G] = dL/dgamma per group (summed over samples by the caller for InstanceNorm); any of the three may
+ * be NULL.  The mean and rstd are the batch statistics of x, so gx includes their dependence on x.  act NONE, or LRELU /
+ * RELU with scale_shift (the mask is piecewise constant: no second-order term); TANH / SIGMOID give
+ * B200GAN_E_UNSUPPORTED.  sums: fp64 [5][G] workspace, zero on entry, handed back zeroed.  No host synchronisation. */
+int b200gan_norm_dbwd(const b200gan_norm_desc *d, const float *dy, const float *x, const float *mean_rstd,
+                      const float *scale_shift, const float *gamma, const float *u, const float *ugamma_ubeta,
+                      double *sums, float *gx, float *gdy, float *ggamma_per_group, void *stream);
+
 /* ---- BatchNorm2d [-> LeakyReLU / ReLU] [-> Upsample x2] -> Conv2d backward (dcgan.py:53-55,56-59) ------------------ */
 /* The conv's data gradient dx as b200gan_conv2d_dgrad (ALGO_TC, packed PACK_TC_DGRAD[_UP2]) writes it, bit for bit, and
  * in the same epilogue the sums the norm backward needs: sums[0..C) += sum dy', sums[C..2C) += sum dy' * xhat, with

@@ -95,6 +95,7 @@ SIGNATURES = {
     "b200gan_norm_finalize": (c_i32, [_P(NormDesc), c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "b200gan_norm_apply": (c_i32, [_P(NormDesc), c_vp, c_vp, c_vp, c_vp]),
     "b200gan_norm_bwd": (c_i32, [_P(NormDesc), c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "b200gan_norm_dbwd": (c_i32, [_P(NormDesc)] + [c_vp] * 12),
     "b200gan_conv2d_dgrad_norm_supported": (c_i32, [_P(ConvGeom)]),
     "b200gan_conv2d_dgrad_norm": (c_i32, [_P(ConvGeom), _P(NormDesc)] + [c_vp] * 8),
     "b200gan_norm_bwd_from_sums": (c_i32, [_P(NormDesc)] + [c_vp] * 9),

@@ -165,60 +165,69 @@ class ConvFn(torch.autograd.Function):
 # conv is bilinear in (x, w): the backward of its backward needs no new kernels.  With F = fprop(x, w):
 #   D = dgrad(dz, w)  (= dF/dx applied to dz):   dD/d(dz) applied to u = fprop(u, w),   dD/dw applied to u = wgrad(u, dz)
 #   W = wgrad(x, dz)  (= dF/dw applied to dz):   dW/dx applied to v  = dgrad(dz, v),    dW/d(dz) applied to v = fprop(x, v)
-def _plain_fprop(g, x, w):
-    algo, kind = ops.conv_plan(g, 0)
+# simt=True: the fp32 SIMT kernels whatever the geometry -- the double backward of a fused chain with BatchNorm2d, whose
+# own kernels are fp32 (csrc/narrow_block.cu); a norm-free chain keeps the routing of ConvFn
+def _plain_fprop(g, x, w, simt=False):
+    algo, kind = (ALGO_SIMT, PACK_SIMT_FPROP) if simt else ops.conv_plan(g, 0)
     return ops.conv_fprop(g, x, ops.pack_weights(g, w, kind), algo)
 
 
-def _plain_dgrad(g, dz, w):
-    algo, kind = ops.conv_plan(g, 1)
+def _plain_dgrad(g, dz, w, simt=False):
+    algo, kind = (ALGO_SIMT, PACK_SIMT_DGRAD) if simt else ops.conv_plan(g, 1)
     return ops.conv_dgrad(g, dz, ops.pack_weights(g, w, kind), algo)
 
 
-def _plain_wgrad(g, x, dz, wshape):
-    return ops.conv_wgrad(g, x, dz, wshape, False, ops.conv_plan(g, 2)[0])[0]
+def _plain_wgrad(g, x, dz, wshape, simt=False):
+    return ops.conv_wgrad(g, x, dz, wshape, False, ALGO_SIMT if simt else ops.conv_plan(g, 2)[0])[0]
 
 
 class ConvDgradFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, dz, weight, g):
-        ctx.g = g
+    def forward(ctx, dz, weight, g, simt=False):
+        ctx.g, ctx.simt = g, simt
         ctx.save_for_backward(dz, weight)
-        return _plain_dgrad(g, _as_cl(dz.detach()), weight.detach())
+        return _plain_dgrad(g, _as_cl(dz.detach()), weight.detach(), simt)
 
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, u):
         dz, weight = ctx.saved_tensors
-        g, u = ctx.g, _as_cl(u)
-        ddz = _plain_fprop(g, u, weight.detach()) if ctx.needs_input_grad[0] else None
-        dw = _plain_wgrad(g, u, _as_cl(dz.detach()), tuple(weight.shape)) if ctx.needs_input_grad[1] else None
-        return ddz, dw, None
+        g, u, simt = ctx.g, _as_cl(u), ctx.simt
+        ddz = _plain_fprop(g, u, weight.detach(), simt) if ctx.needs_input_grad[0] else None
+        dw = _plain_wgrad(g, u, _as_cl(dz.detach()), tuple(weight.shape), simt) if ctx.needs_input_grad[1] else None
+        return ddz, dw, None, None
 
 
 class ConvWgradFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, dz, g, wshape):
-        ctx.g = g
+    def forward(ctx, x, dz, g, wshape, simt=False):
+        ctx.g, ctx.simt = g, simt
         ctx.save_for_backward(x, dz)
-        return _plain_wgrad(g, _as_cl(x.detach()), _as_cl(dz.detach()), wshape)
+        return _plain_wgrad(g, _as_cl(x.detach()), _as_cl(dz.detach()), wshape, simt)
 
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, v):
         x, dz = ctx.saved_tensors
-        g, v = ctx.g, v.contiguous()
-        dx = _plain_dgrad(g, _as_cl(dz.detach()), v) if ctx.needs_input_grad[0] else None
-        ddz = _plain_fprop(g, _as_cl(x.detach()), v) if ctx.needs_input_grad[1] else None
-        return dx, ddz, None, None
+        g, v, simt = ctx.g, v.contiguous(), ctx.simt
+        dx = _plain_dgrad(g, _as_cl(dz.detach()), v, simt) if ctx.needs_input_grad[0] else None
+        ddz = _plain_fprop(g, _as_cl(x.detach()), v, simt) if ctx.needs_input_grad[1] else None
+        return dx, ddz, None, None, None
 
 
 def _conv_backward_differentiable(ctx, dy):
     """(dx, dw, db) of a conv block [+bias] [act] [* Dropout2d scale] from differentiable nodes, for a backward under
-    autograd.grad(..., create_graph=True).  ctx: a ConvFn / NbConvFn context, which saves (x, weight, y, chan_scale)
-    and has .spec (act, slope), .g and .has_bias.  dz is rebuilt from (y, act, slope, chan_scale)."""
+    autograd.grad(..., create_graph=True).  ctx: a ConvFn context, which saves (x, weight, y, chan_scale) and has
+    .spec (act, slope), .g and .has_bias."""
     x, weight, y, chan_scale = ctx.saved_tensors
-    act, slope, g = ctx.spec.act, ctx.spec.slope, ctx.g
+    nig = ctx.needs_input_grad
+    return _conv_bwd_nodes(dy, x, weight, y, chan_scale, ctx.spec.act, ctx.spec.slope, ctx.g, nig[0], nig[1],
+                           ctx.has_bias and nig[2])
+
+
+def _conv_bwd_nodes(dy, x, weight, y, chan_scale, act, slope, g, need_dx, need_dw, need_db, simt=False):
+    """_conv_backward_differentiable on explicit operands: x is the conv's input (a differentiable recomputation of it
+    when the conv reads a virtual BatchNorm output); dz is rebuilt from (y, act, slope, chan_scale)."""
     if chan_scale is not None and act in (ACT_TANH, ACT_SIGMOID):
         raise NotImplementedError("b200gan: double backward through Dropout2d fused with tanh / sigmoid")
     dz = dy
@@ -232,10 +241,80 @@ def _conv_backward_differentiable(ctx, dy):
         dz = dz * (y * (1 - y))
     if chan_scale is not None:
         dz = dz * chan_scale.view(chan_scale.shape[0], chan_scale.shape[1], 1, 1)
-    dx = ConvDgradFn.apply(dz, weight, g) if ctx.needs_input_grad[0] else None
-    dw = ConvWgradFn.apply(x, dz, g, tuple(weight.shape)) if ctx.needs_input_grad[1] else None
-    db = dz.sum((0, 2, 3)) if (ctx.has_bias and ctx.needs_input_grad[2]) else None
+    dx = ConvDgradFn.apply(dz, weight, g, simt) if need_dx else None
+    dw = ConvWgradFn.apply(x, dz, g, tuple(weight.shape), simt) if need_dw else None
+    db = dz.sum((0, 2, 3)) if need_db else None
     return dx, dw, db
+
+
+# ---- double backward through training-mode norms (SURVEY.md 8f N2: penalties on normalised conv critics) --------------
+def _refuse_second_order_act(act, what):
+    if act in (ACT_TANH, ACT_SIGMOID):
+        raise NotImplementedError(f"b200gan: double backward through {what} fused with tanh / sigmoid (its activation "
+                                  "has a second-order term of its own)")
+
+
+def _norm_params_grads(dgb, n, c, per_sample):
+    """(dgamma, dbeta) per channel from the [2][G] per-group output of the norm backward"""
+    groups = dgb.numel() // 2
+    dgamma, dbeta = dgb[:groups], dgb[groups:]
+    if per_sample:  # affine InstanceNorm2d: parameters are shared across samples
+        dgamma, dbeta = dgamma.view(n, c).sum(0), dbeta.view(n, c).sum(0)
+    return dgamma, dbeta
+
+
+class NormBwdFn(torch.autograd.Function):
+    """The first-order backward of NormFn, (dy, x, gamma) -> (dx, dgamma, dbeta), as a node that can be differentiated
+    once more (autograd.grad(..., create_graph=True) through a training-mode norm).  mean_rstd / scale_shift are the
+    batch statistics of x and its affine transform; the double backward (ops.norm_double_backward) includes their
+    dependence on x.  Activation none / LeakyReLU / ReLU, the mask recomputed from x."""
+
+    @staticmethod
+    def forward(ctx, dy, x, gamma, mean_rstd, scale_shift, spec, need_params):
+        ctx.set_materialize_grads(False)
+        dy = _as_cl(dy.detach())
+        dx, dgb = ops.norm_backward(dy, x.detach(), None, mean_rstd, None if gamma is None else gamma.detach(),
+                                    spec.per_sample, spec.eps, spec.act, spec.slope, need_params, spec.rtf_dx,
+                                    scale_shift)
+        ctx.spec, ctx.dy = spec, dy
+        ctx.save_for_backward(x, gamma, mean_rstd, scale_shift)
+        if not need_params:
+            return dx, None, None
+        return (dx,) + _norm_params_grads(dgb, x.shape[0], x.shape[1], spec.per_sample)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, u, ugamma, ubeta):
+        x, gamma, mean_rstd, scale_shift = ctx.saved_tensors
+        spec, nig = ctx.spec, ctx.needs_input_grad
+        need_ggamma = gamma is not None and nig[2]
+        if (u is None and ugamma is None and ubeta is None) or not (nig[0] or nig[1] or need_ggamma):
+            return (None,) * 7
+        u = torch.zeros_like(x, memory_format=torch.channels_last) if u is None else _as_cl(u)
+        ugb = None
+        if gamma is not None and (ugamma is not None or ubeta is not None):
+            zero = torch.zeros_like(gamma)
+            ugb = torch.cat([zero if ugamma is None else ugamma, zero if ubeta is None else ubeta]).contiguous()
+        gx, gdy, gg = ops.norm_double_backward(ctx.dy, x.detach(), mean_rstd, scale_shift,
+                                               None if gamma is None else gamma.detach(), u, ugb, spec.per_sample,
+                                               spec.act, spec.slope, nig[1], nig[0], need_ggamma)
+        if gg is not None and spec.per_sample:
+            gg = gg.view(x.shape[0], x.shape[1]).sum(0)
+        return gdy, gx, gg, None, None, None, None
+
+
+def _norm_recompute(x, gamma, beta, spec):
+    """(NormFn output, mean_rstd, scale_shift) of x with batch statistics and no running-statistics update: the
+    normalised tensor a fused node never kept, recomputed as a differentiable function of (x, gamma, beta)."""
+    box = []
+    y = NormFn.apply(x, gamma, beta, None, None, None, None, spec, box)
+    return (y,) + box[0]
+
+
+def _bn_consts(a, gamma, beta, eps):
+    """(mean_rstd, scale_shift) of a BatchNorm2d of `a` with batch statistics, without a running-statistics update"""
+    return ops.norm_finalize(a.shape, ops.norm_stats(a, False), gamma, beta, None, None, None, False, eps, 0.0,
+                             a.device)
 
 
 
@@ -243,13 +322,16 @@ class NormFn(torch.autograd.Function):
     """Training-mode BatchNorm2d / InstanceNorm2d with an optional fused activation."""
 
     @staticmethod
-    def forward(ctx, x, gamma, beta, stats, running_mean, running_var, nbt, spec: NormSpec):
+    def forward(ctx, x, gamma, beta, stats, running_mean, running_var, nbt, spec: NormSpec, box=None):
+        """box: None, or a list that receives (mean_rstd, scale_shift) (_norm_recompute)"""
         ops._require_cuda(x, "norm input")
         x = _as_cl(x)
         y, mean_rstd, scale_shift = ops.norm_forward(
             x, None if gamma is None else gamma.detach(), None if beta is None else beta.detach(), running_mean,
             running_var, nbt, spec.per_sample, spec.eps, spec.momentum, spec.act, spec.slope, stats, spec.rtf_out,
             return_scale_shift=True)
+        if box is not None:
+            box.append((mean_rstd, scale_shift))
         ctx.spec = spec
         # LeakyReLU / ReLU masks are recomputed from x in backward (sign of x * scale + shift): y need not be kept
         mask_from_x = spec.act in (ACT_LRELU, ACT_RELU)
@@ -258,22 +340,23 @@ class NormFn(torch.autograd.Function):
         return y
 
     @staticmethod
-    @torch.autograd.function.once_differentiable
     def backward(ctx, dy):
         x, y, mean_rstd, gamma, scale_shift = ctx.saved_tensors
         spec = ctx.spec
-        dy = _as_cl(dy)
         need_params = gamma is not None and (ctx.needs_input_grad[1] or ctx.needs_input_grad[2])
+        if torch.is_grad_enabled():
+            # autograd.grad(..., create_graph=True): a gradient penalty through this norm (dragan.py:144-167,
+            # dualgan.py:116-135) differentiates THROUGH this backward
+            _refuse_second_order_act(spec.act, "a normalisation")
+            dx, dgamma, dbeta = NormBwdFn.apply(dy, x, gamma, mean_rstd, scale_shift, spec, need_params)
+            return dx, dgamma, dbeta, None, None, None, None, None, None
+        x, dy = x.detach(), _as_cl(dy.detach())
         dx, dgb = ops.norm_backward(dy, x, y, mean_rstd, None if gamma is None else gamma.detach(), spec.per_sample,
                                     spec.eps, spec.act, spec.slope, need_params, spec.rtf_dx, scale_shift)
         dgamma = dbeta = None
         if need_params:
-            n, c = x.shape[0], x.shape[1]
-            groups = dgb.numel() // 2
-            dgamma, dbeta = dgb[:groups], dgb[groups:]
-            if spec.per_sample:  # affine InstanceNorm2d: parameters are shared across samples
-                dgamma, dbeta = dgamma.view(n, c).sum(0), dbeta.view(n, c).sum(0)
-        return dx, dgamma, dbeta, None, None, None, None, None
+            dgamma, dbeta = _norm_params_grads(dgb, x.shape[0], x.shape[1], spec.per_sample)
+        return dx, dgamma, dbeta, None, None, None, None, None, None
 
 
 class NormConvFn(torch.autograd.Function):
@@ -305,7 +388,7 @@ class NormConvFn(torch.autograd.Function):
         ctx.has_bias = bias is not None
         # the norm output `a` is the conv's weight-gradient operand; the conv's output is kept only for its activation
         ctx.save_for_backward(x, mean_rstd, scale_shift, gamma, a, weight, y if cspec.act != ACT_NONE else None,
-                              chan_scale)
+                              chan_scale, beta)
         if out_stats is not None:
             ctx.mark_non_differentiable(out_stats)
             ctx.set_materialize_grads(False)
@@ -313,16 +396,30 @@ class NormConvFn(torch.autograd.Function):
         return y
 
     @staticmethod
-    @torch.autograd.function.once_differentiable
     def backward(ctx, dy, *unused):
-        x, mean_rstd, scale_shift, gamma, a, weight, y, chan_scale = ctx.saved_tensors
+        x, mean_rstd, scale_shift, gamma, a, weight, y, chan_scale, beta = ctx.saved_tensors
         nspec, cspec, g = ctx.nspec, ctx.cspec, ctx.g
-        dy = _as_cl(dy)
+        nig = ctx.needs_input_grad
+        if torch.is_grad_enabled():
+            # create_graph=True: the norm output recomputed as a differentiable NormFn output (no running-statistics
+            # update), the conv's differentiable backward on it, and the norm's backward as NormBwdFn
+            if cspec.up != 1 or cspec.pad_mode != PAD_ZERO:
+                raise NotImplementedError("b200gan: double backward through a conv with a folded upsample / reflection "
+                                          "padding")
+            _refuse_second_order_act(nspec.act, "a normalisation")
+            need_params = gamma is not None and (nig[1] or nig[2])
+            a, mr, ss = _norm_recompute(x, gamma, beta, nspec)
+            da, dw, db = _conv_bwd_nodes(dy, a, weight, y, chan_scale, cspec.act, cspec.slope, g, nig[0] or need_params,
+                                         nig[7], ctx.has_bias and nig[8])
+            dx = dgamma = dbeta = None
+            if da is not None:
+                dx, dgamma, dbeta = NormBwdFn.apply(da, x, gamma, mr, ss, nspec, need_params)
+            return dx, dgamma, dbeta, None, None, None, None, dw, db, None, None, None, None
+        x, a, y, dy = x.detach(), a.detach(), None if y is None else y.detach(), _as_cl(dy.detach())
         if cspec.act != ACT_NONE or chan_scale is not None:
             dz = ops.epilogue_bwd(dy, y, chan_scale, cspec.act, cspec.slope, cspec.rtf_dz)
         else:
             dz = dy
-        nig = ctx.needs_input_grad
         dx = dgamma = dbeta = dw = db = None
         need_params = gamma is not None and (nig[1] or nig[2])
         if nig[0] or need_params:
@@ -382,11 +479,13 @@ class TailFn(torch.autograd.Function):
         return out
 
     @staticmethod
-    @torch.autograd.function.once_differentiable
     def backward(ctx, dout):
+        if torch.is_grad_enabled():
+            raise NotImplementedError("b200gan: double backward (create_graph=True) through the fused generator tail "
+                                      "(BatchNorm2d -> activation -> Conv2d(C, K<=3, 3, 1, 1))")
         a, mean_rstd, scale_shift, weight, out = ctx.saved_tensors
         spec = ctx.spec
-        dout = _as_cl(dout)
+        a, out, dout = a.detach(), None if out is None else out.detach(), _as_cl(dout.detach())
         g = ops.epilogue_bwd(dout, out, None, spec.act_out, 0.0) if spec.act_out != ACT_NONE else dout
         need_affine = ctx.has_affine and (ctx.needs_input_grad[2] or ctx.needs_input_grad[3])
         need_bias = ctx.has_bias and ctx.needs_input_grad[8]
@@ -410,12 +509,19 @@ class AffineActFn(torch.autograd.Function):
         return y
 
     @staticmethod
-    @torch.autograd.function.once_differentiable
     def backward(ctx, dy):
         y, scale_shift = ctx.saved_tensors
-        dy = _as_cl(dy)
-        dz = ops.epilogue_bwd(dy, y, None, ctx.act, ctx.slope) if ctx.act != ACT_NONE else dy
         c = y.shape[1]
+        if torch.is_grad_enabled():
+            # create_graph=True: linear in x apart from the piecewise-constant mask, so differentiable torch ops suffice
+            _refuse_second_order_act(ctx.act, "an eval-mode BatchNorm2d")
+            if ctx.act == ACT_LRELU:
+                dy = dy * torch.where(y > 0, 1.0, ctx.slope)
+            elif ctx.act == ACT_RELU:
+                dy = dy * (y > 0).to(dy.dtype)
+            return dy * scale_shift[:c].view(1, c, 1, 1), None, None, None
+        y, dy = y.detach(), _as_cl(dy.detach())
+        dz = ops.epilogue_bwd(dy, y, None, ctx.act, ctx.slope) if ctx.act != ACT_NONE else dy
         zero = torch.zeros_like(scale_shift)
         zero[:c] = scale_shift[:c]
         # dx = dz * scale: an affine apply with shift = 0
@@ -509,6 +615,33 @@ class NbSpec:
     groups: int = 1           # statistics groups of the batch (ops.bn_groups)
 
 
+class ChainPass:
+    """Shared by the nodes of one forward of a fused chain.  Once a backward under create_graph=True has run through the
+    chain, its grad-mode nodes feed TRUE gradients (w.r.t. the stored raw outputs a_l) back into the chain's forward
+    nodes, which the virtual-gradient protocol would add to virtual ones.  So from then on (true_grads) every first-order
+    backward of these nodes takes and returns true gradients: each node finishes the backward of its own input
+    BatchNorm and calls nb_dz without an output edge."""
+
+    def __init__(self):
+        self.true_grads = False
+
+
+def _finish_bn(g, a, edge, sums, need_gamma, need_beta):
+    """(da, dgamma, dbeta): the backward of the chain BatchNorm `edge` on its raw input a, given the gradient g w.r.t.
+    its (virtual) output and sums = (sum g, sum g * ahat) from nb_dgrad / nb_tail_bwd; hands `sums` back zeroed"""
+    mean_rstd, _ = _bn_consts(a, edge.gamma, edge.beta, edge.eps)
+    need = edge.gamma is not None and (need_gamma or need_beta)
+    da, dgb = ops.norm_backward_from_sums(g, a, mean_rstd, edge.gamma, sums, edge.eps, need_params=need)
+    c = a.shape[1]
+    return da, (dgb[:c] if need and need_gamma else None), (dgb[c:] if need and need_beta else None)
+
+
+def _refuse_grouped_chain(groups):
+    if groups > 1:
+        raise NotImplementedError("b200gan: double backward (create_graph=True) through a fused chain under "
+                                  "ops.bn_groups > 1")
+
+
 class NbConvFn(torch.autograd.Function):
     """One layer of a fused narrow chain (csrc/narrow_block.cu): conv over the (virtually normalised) stored output of
     the previous layer, + bias, activation, Dropout2d scale, + the batch sums for the following BatchNorm.
@@ -517,10 +650,12 @@ class NbConvFn(torch.autograd.Function):
     incoming gradient is w.r.t. the VIRTUAL normalised output (the consumer could not finish the BatchNorm backward
     without the batch sums); by then the consumer has stored those sums in out_edge.sums.  This node finishes the norm
     backward (nb_dz), computes its parameter gradients, and hands ITS producer a virtual gradient plus in_edge.sums.
-    Only valid when the stored output has exactly one consumer: the next node of the same chain."""
+    Only valid when the stored output has exactly one consumer: the next node of the same chain.  After a backward under
+    create_graph=True, true gradients instead (ChainPass)."""
 
     @staticmethod
-    def forward(ctx, x, weight, bias, chan_scale, in_gamma, in_beta, in_rm, in_rv, in_nbt, in_edge, out_box, spec, cache):
+    def forward(ctx, x, weight, bias, chan_scale, in_gamma, in_beta, in_rm, in_rv, in_nbt, in_edge, out_box, spec, cache,
+                chain):
         ops._require_cuda(x, "conv input")
         x = _as_cl(x)
         g, _ = ops.make_geom(tuple(x.shape), tuple(weight.shape), spec.stride, (spec.pad,) * 4)
@@ -528,9 +663,9 @@ class NbConvFn(torch.autograd.Function):
         packed = cache.get(g, w, PACK_SIMT_FPROP)
         y, stats = ops.nb_fprop(g, x, packed, None if bias is None else bias.detach(), spec.act, spec.slope, chan_scale,
                                 in_edge, in_rm, in_rv, in_nbt, spec.momentum, spec.want_stats, spec.groups)
-        ctx.g, ctx.spec, ctx.cache, ctx.in_edge, ctx.out_box = g, spec, cache, in_edge, out_box
+        ctx.g, ctx.spec, ctx.cache, ctx.in_edge, ctx.out_box, ctx.chain = g, spec, cache, in_edge, out_box, chain
         ctx.has_bias = bias is not None
-        ctx.save_for_backward(x, weight, y, chan_scale)
+        ctx.save_for_backward(x, weight, y, chan_scale, in_gamma, in_beta)
         if spec.want_stats:
             ctx.mark_non_differentiable(stats)
             return y, stats
@@ -538,16 +673,34 @@ class NbConvFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, gy, *unused):
-        x, weight, y, chan_scale = ctx.saved_tensors
+        x, weight, y, chan_scale, in_gamma, in_beta = ctx.saved_tensors
         g, spec, in_edge = ctx.g, ctx.spec, ctx.in_edge
         out_edge = ctx.out_box[0] if ctx.out_box else None
+        nig = ctx.needs_input_grad
         if torch.is_grad_enabled():
             # autograd.grad(..., create_graph=True) through a chain: the gradient penalty of a conv critic (SURVEY.md 8f
-            # N2; critics carry no BatchNorm, stargan/models.py:87-115).  Same differentiable nodes as ConvFn.
-            if in_edge is not None or out_edge is not None:
-                raise NotImplementedError("b200gan: double backward through a fused conv chain with BatchNorm2d; set "
-                                          "B200GAN_FUSE_CHAIN=0 for this model")
-            return _conv_backward_differentiable(ctx, gy) + (None,) * 10
+            # N2: stargan.py:142-161 without norms, dragan.py:144-167 with BatchNorm2d).  gy and the returned gradient
+            # are TRUE gradients w.r.t. the raw stored tensors: the input BatchNorm's output is recomputed as a
+            # differentiable NormFn output, the conv runs the same differentiable nodes as ConvFn, and the norm's
+            # backward is NormBwdFn.  edge.sums is neither read nor written.
+            _refuse_grouped_chain(spec.groups)
+            ctx.chain.true_grads = True
+            need_params = in_edge is not None and in_gamma is not None and (nig[4] or nig[5])
+            xin, mr, ss = x, None, None
+            if in_edge is not None:
+                xin, mr, ss = _norm_recompute(x, in_gamma, in_beta, NormSpec(eps=in_edge.eps))
+            dxin, dw, db = _conv_bwd_nodes(gy, xin, weight, y, chan_scale, spec.act, spec.slope, g, nig[0] or need_params,
+                                           nig[1], ctx.has_bias and nig[2],
+                                           simt=in_edge is not None or out_edge is not None)
+            gx = dgamma = dbeta = None
+            if in_edge is None:
+                gx = dxin
+            elif dxin is not None:
+                gx, dgamma, dbeta = NormBwdFn.apply(dxin, x, in_gamma, mr, ss, NormSpec(eps=in_edge.eps), need_params)
+            return gx, dw, db, None, dgamma, dbeta, None, None, None, None, None, None, None, None
+        true_grads = ctx.chain.true_grads
+        if true_grads:
+            out_edge = None  # gy is w.r.t. the stored output itself
         gy, y, x = gy.detach(), y.detach(), x.detach()
         if out_edge is not None and out_edge.sums is None:
             raise RuntimeError("b200gan: fused conv chain: the consumer of this layer did not run its backward first")
@@ -562,7 +715,9 @@ class NbConvFn(torch.autograd.Function):
         if need_in:
             packed = ctx.cache.get(g, weight.detach(), PACK_SIMT_DGRAD)
             gx, sums = ops.nb_dgrad(g, dz, packed, in_edge, x)
-            if in_edge is not None:
+            if in_edge is not None and true_grads:
+                gx, dgamma, dbeta = _finish_bn(gx, x, in_edge, sums, ctx.needs_input_grad[4], ctx.needs_input_grad[5])
+            elif in_edge is not None:
                 in_edge.sums = sums
                 c = g.C
                 if ctx.needs_input_grad[4] or ctx.needs_input_grad[5]:
@@ -570,27 +725,38 @@ class NbConvFn(torch.autograd.Function):
                     dgb = sums.float() if in_edge.groups == 1 else sums.view(in_edge.groups, 2 * c).sum(0).float()
                     dgamma = dgb[c:] if ctx.needs_input_grad[4] else None
                     dbeta = dgb[:c] if ctx.needs_input_grad[5] else None
-        return gx, dw, db, None, dgamma, dbeta, None, None, None, None, None, None, None
+        return gx, dw, db, None, dgamma, dbeta, None, None, None, None, None, None, None, None
 
 
 class NbTailFn(torch.autograd.Function):
     """End of a fused narrow chain: the last BatchNorm's output as a real tensor (optionally NCHW-contiguous: the layout
-    the script's `.view(N, -1)` needs, dcgan.py:96)."""
+    the script's `.view(N, -1)` needs, dcgan.py:96).  Returns a virtual gradient as NbConvFn does, or, under
+    create_graph=True and after it (ChainPass), the true gradient w.r.t. `a`."""
 
     @staticmethod
-    def forward(ctx, a, gamma, beta, rm, rv, nbt, edge, momentum, nchw):
+    def forward(ctx, a, gamma, beta, rm, rv, nbt, edge, momentum, nchw, chain):
         a = _as_cl(a)
         out = ops.nb_tail_fwd(a, edge, rm, rv, nbt, momentum, nchw)
-        ctx.edge, ctx.nchw = edge, nchw
-        ctx.save_for_backward(a)
+        ctx.edge, ctx.nchw, ctx.chain = edge, nchw, chain
+        ctx.save_for_backward(a, gamma, beta)
         return out
 
     @staticmethod
-    @torch.autograd.function.once_differentiable
     def backward(ctx, dout):
-        (a,) = ctx.saved_tensors
+        a, gamma, beta = ctx.saved_tensors
+        nig = ctx.needs_input_grad
+        if torch.is_grad_enabled():
+            _refuse_grouped_chain(ctx.edge.groups)
+            ctx.chain.true_grads = True
+            mr, ss = _bn_consts(a.detach(), ctx.edge.gamma, ctx.edge.beta, ctx.edge.eps)
+            need_params = gamma is not None and (nig[1] or nig[2])
+            da, dgamma, dbeta = NormBwdFn.apply(dout, a, gamma, mr, ss, NormSpec(eps=ctx.edge.eps), need_params)
+            return da, dgamma, dbeta, None, None, None, None, None, None, None
+        a, dout = a.detach(), dout.detach()
         dout = dout.contiguous() if ctx.nchw else _as_cl(dout)
         g, sums = ops.nb_tail_bwd(a, ctx.edge, dout, ctx.nchw)
+        if ctx.chain.true_grads:
+            return _finish_bn(g, a, ctx.edge, sums, nig[1], nig[2]) + (None,) * 7
         ctx.edge.sums = sums
         c = a.shape[1]
         dgamma = dbeta = None
@@ -599,7 +765,7 @@ class NbTailFn(torch.autograd.Function):
             dgb = sums.float() if grp == 1 else sums.view(grp, 2 * c).sum(0).float()
             dgamma = dgb[c:] if ctx.needs_input_grad[1] else None
             dbeta = dgb[:c] if ctx.needs_input_grad[2] else None
-        return g, dgamma, dbeta, None, None, None, None, None, None
+        return g, dgamma, dbeta, None, None, None, None, None, None, None
 
 
 class _tf32_matmul:

@@ -666,6 +666,7 @@ class Sequential(_T["Sequential"]):
                     part = _dropout2d_scale((x.shape[0] // groups, cs.conv.out_channels), cs.dropout2d.p, x.device)
                     scales[li] = part if scales[li] is None else torch.cat([scales[li], part])
         edge, prev_norm = None, None
+        chain = F.ChainPass()
         for li, (cs, ns, oshape) in enumerate(plan):
             conv = cs.conv
             scale = scales[li]
@@ -683,7 +684,8 @@ class Sequential(_T["Sequential"]):
                 cache = PackCache()
                 conv.__dict__["_b200_cache"] = cache
             out_box = []
-            res = F.NbConvFn.apply(x, conv.weight, conv.bias, scale, gam, bet, rm, rv, nbt, edge, out_box, spec, cache)
+            res = F.NbConvFn.apply(x, conv.weight, conv.bias, scale, gam, bet, rm, rv, nbt, edge, out_box, spec, cache,
+                                   chain)
             if ns is not None:
                 x, stats = res
                 norm = ns.norm
@@ -700,7 +702,7 @@ class Sequential(_T["Sequential"]):
             momentum = 0.0
             if norm.track_running_stats and norm.running_mean is not None:
                 rm, rv, nbt, momentum = norm.running_mean, norm.running_var, norm.num_batches_tracked, float(norm.momentum)
-            x = F.NbTailFn.apply(x, norm.weight, norm.bias, rm, rv, nbt, edge, momentum, bool(nchw_out))
+            x = F.NbTailFn.apply(x, norm.weight, norm.bias, rm, rv, nbt, edge, momentum, bool(nchw_out), chain)
         return x
 
     def _forward_2d(self, x):

@@ -332,6 +332,22 @@ def norm_backward(dy, x, y, mean_rstd, gamma, per_sample, eps, act=ACT_NONE, slo
     return dx, dgb
 
 
+def norm_double_backward(dy, x, mean_rstd, scale_shift, gamma, u, ugamma_ubeta, per_sample, act, slope, need_gx,
+                         need_gdy, need_ggamma):
+    """Backward of norm_backward (act NONE / LRELU / RELU): (gx, gdy, ggamma per group), each None unless asked for.
+    u: the gradient w.r.t. dx; ugamma_ubeta: [2][C] gradients w.r.t. dgamma, dbeta, or None (= 0)."""
+    d = _norm_desc(x.shape, per_sample, 0.0, 0.0, act, slope, False)
+    groups = mean_rstd.numel() // 2
+    sums = zero_scratch(x.device, 5 * groups)
+    gx = torch.empty_like(x, memory_format=CL) if need_gx else None
+    gdy = torch.empty_like(x, memory_format=CL) if need_gdy else None
+    gg = torch.empty(groups, device=x.device, dtype=torch.float32) if need_ggamma else None
+    _lib.check(_lib.load().b200gan_norm_dbwd(ctypes.byref(d), dy.data_ptr(), x.data_ptr(), mean_rstd.data_ptr(),
+                                             _ptr(scale_shift), _ptr(gamma), u.data_ptr(), _ptr(ugamma_ubeta),
+                                             sums.data_ptr(), _ptr(gx), _ptr(gdy), _ptr(gg), _stream()), "norm_dbwd")
+    return gx, gdy, gg
+
+
 # ---- BatchNorm2d [act] [Upsample x2] Conv2d backward: the norm's sums from the conv's data-gradient epilogue ----------
 def conv_dgrad_norm_supported(g):
     if Config.algo == "simt":

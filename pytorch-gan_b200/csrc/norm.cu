@@ -158,12 +158,73 @@ __device__ __forceinline__ float norm_act_grad(float xv, float sc, float sh, flo
   return act_grad_from_out(yv, act, slope);
 }
 
+// the block's per-thread partials red[t][0 .. n) summed per group in fp64 and added to out[j * G + g], j < n
+template <int VEC>
+__device__ __forceinline__ void norm_block_sums(float (&red)[256][2 * VEC], const GroupSlice &s, int gbase, int G,
+                                                int n, double *__restrict__ out) {
+  __syncthreads();
+  if (threadIdx.x < s.CVs) {
+    for (int k = 0; k < n; ++k) {
+      double t = 0.0;
+      for (int r = 0; r < s.rpb; ++r) t += (double)red[r * s.CVs + threadIdx.x][k];
+      atomicAdd(out + (k / VEC) * G + gbase + k % VEC, t);
+    }
+  }
+}
+
+// double-backward mode of pass 1 (u given, act none / LeakyReLU / ReLU with the mask from x): sums[g] += sum u,
+// sums[G+g] += sum u * xhat, sums[2G+g] += sum u * dy'.  The third sum goes through the shared slots after the first two.
+template <int VEC>
+__device__ __forceinline__ void norm_dbwd_reduce(float (&red)[256][2 * VEC], const GroupSlice &s, int gbase,
+                                                 const float *__restrict__ dy, const float *__restrict__ x,
+                                                 const float *__restrict__ u, const float (&mean)[VEC],
+                                                 const float (&rstd)[VEC], const float (&sc)[VEC],
+                                                 const float (&sh)[VEC], double *__restrict__ sums, int64_t rows,
+                                                 int G, int act, float slope) {
+  using V = typename vec_of<VEC>::type;
+  const int64_t base = (gridDim.y > 1 ? (int64_t)blockIdx.y * rows : 0);
+  const V *dyv = reinterpret_cast<const V *>(dy) + base * s.CV + s.cv;
+  const V *xv = reinterpret_cast<const V *>(x) + base * s.CV + s.cv;
+  const V *uv = reinterpret_cast<const V *>(u) + base * s.CV + s.cv;
+  float su[VEC], st[VEC], sq[VEC];
+#pragma unroll
+  for (int j = 0; j < VEC; ++j) su[j] = st[j] = sq[j] = 0.f;
+  const int CV = s.CV;
+  const int64_t step = (int64_t)gridDim.x * s.rpb;
+#pragma unroll 2
+  for (int64_t r = s.first_row(rows); r < rows; r += step) {
+    float dd[VEC], xx[VEC], uu[VEC];
+    unpack(__ldg(dyv + r * CV), dd);
+    unpack(__ldg(xv + r * CV), xx);
+    unpack(__ldg(uv + r * CV), uu);
+#pragma unroll
+    for (int j = 0; j < VEC; ++j) {
+      const float g = dd[j] * norm_act_grad(xx[j], sc[j], sh[j], 0.f, true, act, slope);
+      su[j] += uu[j];
+      st[j] = fmaf(uu[j], (xx[j] - mean[j]) * rstd[j], st[j]);
+      sq[j] = fmaf(uu[j], g, sq[j]);
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < VEC; ++j) {
+    red[threadIdx.x][j] = su[j];
+    red[threadIdx.x][VEC + j] = st[j];
+  }
+  norm_block_sums<VEC>(red, s, gbase, G, 2 * VEC, sums);
+  __syncthreads();
+#pragma unroll
+  for (int j = 0; j < VEC; ++j) red[threadIdx.x][j] = sq[j];
+  norm_block_sums<VEC>(red, s, gbase, G, VEC, sums + 2 * G);
+}
+
 // pass 1: sums[g] += sum dy', sums[G+g] += sum dy' * xhat   with dy' = dy * act'
+// (u != NULL: the double-backward mode norm_dbwd_reduce, into sums[0 .. 3G))
 template <int VEC>
 __global__ void __launch_bounds__(256)
 norm_bwd_reduce_kernel(const float *__restrict__ dy, const float *__restrict__ x, const float *__restrict__ y,
                        const float *__restrict__ mean_rstd, const float *__restrict__ scale_shift,
-                       double *__restrict__ sums, int64_t rows, int C, int G, int act, float slope) {
+                       double *__restrict__ sums, int64_t rows, int C, int G, int act, float slope,
+                       const float *__restrict__ u) {
   using V = typename vec_of<VEC>::type;
   __shared__ float red[256][2 * VEC];
   const GroupSlice s(C, VEC);
@@ -176,6 +237,10 @@ norm_bwd_reduce_kernel(const float *__restrict__ dy, const float *__restrict__ x
     rstd[j] = __ldg(mean_rstd + G + gbase + j);
     sc[j] = from_x ? __ldg(scale_shift + gbase + j) : 1.f;
     sh[j] = from_x ? __ldg(scale_shift + G + gbase + j) : 0.f;
+  }
+  if (u != nullptr) {
+    norm_dbwd_reduce<VEC>(red, s, gbase, dy, x, u, mean, rstd, sc, sh, sums, rows, G, act, slope);
+    return;
   }
   const int64_t base = (gridDim.y > 1 ? (int64_t)blockIdx.y * rows : 0);
   const V *dyv = reinterpret_cast<const V *>(dy) + base * s.CV + s.cv;
@@ -222,16 +287,87 @@ norm_bwd_reduce_kernel(const float *__restrict__ dy, const float *__restrict__ x
   }
 }
 
+// double-backward mode of pass 2.  sums[5][G] = S1 = sum g, S2 = sum g * xhat, U = sum u, T = sum u * xhat,
+// Q = sum u * g over the m elements of a group, with g = dy * act'; A = S1/m, B = S2/m.  Per element
+//   gdy = act' * (gamma r (u - U/m - xhat T/m) + ugamma xhat + ubeta)
+//   gx  = ugamma r (g - A - xhat B) - (gamma r^2 / m) (xhat (Q - A U - 3 B T) + T (g - A) + B (m u - U))
+// written as gx = c1 g + c2 x + c3 u + c4 and gdy = act' (c5 u + c6 x + c7), the per-group constants formed in fp64
+// (xhat = x r - mean r is folded into c2, c4 and c6, c7).  c5 = gamma r is the forward's scale (the same fp32
+// product), so it shares the mask's register.  gx, gdy: either may be NULL.
+template <int VEC>
+__device__ __forceinline__ void norm_dbwd_apply(const GroupSlice &s, int gbase, const float *__restrict__ dy,
+                                                const float *__restrict__ x, const float *__restrict__ u,
+                                                const float *__restrict__ mean_rstd,
+                                                const float *__restrict__ scale_shift, const float *__restrict__ gamma,
+                                                const float *__restrict__ ugb, const double *__restrict__ sums,
+                                                float *__restrict__ gx, float *__restrict__ gdy, int64_t rows, int C,
+                                                int G, float inv_count, int act, float slope) {
+  using V = typename vec_of<VEC>::type;
+  const bool masked = act != B200GAN_ACT_NONE;
+  float k1[VEC], k2[VEC], k3[VEC], k4[VEC], k6[VEC], k7[VEC], sc[VEC], sh[VEC];
+#pragma unroll
+  for (int j = 0; j < VEC; ++j) {
+    const int g = gbase + j, c = s.cv * VEC + j;  // gamma and ugamma / ubeta are per channel, not per group
+    const double m = (double)rows, r = __ldg(mean_rstd + G + g), mu = __ldg(mean_rstd + g);
+    const double ga = gamma ? __ldg(gamma + c) : 1.0;
+    const double ug = ugb ? __ldg(ugb + c) : 0.0, ub = ugb ? __ldg(ugb + C + c) : 0.0;
+    const double A = sums[g] / m, B = sums[G + g] / m, Um = sums[2 * G + g] / m, Tm = sums[3 * G + g] / m;
+    const double Qm = sums[4 * G + g] / m;
+    const double gr = ga * r, gr2 = gr * r;
+    const double c1 = ug * r - gr2 * Tm;
+    const double c2 = -ug * r * B - gr2 * (Qm - A * Um - 3.0 * B * Tm);  // multiplies xhat
+    const double c6 = ug - gr * Tm;                                        // multiplies xhat
+    k1[j] = (float)c1;
+    k2[j] = (float)(c2 * r);
+    k3[j] = (float)(-gr2 * B);
+    k4[j] = (float)(-A * c1 + gr2 * B * Um - c2 * r * mu);
+    k6[j] = (float)(c6 * r);
+    k7[j] = (float)(ub - gr * Um - c6 * r * mu);
+    sc[j] = masked ? __ldg(scale_shift + g) : (float)gr;
+    sh[j] = masked ? __ldg(scale_shift + G + g) : 0.f;
+  }
+  const int64_t base = (gridDim.y > 1 ? (int64_t)blockIdx.y * rows : 0);
+  const V *dyv = reinterpret_cast<const V *>(dy) + base * s.CV + s.cv;
+  const V *xv = reinterpret_cast<const V *>(x) + base * s.CV + s.cv;
+  const V *uv = reinterpret_cast<const V *>(u) + base * s.CV + s.cv;
+  V *gxv = reinterpret_cast<V *>(gx) + base * s.CV + s.cv;
+  V *gdyv = reinterpret_cast<V *>(gdy) + base * s.CV + s.cv;
+  const int CV = s.CV;
+  const int64_t step = (int64_t)gridDim.x * s.rpb;
+#pragma unroll 1
+  for (int64_t r = s.first_row(rows); r < rows; r += step) {
+    float dd[VEC], xx[VEC], uu[VEC], o[VEC], p[VEC];
+    unpack(__ldg(xv + r * CV), xx);
+    unpack(__ldg(uv + r * CV), uu);
+    unpack(gx ? __ldg(dyv + r * CV) : V{}, dd);
+#pragma unroll
+    for (int j = 0; j < VEC; ++j) {
+      const float ap = norm_act_grad(xx[j], sc[j], sh[j], 0.f, true, act, slope);
+      o[j] = fmaf(k1[j], dd[j] * ap, fmaf(k2[j], xx[j], fmaf(k3[j], uu[j], k4[j])));
+      p[j] = ap * fmaf(sc[j], uu[j], fmaf(k6[j], xx[j], k7[j]));
+    }
+    if (gx) gxv[r * CV] = pack(o);
+    if (gdy) gdyv[r * CV] = pack(p);
+  }
+}
+
 // pass 2: dx = gamma*rstd * (dy' - mean(dy') - xhat * mean(dy' xhat))
+// (u != NULL: the double-backward mode norm_dbwd_apply, dx = gx)
 template <int VEC>
 __global__ void __launch_bounds__(256)
 norm_bwd_apply_kernel(const float *__restrict__ dy, const float *__restrict__ x, const float *__restrict__ y,
                       const float *__restrict__ mean_rstd, const float *__restrict__ scale_shift,
                       const float *__restrict__ gamma, const double *__restrict__ sums, float *__restrict__ dx,
-                      int64_t rows, int C, int G, float inv_count, int act, float slope, int rtf) {
+                      int64_t rows, int C, int G, float inv_count, int act, float slope, int rtf,
+                      const float *__restrict__ u, const float *__restrict__ ugb, float *__restrict__ gdy) {
   using V = typename vec_of<VEC>::type;
   const GroupSlice s(C, VEC);
   const int gbase = (gridDim.y > 1 ? blockIdx.y * C : 0) + s.cv * VEC;
+  if (u != nullptr) {
+    norm_dbwd_apply<VEC>(s, gbase, dy, x, u, mean_rstd, scale_shift, gamma, ugb, sums, dx, gdy, rows, C, G, inv_count,
+                         act, slope);
+    return;
+  }
   const bool from_x = scale_shift != nullptr && (act == B200GAN_ACT_LRELU || act == B200GAN_ACT_RELU);
   float mean[VEC], rstd[VEC], gr[VEC], m1[VEC], m2[VEC], sc[VEC], sh[VEC];
 #pragma unroll
@@ -268,10 +404,19 @@ norm_bwd_apply_kernel(const float *__restrict__ dy, const float *__restrict__ x,
   }
 }
 
-// pass 3: dgamma / dbeta per group; hands the workspace back zeroed
-__global__ void norm_bwd_params_kernel(double *__restrict__ sums, float *__restrict__ dgb, int G) {
+// pass 3: dgamma / dbeta per group; hands the workspace back zeroed.  Double-backward mode (mean_rstd given, sums[5][G]
+// as norm_dbwd_apply reads it): ggamma[g] = r (Q - S1 U / m - S2 T / m) (ggamma may be NULL)
+__global__ void norm_bwd_params_kernel(double *__restrict__ sums, float *__restrict__ dgb, int G,
+                                       const float *__restrict__ mean_rstd, float *__restrict__ ggamma, double count) {
   int g = blockIdx.x * blockDim.x + threadIdx.x;
   if (g >= G) return;
+  if (mean_rstd) {
+    if (ggamma)
+      ggamma[g] = (float)((double)mean_rstd[G + g] *
+                          (sums[4 * G + g] - (sums[g] * sums[2 * G + g] + sums[G + g] * sums[3 * G + g]) / count));
+    for (int k = 0; k < 5; ++k) sums[k * G + g] = 0.0;
+    return;
+  }
   if (dgb) {
     dgb[g] = (float)sums[G + g];  // dgamma = sum dy' * xhat
     dgb[G + g] = (float)sums[g];  // dbeta  = sum dy'
@@ -326,9 +471,9 @@ static int norm_bwd_apply_params(const b200gan_norm_desc *d, const float *dy, co
   const float inv = (float)(1.0 / (d->per_sample ? (double)d->HW : (double)d->N * (double)d->HW));
   auto apply = vec == 4 ? norm_bwd_apply_kernel<4> : norm_bwd_apply_kernel<1>;
   apply<<<grid, 256, 0, st>>>(dy, x, y, mean_rstd, scale_shift, gamma, sums, dx, rows, d->C, G, inv, d->act, d->slope,
-                              d->round_tf32);
+                              d->round_tf32, nullptr, nullptr, nullptr);
   B2_LAUNCH_CHECK();
-  norm_bwd_params_kernel<<<ceil_div(G, 128), 128, 0, st>>>(sums, dgamma_dbeta, G);
+  norm_bwd_params_kernel<<<ceil_div(G, 128), 128, 0, st>>>(sums, dgamma_dbeta, G, nullptr, nullptr, 0.0);
   B2_LAUNCH_CHECK();
   return B200GAN_OK;
 }
@@ -398,7 +543,7 @@ extern "C" int b200gan_norm_bwd(const b200gan_norm_desc *d, const float *dy, con
   int64_t rows;
   const dim3 grid = slice_grid(d, vec, rows);
   auto reduce = vec == 4 ? norm_bwd_reduce_kernel<4> : norm_bwd_reduce_kernel<1>;
-  reduce<<<grid, 256, 0, st>>>(dy, x, yy, mean_rstd, scale_shift, sums, rows, d->C, G, d->act, d->slope);
+  reduce<<<grid, 256, 0, st>>>(dy, x, yy, mean_rstd, scale_shift, sums, rows, d->C, G, d->act, d->slope, nullptr);
   B2_LAUNCH_CHECK();
   return norm_bwd_apply_params(d, dy, x, yy, mean_rstd, scale_shift, gamma, sums, dx, dgamma_dbeta, vec, grid, rows, st);
 }
@@ -415,4 +560,36 @@ extern "C" int b200gan_norm_bwd_from_sums(const b200gan_norm_desc *d, const floa
   const dim3 grid = slice_grid(d, vec, rows);
   return norm_bwd_apply_params(d, dy, x, x, mean_rstd, scale_shift, gamma, sums, dx, dgamma_dbeta, vec, grid, rows,
                                as_stream(stream));
+}
+
+extern "C" int b200gan_norm_dbwd(const b200gan_norm_desc *d, const float *dy, const float *x, const float *mean_rstd,
+                                 const float *scale_shift, const float *gamma, const float *u, const float *ugamma_ubeta,
+                                 double *sums, float *gx, float *gdy, float *ggamma_per_group, void *stream) {
+  if (int e = check_desc(d)) return e;
+  if (d->act != B200GAN_ACT_NONE && d->act != B200GAN_ACT_LRELU && d->act != B200GAN_ACT_RELU)
+    B2_UNSUPPORTED("norm_dbwd: a fused Tanh / Sigmoid has a second-order term of its own (activation %d)", d->act);
+  B2_CHECK_ARG(dy && x && mean_rstd && u && sums, "norm_dbwd: null pointer");
+  B2_CHECK_ARG(d->act == B200GAN_ACT_NONE || scale_shift, "norm_dbwd: LeakyReLU / ReLU needs scale_shift for the mask");
+  cudaStream_t st = as_stream(stream);
+  const int G = d->per_sample ? d->N * d->C : d->C;
+  const float *ss = d->act == B200GAN_ACT_NONE ? nullptr : scale_shift;
+  const int vec = vec_width(d->C, {dy, x, u, gx, gdy});
+  int64_t rows;
+  const dim3 grid = slice_grid(d, vec, rows);
+  auto reduce = vec == 4 ? norm_bwd_reduce_kernel<4> : norm_bwd_reduce_kernel<1>;
+  // S1, S2 as the first-order backward forms them, then U, T, Q
+  reduce<<<grid, 256, 0, st>>>(dy, x, x, mean_rstd, ss, sums, rows, d->C, G, d->act, d->slope, nullptr);
+  B2_LAUNCH_CHECK();
+  reduce<<<grid, 256, 0, st>>>(dy, x, x, mean_rstd, ss, sums + 2 * (int64_t)G, rows, d->C, G, d->act, d->slope, u);
+  B2_LAUNCH_CHECK();
+  if (gx || gdy) {
+    auto apply = vec == 4 ? norm_bwd_apply_kernel<4> : norm_bwd_apply_kernel<1>;
+    apply<<<grid, 256, 0, st>>>(dy, x, x, mean_rstd, ss, gamma, sums, gx, rows, d->C, G, 0.f, d->act, d->slope, 0, u,
+                                ugamma_ubeta, gdy);
+    B2_LAUNCH_CHECK();
+  }
+  const double count = d->per_sample ? (double)d->HW : (double)d->N * (double)d->HW;
+  norm_bwd_params_kernel<<<ceil_div(G, 128), 128, 0, st>>>(sums, nullptr, G, mean_rstd, ggamma_per_group, count);
+  B2_LAUNCH_CHECK();
+  return B200GAN_OK;
 }
