@@ -334,6 +334,21 @@ int b200gan_critic_step_mlp(const b200gan_mlp_critic_desc *d, float lambda_gp, c
                             const float *alpha, const float *W1, const float *b1, const float *W2, const float *b2,
                             const float *W3, const float *b3, float *losses, float *dW1, float *db1, float *dW2,
                             float *db2, float *dW3, float *db3, float *workspace, void *stream);
+/* The vanilla GAN discriminator (gan.py:64-80, bgan.py:66-80, aae.py:90-104): the same critic followed by a Sigmoid,
+ *   y[n] = 1 / (1 + exp(-(a2[n] . W3 + b3))),
+ * on the same two kernels as b200gan_mlp_critic_fwd / _bwd (one cooperative launch each).  The forward writes y[N] in
+ * place of out and keeps m1, a1, m2, a2 as the critic forward does.  The backward first forms the gradient at the
+ * logits, g[n] = dout[n] y[n] (1 - y[n]) (torch's sigmoid backward), then runs the critic backward for g; its outputs
+ * and their NULL rules are those of b200gan_mlp_critic_bwd.  workspace: b200gan_mlp_disc_bwd_workspace_floats()
+ * floats (U1, U2 and g). */
+int b200gan_mlp_disc_fwd(const b200gan_mlp_critic_desc *d, const float *x, const float *W1, const float *b1,
+                         const float *W2, const float *b2, const float *W3, const float *b3, float *y, float *m1,
+                         float *a1, float *m2, float *a2, void *stream);
+size_t b200gan_mlp_disc_bwd_workspace_floats(const b200gan_mlp_critic_desc *d);
+int b200gan_mlp_disc_bwd(const b200gan_mlp_critic_desc *d, const float *dout, const float *y, const float *x,
+                         const float *W1, const float *W2, const float *W3, const float *m1, const float *a1,
+                         const float *m2, const float *a2, float *dx, float *dW1, float *db1, float *dW2, float *db2,
+                         float *dW3, float *db3, float *workspace, void *stream);
 
 /* ---- MLP generator: forward and backward (csrc/mlp_generator/mlp_generator.cu) ------------------------------------ */
 /* The MLP generator of wgan_gp.py:42-65 / gan.py:38-61 (Linear weights W[l][width[l+1]][width[l]], biases b[l]):

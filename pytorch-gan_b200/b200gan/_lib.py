@@ -117,6 +117,9 @@ SIGNATURES = {
     "b200gan_mlp_critic_dbwd": (c_i32, [_P(MlpCriticDesc)] + [c_vp] * 15),
     "b200gan_critic_step_workspace_floats": (c_sz, [_P(MlpCriticDesc)]),
     "b200gan_critic_step_mlp": (c_i32, [_P(MlpCriticDesc), c_f32] + [c_vp] * 18),
+    "b200gan_mlp_disc_fwd": (c_i32, [_P(MlpCriticDesc)] + [c_vp] * 13),
+    "b200gan_mlp_disc_bwd_workspace_floats": (c_sz, [_P(MlpCriticDesc)]),
+    "b200gan_mlp_disc_bwd": (c_i32, [_P(MlpCriticDesc)] + [c_vp] * 19),
     "b200gan_mlp_gen_saved_floats": (c_sz, [_P(MlpGenDesc)]),
     "b200gan_mlp_gen_workspace_floats": (c_sz, [_P(MlpGenDesc)]),
     "b200gan_mlp_gen_fwd": (c_i32, [_P(MlpGenDesc)] + [c_vp] * 5),

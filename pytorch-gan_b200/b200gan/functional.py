@@ -950,6 +950,45 @@ def mlp_critic(x, l1, l2, l3, slope):
     return MlpCriticFn.apply(x, l1.weight, l1.bias, l2.weight, l2.bias, l3.weight, l3.bias, float(slope))
 
 
+# ---- the vanilla GAN discriminator: the MLP critic -> Sigmoid (csrc/mlp_critic.cu) ---------------------------------
+class MlpDiscriminatorFn(torch.autograd.Function):
+    """sigmoid(D(x)), D the MLP critic above (gan.py:64-80, bgan.py:66-80, aae.py:90-104): one launch forward, one
+    launch backward, on the critic kernels in their Sigmoid mode.  A backward under grad mode (autograd.grad(...,
+    create_graph=True): a penalty through the discriminator) recomputes the six modules from the saved inputs with
+    torch ops, so its gradients stay differentiable in every input."""
+
+    @staticmethod
+    def forward(ctx, x, w1, b1, w2, b2, w3, b3, slope):
+        y, m1, a1, m2, a2 = ops.mlp_disc_fwd(x.detach(), *[t.detach() for t in (w1, b1, w2, b2, w3, b3)], slope)
+        ctx.slope = slope
+        ctx.save_for_backward(x, w1, b1, w2, b2, w3, b3, y, m1, a1, m2, a2)
+        return y
+
+    @staticmethod
+    def backward(ctx, dout):
+        x, w1, b1, w2, b2, w3, b3, y, m1, a1, m2, a2 = ctx.saved_tensors
+        need = tuple(ctx.needs_input_grad[:7])
+        if torch.is_grad_enabled():
+            inputs = (x, w1, b1, w2, b2, w3, b3)
+            lrelu = torch.nn.functional.leaky_relu
+            h = lrelu(torch.addmm(b1, x, w1.t()), ctx.slope)
+            h = lrelu(torch.addmm(b2, h, w2.t()), ctx.slope)
+            out = torch.sigmoid(torch.addmm(b3, h, w3.t()))
+            grads = iter(torch.autograd.grad(out, [t for t, n in zip(inputs, need) if n], dout, create_graph=True))
+            return tuple(next(grads) if n else None for n in need) + (None,)
+        grads = ops.mlp_disc_bwd(dout, y, x.detach(), w1.detach(), w2.detach(), w3.detach(), m1, a1, m2, a2, need)
+        return (*grads, None)
+
+
+def mlp_discriminator(x, l1, l2, l3, slope):
+    """Linear l1 -> LeakyReLU(slope) -> Linear l2 -> LeakyReLU(slope) -> Linear l3 (-> 1) -> Sigmoid on x [N, Din] as
+    MlpDiscriminatorFn.  Without autograd (torch.no_grad(), nothing requiring grad) the forward records no node."""
+    params = (l1.weight, l1.bias, l2.weight, l2.bias, l3.weight, l3.bias)
+    if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in params)):
+        return MlpDiscriminatorFn.apply(x, *params, float(slope))
+    return ops.mlp_disc_fwd(x, *[p.detach() for p in params], float(slope))[0]
+
+
 # ---- the MLP generator under autograd (csrc/mlp_generator) --------------------------------------------------------
 class MlpGenSpec:
     """The non-tensor half of a generator call: per layer whether a BatchNorm1d follows its Linear and that norm's

@@ -588,6 +588,23 @@ def mlp_critic_layers(mods, in_features):
     return l1, l2, l3, float(mods[1].negative_slope)
 
 
+def mlp_discriminator_layers(mods, in_features):
+    """(Linear 1, Linear 2, Linear 3, slope) if the module list `mods` is exactly the vanilla GAN discriminator of
+    gan.py:64-80 / bgan.py:66-80 / aae.py:90-104 -- the critic mlp_critic_layers accepts, with a slope >= 0, followed by
+    a Sigmoid -- which runs as functional.MlpDiscriminatorFn; else None.  Stock or drop-in classes only, without hooks.
+    No side effects."""
+    if len(mods) != 6:
+        return None
+    sig = mods[5]
+    if (type(sig) not in (_T["Sigmoid"], REPLACEMENTS["Sigmoid"]) or sig._forward_hooks or sig._forward_pre_hooks
+            or sig._backward_hooks):
+        return None
+    critic = mlp_critic_layers(mods[:5], in_features)
+    if critic is None or critic[3] < 0:
+        return None
+    return critic
+
+
 def mlp_generator_layers(mods, in_features):
     """([(Linear, BatchNorm1d or None)], slope) if the module list `mods` is the MLP generator of wgan_gp.py:42-65 /
     gan.py:38-61 -- [Linear -> (BatchNorm1d)? -> LeakyReLU(s)] x (L - 1), Linear -> Tanh, at most 8 Linears of at most
@@ -706,12 +723,15 @@ class Sequential(_T["Sequential"]):
         return x
 
     def _forward_2d(self, x):
-        """Matrix input: the whole MLP critic (wgan_gp.py:72-78) as one node, or Linear(K, 1) + activation (the adv_layer
-        of a discriminator, dcgan.py:92) as one node."""
+        """Matrix input: the whole MLP critic (wgan_gp.py:72-78), the whole vanilla GAN discriminator (gan.py:64-80), the
+        MLP generator, or Linear(K, 1) + activation (the adv_layer of a discriminator, dcgan.py:92) as one node."""
         mods = list(self._modules.values())
         critic = mlp_critic_layers(mods, x.shape[1])
         if critic is not None and x.shape[0] >= 1:
             return F.mlp_critic(x, *critic)
+        disc = mlp_discriminator_layers(mods, x.shape[1])
+        if disc is not None and x.shape[0] >= 1:
+            return F.mlp_discriminator(x, *disc)
         gen = mlp_generator_layers(mods, x.shape[1])
         # one row with a norm: the stock BatchNorm1d raises torch's own ValueError on the leaf-by-leaf path below
         if gen is not None and (x.shape[0] >= 2 or all(bn is None for _, bn in gen[0])) \

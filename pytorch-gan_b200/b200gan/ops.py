@@ -647,6 +647,42 @@ def mlp_critic_dbwd(u, dout, u1, u2, m1, m2, w1, w2, w3, need):
     return ddout, dw1, dw2, dw3
 
 
+def mlp_disc_fwd(x, w1, b1, w2, b2, w3, b3, slope):
+    """sigmoid(D(x)), the vanilla GAN discriminator, in one launch.  Returns (y [N, 1], m1, a1, m2, a2) as
+    mlp_critic_fwd does (see b200gan_mlp_disc_fwd in include/b200gan.h)."""
+    x, w1, b1, w2, b2, w3, b3 = _f32("mlp_disc operand", x, w1, b1, w2, b2, w3, b3)
+    d = _mlp_critic_desc(x, w1, w2, w3, slope)
+    if b1.numel() != d.H1 or b2.numel() != d.H2 or b3.numel() != 1:
+        raise RuntimeError("b200gan mlp_disc: bias sizes do not match the layers")
+    dev, n = x.device, d.N
+    y = torch.empty((n, 1), device=dev, dtype=torch.float32)
+    m1, a1 = (torch.empty((n, d.H1), device=dev, dtype=torch.float32) for _ in range(2))
+    m2, a2 = (torch.empty((n, d.H2), device=dev, dtype=torch.float32) for _ in range(2))
+    _lib.check(_lib.load().b200gan_mlp_disc_fwd(ctypes.byref(d), x.data_ptr(), w1.data_ptr(), b1.data_ptr(),
+                                                w2.data_ptr(), b2.data_ptr(), w3.data_ptr(), b3.data_ptr(), y.data_ptr(),
+                                                m1.data_ptr(), a1.data_ptr(), m2.data_ptr(), a2.data_ptr(), _stream()),
+               "mlp_disc_fwd")
+    return y, m1, a1, m2, a2
+
+
+def mlp_disc_bwd(dout, y, x, w1, w2, w3, m1, a1, m2, a2, need):
+    """Backward of mlp_disc_fwd for the output gradient dout [N, 1], y its output.  need: 7 flags for the gradients of
+    (x, W1, b1, W2, b2, W3, b3); the others come back as None."""
+    dout, y, x, w1, w2, w3, m1, a1, m2, a2 = _f32("mlp_disc operand", dout, y, x, w1, w2, w3, m1, a1, m2, a2)
+    d = _mlp_critic_desc(x, w1, w2, w3, 0.0)  # the masks carry the slope
+    if dout.numel() != d.N or y.numel() != d.N or m1.shape != (d.N, d.H1) or m2.shape != (d.N, d.H2):
+        raise RuntimeError("b200gan mlp_disc_bwd: dout / saved activations do not match the layers")
+    lib, dev, f32 = _lib.load(), x.device, torch.float32
+    shapes = ((d.N, d.Din), tuple(w1.shape), (d.H1,), tuple(w2.shape), (d.H2,), tuple(w3.shape), (1,))
+    grads = [torch.empty(s_, device=dev, dtype=f32) if nd else None for s_, nd in zip(shapes, need)]
+    ws = torch.empty(lib.b200gan_mlp_disc_bwd_workspace_floats(ctypes.byref(d)), device=dev, dtype=f32)
+    _lib.check(lib.b200gan_mlp_disc_bwd(ctypes.byref(d), dout.data_ptr(), y.data_ptr(), x.data_ptr(), w1.data_ptr(),
+                                        w2.data_ptr(), w3.data_ptr(), m1.data_ptr(), a1.data_ptr(), m2.data_ptr(),
+                                        a2.data_ptr(), *[_ptr(g) for g in grads], ws.data_ptr(), _stream()),
+               "mlp_disc_bwd")
+    return tuple(grads)
+
+
 def critic_step_mlp(real, fake, alpha, w1, b1, w2, b2, w3, b3, slope, lambda_gp):
     """wgan_gp.py:164-173 for the MLP critic in one kernel.  Returns (losses[2], dW1, db1, dW2, db2, dW3, db3)."""
     real, fake, alpha, w1, b1, w2, b2, w3, b3 = _f32("critic_step operand", real, fake, alpha, w1, b1, w2, b2, w3, b3)

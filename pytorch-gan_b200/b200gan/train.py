@@ -91,6 +91,29 @@ def dcgan_step(generator, discriminator, opt_g, opt_d, real_imgs, z, loss=None, 
     return g_loss.detach(), d_loss.detach(), gen_imgs.detach()
 
 
+def gan_step(generator, discriminator, opt_g, opt_d, real_imgs, z, loss=None):
+    """implementations/gan/gan.py:124-161, the vanilla MLP GAN: on the drop-in modules the generator runs on the fused
+    MLP generator kernels and each discriminator pass on the critic kernels' Sigmoid mode (functional.MlpGeneratorFn,
+    functional.MlpDiscriminatorFn).  D is frozen during the G step, as in dcgan_step."""
+    loss = loss or torch.nn.BCELoss()
+    n = real_imgs.shape[0]
+    valid = torch.ones(n, 1, device=real_imgs.device)           # :125
+    fake = torch.zeros(n, 1, device=real_imgs.device)           # :126
+    opt_g.zero_grad()                                           # :135
+    gen_imgs = generator(z)                                     # :141
+    with frozen(discriminator):
+        g_loss = loss(discriminator(gen_imgs), valid)           # :144
+        g_loss.backward()                                       # :146
+    opt_g.step()                                                # :147
+    opt_d.zero_grad()                                           # :153
+    real_loss = loss(discriminator(real_imgs), valid)           # :156
+    fake_loss = loss(discriminator(gen_imgs.detach()), fake)    # :157
+    d_loss = (real_loss + fake_loss) / 2                        # :158
+    d_loss.backward()                                           # :160
+    opt_d.step()                                                # :161
+    return g_loss.detach(), d_loss.detach(), gen_imgs.detach()
+
+
 def wgan_gp_critic_step(generator, discriminator, opt_d, real_imgs, z, alpha, lambda_gp=10.0, fused_gp=True,
                         reduce_d=None):
     """One critic iteration of implementations/wgan_gp/wgan_gp.py:155-174.  `alpha` [N,1,1,1] is the

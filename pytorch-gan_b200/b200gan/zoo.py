@@ -130,6 +130,23 @@ class WGANGPDiscriminator(tnn.Module):
         return self.model(img.view(img.shape[0], -1))
 
 
+class GANDiscriminator(tnn.Module):
+    """gan/gan.py:64-80 (bgan/bgan.py:66-80 is the same module).  gan.py's generator (gan.py:38-61) is WGANGPGenerator at
+    img_shape (1, 28, 28)."""
+
+    def __init__(self, img_shape=(1, 28, 28), nn=None):
+        super().__init__()
+        nn = nn or namespace()
+        n_in = 1
+        for v in img_shape:
+            n_in *= v
+        self.model = nn.Sequential(nn.Linear(n_in, 512), nn.LeakyReLU(0.2, inplace=True), nn.Linear(512, 256),
+                                   nn.LeakyReLU(0.2, inplace=True), nn.Linear(256, 1), nn.Sigmoid())
+
+    def forward(self, img):
+        return self.model(img.view(img.shape[0], -1))
+
+
 # ------------------------------------------------------------------------------------------------
 # Pix2Pix (BASELINE config 3): pix2pix/models.py:20-133
 # ------------------------------------------------------------------------------------------------

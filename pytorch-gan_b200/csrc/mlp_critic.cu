@@ -15,6 +15,10 @@
 // dependent phases are separated by grid.sync(); every phase spreads 32x32 fp32 FFMA output tiles (tile_gemm.cuh)
 // over the grid.  Column sums run one thread per column in a fixed order: the results are deterministic.
 // critic_step_kernel (below) is the whole WGAN-GP critic iteration, penalty included, in one such launch.
+// The vanilla GAN's discriminator (gan.py:64-80, bgan.py:66-80, aae.py:90-104) is the same critic followed by a Sigmoid:
+// a run-time mode of the forward and backward kernels (b200gan_mlp_disc_*), off for the critic entry points.
+//   forward        y = 1 / (1 + exp(-out))
+//   backward       g = dout * y * (1 - y) (torch's sigmoid backward), then the critic backward above with dout := g
 #include "common.cuh"
 #include "tile_gemm.cuh"
 #include <cooperative_groups.h>
@@ -26,6 +30,7 @@ namespace b200gan {
 struct McFwdP {
   int N, Din, H1, H2;
   float slope;
+  int sigmoid;  // out = sigmoid(W3 a2 + b3)
   const float *x, *W1, *b1, *W2, *b2, *W3, *b3;
   float *out, *m1, *a1, *m2, *a2;
 };
@@ -34,6 +39,8 @@ struct McBwdP {
   int N, Din, H1, H2;
   const float *dout, *x, *W1, *W2, *W3, *m1, *a1, *m2, *a2;
   float *dx, *dW1, *db1, *dW2, *db2, *dW3, *db3, *U1, *U2;
+  const float *y;  // non-NULL: the Sigmoid mode; y is the forward's output, g [N] the gradient at the logits
+  float *g;
 };
 
 struct McDbwdP {
@@ -42,15 +49,19 @@ struct McDbwdP {
   float *dW1, *dW2, *dW3, *ddout, *t, *s;
 };
 
-// out[r] = sum_c A[r][c] * w[c] (+ bias), one warp per row
-__device__ __forceinline__ void row_dots(const float *A, const float *w, const float *bias, float *out, int R, int C) {
+// out[r] = sum_c A[r][c] * w[c] (+ bias), one warp per row; sigmoid of that when sig
+__device__ __forceinline__ void row_dots(const float *A, const float *w, const float *bias, float *out, int R, int C,
+                                         int sig = 0) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   for (int r = blockIdx.x * 8 + warp; r < R; r += gridDim.x * 8) {
     float s = 0.f;
     for (int c = lane; c < C; c += 32) s = fmaf(A[(size_t)r * C + c], w[c], s);
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    if (lane == 0) out[r] = bias ? s + bias[0] : s;
+    if (lane == 0) {
+      const float v = bias ? s + bias[0] : s;
+      out[r] = sig ? 1.f / (1.f + expf(-v)) : v;
+    }
   }
 }
 
@@ -89,8 +100,8 @@ __global__ void __launch_bounds__(256) mlp_critic_fwd_kernel(McFwdP p) {
   // P2: h2 = a1 W2^T + b2
   lrelu_layer(p.a1, p.W2, p.b2, p.slope, p.m2, p.a2, p.N, p.H1, p.H2, As, Bs);
   grid.sync();
-  // P3: out = a2 W3^T + b3
-  row_dots(p.a2, p.W3, p.b3, p.out, p.N, p.H2);
+  // P3: out = a2 W3^T + b3 (or its sigmoid)
+  row_dots(p.a2, p.W3, p.b3, p.out, p.N, p.H2, p.sigmoid);
 }
 
 __global__ void __launch_bounds__(256) mlp_critic_bwd_kernel(McBwdP p) {
@@ -100,15 +111,21 @@ __global__ void __launch_bounds__(256) mlp_critic_bwd_kernel(McBwdP p) {
   const int N = p.N, Din = p.Din, H1 = p.H1, H2 = p.H2;
   const int nb = gridDim.x, bid = blockIdx.x;
   const int64_t gtid = (int64_t)bid * blockDim.x + threadIdx.x, gthreads = (int64_t)nb * blockDim.x;
+  // P0 (Sigmoid mode): g = dout * y * (1 - y), the gradient at the logits, which P1-P3 read in place of dout
+  if (p.y) {
+    for (int64_t i = gtid; i < N; i += gthreads) p.g[i] = p.dout[i] * p.y[i] * (1.f - p.y[i]);
+    grid.sync();
+  }
+  const float *dout = p.y ? p.g : p.dout;
   // P1: U2 = dout W3 * m2;  dW3 = dout^T a2;  db3 = sum dout
   for (int64_t i = gtid; i < (int64_t)N * H2; i += gthreads) {
     const int n = (int)(i / H2), j = (int)(i % H2);
-    p.U2[i] = p.dout[n] * p.W3[j] * p.m2[i];
+    p.U2[i] = dout[n] * p.W3[j] * p.m2[i];
   }
-  if (p.dW3) col_sums(p.a2, p.dout, p.dW3, N, H2);
+  if (p.dW3) col_sums(p.a2, dout, p.dW3, N, H2);
   if (p.db3 && gtid == 0) {
     float s = 0.f;
-    for (int n = 0; n < N; ++n) s += p.dout[n];
+    for (int n = 0; n < N; ++n) s += dout[n];
     p.db3[0] = s;
   }
   grid.sync();
@@ -341,6 +358,41 @@ static bool dims_ok(const b200gan_mlp_critic_desc *d) {
   return d->N > 0 && d->Din > 0 && d->H1 > 0 && d->H2 > 0;
 }
 
+static int critic_fwd(const b200gan_mlp_critic_desc *d, const float *x, const float *W1, const float *b1,
+                      const float *W2, const float *b2, const float *W3, const float *b3, float *out, float *m1,
+                      float *a1, float *m2, float *a2, int sigmoid, void *stream, const char *what) {
+  B2_CHECK_ARG(d && x && W1 && b1 && W2 && b2 && W3 && b3 && out && m1 && a1 && m2 && a2, "%s: null pointer", what);
+  B2_CHECK_ARG(dims_ok(d), "%s: bad dims", what);
+  McFwdP p;
+  p.N = d->N; p.Din = d->Din; p.H1 = d->H1; p.H2 = d->H2; p.slope = d->slope; p.sigmoid = sigmoid;
+  p.x = x; p.W1 = W1; p.b1 = b1; p.W2 = W2; p.b2 = b2; p.W3 = W3; p.b3 = b3;
+  p.out = out; p.m1 = m1; p.a1 = a1; p.m2 = m2; p.a2 = a2;
+  return launch_coop(mlp_critic_fwd_kernel, p, stream, what);
+}
+
+// y == NULL: the critic backward for dout; else the Sigmoid mode, g in the workspace after U1 and U2
+static int critic_bwd(const b200gan_mlp_critic_desc *d, const float *dout, const float *y, const float *x,
+                      const float *W1, const float *W2, const float *W3, const float *m1, const float *a1,
+                      const float *m2, const float *a2, float *dx, float *dW1, float *db1, float *dW2, float *db2,
+                      float *dW3, float *db3, float *U1, float *U2, float *workspace, void *stream, const char *what) {
+  B2_CHECK_ARG(d && dout && W2 && W3 && m1 && m2, "%s: null pointer", what);
+  B2_CHECK_ARG(dims_ok(d), "%s: bad dims", what);
+  B2_CHECK_ARG(!dx || W1, "%s: dx needs W1", what);
+  B2_CHECK_ARG(!dW1 || x, "%s: dW1 needs x", what);
+  B2_CHECK_ARG(!dW2 || a1, "%s: dW2 needs a1", what);
+  B2_CHECK_ARG(!dW3 || a2, "%s: dW3 needs a2", what);
+  B2_CHECK_ARG((U1 && U2) || workspace, "%s: U1/U2 need a workspace when not requested", what);
+  McBwdP p;
+  p.N = d->N; p.Din = d->Din; p.H1 = d->H1; p.H2 = d->H2;
+  p.dout = dout; p.x = x; p.W1 = W1; p.W2 = W2; p.W3 = W3; p.m1 = m1; p.a1 = a1; p.m2 = m2; p.a2 = a2;
+  p.dx = dx; p.dW1 = dW1; p.db1 = db1; p.dW2 = dW2; p.db2 = db2; p.dW3 = dW3; p.db3 = db3;
+  p.U1 = U1 ? U1 : workspace;
+  p.U2 = U2 ? U2 : workspace + (size_t)d->N * d->H1;
+  p.y = y;
+  p.g = y ? workspace + (size_t)d->N * ((size_t)d->H1 + d->H2) : nullptr;
+  return launch_coop(mlp_critic_bwd_kernel, p, stream, what);
+}
+
 }  // namespace b200gan
 
 using namespace b200gan;
@@ -349,14 +401,7 @@ extern "C" int b200gan_mlp_critic_fwd(const b200gan_mlp_critic_desc *d, const fl
                                       const float *b1, const float *W2, const float *b2, const float *W3,
                                       const float *b3, float *out, float *m1, float *a1, float *m2, float *a2,
                                       void *stream) {
-  B2_CHECK_ARG(d && x && W1 && b1 && W2 && b2 && W3 && b3 && out && m1 && a1 && m2 && a2,
-               "mlp_critic_fwd: null pointer");
-  B2_CHECK_ARG(dims_ok(d), "mlp_critic_fwd: bad dims");
-  McFwdP p;
-  p.N = d->N; p.Din = d->Din; p.H1 = d->H1; p.H2 = d->H2; p.slope = d->slope;
-  p.x = x; p.W1 = W1; p.b1 = b1; p.W2 = W2; p.b2 = b2; p.W3 = W3; p.b3 = b3;
-  p.out = out; p.m1 = m1; p.a1 = a1; p.m2 = m2; p.a2 = a2;
-  return launch_coop(mlp_critic_fwd_kernel, p, stream, "mlp_critic_fwd");
+  return critic_fwd(d, x, W1, b1, W2, b2, W3, b3, out, m1, a1, m2, a2, 0, stream, "mlp_critic_fwd");
 }
 
 extern "C" size_t b200gan_mlp_critic_bwd_workspace_floats(const b200gan_mlp_critic_desc *d) {
@@ -369,20 +414,8 @@ extern "C" int b200gan_mlp_critic_bwd(const b200gan_mlp_critic_desc *d, const fl
                                       const float *a1, const float *m2, const float *a2, float *dx, float *dW1,
                                       float *db1, float *dW2, float *db2, float *dW3, float *db3, float *U1, float *U2,
                                       float *workspace, void *stream) {
-  B2_CHECK_ARG(d && dout && W2 && W3 && m1 && m2, "mlp_critic_bwd: null pointer");
-  B2_CHECK_ARG(dims_ok(d), "mlp_critic_bwd: bad dims");
-  B2_CHECK_ARG(!dx || W1, "mlp_critic_bwd: dx needs W1");
-  B2_CHECK_ARG(!dW1 || x, "mlp_critic_bwd: dW1 needs x");
-  B2_CHECK_ARG(!dW2 || a1, "mlp_critic_bwd: dW2 needs a1");
-  B2_CHECK_ARG(!dW3 || a2, "mlp_critic_bwd: dW3 needs a2");
-  B2_CHECK_ARG((U1 && U2) || workspace, "mlp_critic_bwd: U1/U2 need a workspace when not requested");
-  McBwdP p;
-  p.N = d->N; p.Din = d->Din; p.H1 = d->H1; p.H2 = d->H2;
-  p.dout = dout; p.x = x; p.W1 = W1; p.W2 = W2; p.W3 = W3; p.m1 = m1; p.a1 = a1; p.m2 = m2; p.a2 = a2;
-  p.dx = dx; p.dW1 = dW1; p.db1 = db1; p.dW2 = dW2; p.db2 = db2; p.dW3 = dW3; p.db3 = db3;
-  p.U1 = U1 ? U1 : workspace;
-  p.U2 = U2 ? U2 : workspace + (size_t)d->N * d->H1;
-  return launch_coop(mlp_critic_bwd_kernel, p, stream, "mlp_critic_bwd");
+  return critic_bwd(d, dout, nullptr, x, W1, W2, W3, m1, a1, m2, a2, dx, dW1, db1, dW2, db2, dW3, db3, U1, U2,
+                    workspace, stream, "mlp_critic_bwd");
 }
 
 extern "C" size_t b200gan_mlp_critic_dbwd_workspace_floats(const b200gan_mlp_critic_desc *d) {
@@ -404,6 +437,27 @@ extern "C" int b200gan_mlp_critic_dbwd(const b200gan_mlp_critic_desc *d, const f
   p.t = workspace;
   p.s = workspace + (size_t)d->N * d->H1;
   return launch_coop(mlp_critic_dbwd_kernel, p, stream, "mlp_critic_dbwd");
+}
+
+extern "C" int b200gan_mlp_disc_fwd(const b200gan_mlp_critic_desc *d, const float *x, const float *W1, const float *b1,
+                                    const float *W2, const float *b2, const float *W3, const float *b3, float *y,
+                                    float *m1, float *a1, float *m2, float *a2, void *stream) {
+  return critic_fwd(d, x, W1, b1, W2, b2, W3, b3, y, m1, a1, m2, a2, 1, stream, "mlp_disc_fwd");
+}
+
+extern "C" size_t b200gan_mlp_disc_bwd_workspace_floats(const b200gan_mlp_critic_desc *d) {
+  if (!d) return 0;
+  return (size_t)d->N * ((size_t)d->H1 + d->H2 + 1);
+}
+
+extern "C" int b200gan_mlp_disc_bwd(const b200gan_mlp_critic_desc *d, const float *dout, const float *y,
+                                    const float *x, const float *W1, const float *W2, const float *W3,
+                                    const float *m1, const float *a1, const float *m2, const float *a2, float *dx,
+                                    float *dW1, float *db1, float *dW2, float *db2, float *dW3, float *db3,
+                                    float *workspace, void *stream) {
+  B2_CHECK_ARG(y && workspace, "mlp_disc_bwd: null pointer");
+  return critic_bwd(d, dout, y, x, W1, W2, W3, m1, a1, m2, a2, dx, dW1, db1, dW2, db2, dW3, db3, nullptr, nullptr,
+                    workspace, stream, "mlp_disc_bwd");
 }
 
 extern "C" size_t b200gan_critic_step_workspace_floats(const b200gan_mlp_critic_desc *d) {
