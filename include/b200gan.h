@@ -469,6 +469,33 @@ int b200gan_linear1_bwd(const float *x, const float *w, const float *y, const fl
 int b200gan_bce_fwd(const float *v, const float *t, float *loss, int64_t n, void *stream);
 int b200gan_bce_bwd(const float *v, const float *t, const float *gout, float *dv, int64_t n, void *stream);
 
+/* ---- MSELoss / L1Loss, reduction 'mean' (csrc/pixel_loss/) --------------------------------------------------------- */
+/* torch.nn.MSELoss() / torch.nn.L1Loss() of an input a and a target b of one logical shape [N][C][H][W] (fewer
+ * dimensions padded with leading 1s): the adversarial loss of LSGAN, Pix2Pix and CycleGAN (lsgan.py:102, pix2pix.py:50,
+ * cyclegan.py:50) and the pixel, cycle and identity losses of the image translators (pix2pix.py:51, cyclegan.py:51-52).
+ * Each operand is dense in its own layout: NCHW-contiguous, or channels_last (NHWC, 4-D only).  0 < n < 2^31. */
+enum { B200GAN_PIXEL_LOSS_MSE = 0, B200GAN_PIXEL_LOSS_L1 = 1 };
+enum { B200GAN_LAYOUT_NCHW = 0, B200GAN_LAYOUT_NHWC = 1 };
+typedef struct b200gan_pixel_loss_desc {
+  int32_t mode;                 /* B200GAN_PIXEL_LOSS_*                          */
+  int32_t layout_a, layout_b;   /* B200GAN_LAYOUT_* of the input and the target  */
+  int32_t reserved;
+  int64_t n;                    /* N * C * H * W                                 */
+  int32_t N, C, H, W;           /* logical shape, padded to 4-D                  */
+} b200gan_pixel_loss_desc;
+/* Bytes of the forward's workspace (0 for an invalid desc).  It holds a completion ticket that must be zero before the
+ * first call; every call leaves it zero again, so one buffer serves any number of calls (and CUDA-graph replays) issued
+ * in order on one stream. */
+size_t b200gan_pixel_loss_workspace_bytes(const b200gan_pixel_loss_desc *d);
+/* loss[0] = mean over the elements of (a - b)^2 (MSE) or |a - b| (L1), summed in a fixed order (fp32 per thread, fp64
+ * across threads and blocks): bit-identical from call to call on one device.  ONE launch.  workspace: 16-byte aligned. */
+int b200gan_pixel_loss_fwd(const b200gan_pixel_loss_desc *d, const float *a, const float *b, float *loss,
+                           void *workspace, void *stream);
+/* Given gout[0] = dL/dloss (read on the device): da = 2 (a - b) gout / n (MSE) or sign(a - b) gout / n (L1, sign(0) =
+ * 0) in a's layout, and db = -da in b's layout when db is not NULL.  ONE launch; da and db are OVERWRITTEN. */
+int b200gan_pixel_loss_bwd(const b200gan_pixel_loss_desc *d, const float *a, const float *b, const float *gout,
+                           float *da, float *db, void *stream);
+
 /* ---- Adam (torch.optim.Adam semantics: dcgan.py:134-135) ---------------------------------------------------------- */
 /* p -= lr * mhat / (sqrt(vhat) + eps), bias-corrected with the step count read from the device.  lr, betas and eps are
  * doubles like torch's Python-side hyper-parameters: torch forms 1 - beta, 1 - beta^t and lr / (1 - beta1^t) in double

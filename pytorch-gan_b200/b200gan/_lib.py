@@ -69,6 +69,15 @@ class TailDesc(ctypes.Structure):
                 ("slope", c_f32), ("act_out", c_i32)]
 
 
+PIXEL_LOSS_MSE, PIXEL_LOSS_L1 = 0, 1
+LAYOUT_NCHW, LAYOUT_NHWC = 0, 1
+
+
+class PixelLossDesc(ctypes.Structure):
+    _fields_ = [("mode", c_i32), ("layout_a", c_i32), ("layout_b", c_i32), ("reserved", c_i32), ("n", c_i64),
+                ("N", c_i32), ("C", c_i32), ("H", c_i32), ("W", c_i32)]
+
+
 class AdamTensor(ctypes.Structure):
     _fields_ = [("p", c_vp), ("g", c_vp), ("m", c_vp), ("v", c_vp), ("n", c_i64)]
 
@@ -138,6 +147,9 @@ SIGNATURES = {
     "b200gan_linear1_bwd": (c_i32, [c_vp] * 7 + [c_i32, c_i32, c_i32, c_vp]),
     "b200gan_bce_fwd": (c_i32, [c_vp, c_vp, c_vp, c_i64, c_vp]),
     "b200gan_bce_bwd": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
+    "b200gan_pixel_loss_workspace_bytes": (c_sz, [_P(PixelLossDesc)]),
+    "b200gan_pixel_loss_fwd": (c_i32, [_P(PixelLossDesc), c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "b200gan_pixel_loss_bwd": (c_i32, [_P(PixelLossDesc), c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "b200gan_adam_multi": (c_i32, [_P(AdamTensor), c_i32, c_f64, c_f64, c_f64, c_f64, c_f32, c_vp, c_vp]),
 }
 

@@ -14,7 +14,7 @@ import torch
 from . import ops
 from ._lib import ConvGeom
 from ._lib import (ACT_LRELU, ACT_NONE, ACT_RELU, ACT_SIGMOID, ACT_TANH, ALGO_SIMT,  # noqa: F401 (re-exported)
-                   PACK_SIMT_DGRAD, PACK_SIMT_FPROP, PAD_ZERO)
+                   PACK_SIMT_DGRAD, PACK_SIMT_FPROP, PAD_ZERO, PIXEL_LOSS_MSE)
 
 
 @dataclass(frozen=True)
@@ -847,6 +847,34 @@ class BCEMeanFn(torch.autograd.Function):
     def backward(ctx, gout):
         v, t = ctx.saved_tensors
         return ops.bce_bwd(v, t, gout.contiguous()), None
+
+
+class PixelLossFn(torch.autograd.Function):
+    """torch.nn.MSELoss() / torch.nn.L1Loss() (reduction 'mean') forward and backward as one kernel each
+    (csrc/pixel_loss/): the adversarial, pixel, cycle and identity losses of the image translators
+    (pix2pix.py:50-51, cyclegan.py:50-52).  Either gradient is optional."""
+
+    @staticmethod
+    def forward(ctx, input, target, mode):
+        ctx.mode = mode
+        ctx.save_for_backward(input, target)
+        return ops.pixel_loss_fwd(input.detach(), target.detach(), mode)
+
+    @staticmethod
+    def backward(ctx, gout):
+        a, b = ctx.saved_tensors
+        need_a, need_b = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+        if not (need_a or need_b):
+            return None, None, None
+        if torch.is_grad_enabled():  # create_graph=True: stay differentiable (plain torch ops on the saved tensors)
+            diff = a - b
+            if ctx.mode == PIXEL_LOSS_MSE:
+                d = diff * (gout * (2.0 / a.numel()))
+            else:
+                d = torch.sign(diff) * (gout / a.numel())
+            return (d if need_a else None), (-d if need_b else None), None
+        da, db = ops.pixel_loss_bwd(a, b, gout.detach().contiguous(), ctx.mode, need_b)
+        return (da if need_a else None), db, None
 
 
 def conv_block(x, weight, bias, chan_scale, spec, cache):

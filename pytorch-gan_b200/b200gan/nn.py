@@ -15,14 +15,15 @@ import torch.nn as tnn
 from . import _lib
 from . import functional as F
 from . import ops
-from ._lib import (ACT_LRELU, ACT_NONE, ACT_RELU, ACT_SIGMOID, ACT_TANH, PAD_REFLECT, PAD_ZERO)
+from ._lib import (ACT_LRELU, ACT_NONE, ACT_RELU, ACT_SIGMOID, ACT_TANH, PAD_REFLECT, PAD_ZERO, PIXEL_LOSS_L1,
+                   PIXEL_LOSS_MSE)
 from .functional import ConvSpec, NormSpec, PackCache
 
 _T = {  # the stock classes, captured before any patching
     n: getattr(tnn, n) for n in (
         "Conv2d", "ConvTranspose2d", "BatchNorm2d", "InstanceNorm2d", "LeakyReLU", "ReLU", "Tanh", "Sigmoid",
         "Upsample", "ZeroPad2d", "ReflectionPad2d", "Dropout", "Dropout2d", "Sequential", "Linear", "BCELoss",
-        "BatchNorm1d")
+        "BatchNorm1d", "MSELoss", "L1Loss")
 }
 
 
@@ -309,6 +310,38 @@ class BCELoss(_T["BCELoss"]):
         if (input.is_cuda and input.dtype == torch.float32 and self.reduction == "mean" and self.weight is None
                 and target.shape == input.shape and target.dtype == torch.float32 and not target.requires_grad):
             return F.BCEMeanFn.apply(input, target)
+        return super().forward(input, target)
+
+
+def pixel_loss_routed(input, target, reduction):
+    """True if MSELoss / L1Loss(input, target) runs on the pixel-loss kernels (functional.PixelLossFn): two CUDA fp32
+    tensors of one shape (no broadcasting) on one device, each NCHW- or channels_last-contiguous, at most 4-D, with at
+    least one element, and reduction 'mean'.  Everything else -- including the legacy size_average / reduce arguments,
+    which the stock constructor maps onto `reduction` -- is the stock module.  No side effects."""
+    if reduction != "mean" or not (torch.is_tensor(input) and torch.is_tensor(target)):
+        return False
+    if not (_on_device(input) and _on_device(target) and input.device == target.device):
+        return False
+    if input.dtype != torch.float32 or target.dtype != torch.float32:
+        return False
+    return ops.pixel_loss_desc(input, target, PIXEL_LOSS_MSE) is not None
+
+
+class MSELoss(_T["MSELoss"]):
+    """nn.MSELoss (lsgan.py:102, pix2pix.py:50, cyclegan.py:50); routing: pixel_loss_routed."""
+
+    def forward(self, input, target):
+        if pixel_loss_routed(input, target, self.reduction):
+            return F.PixelLossFn.apply(input, target, PIXEL_LOSS_MSE)
+        return super().forward(input, target)
+
+
+class L1Loss(_T["L1Loss"]):
+    """nn.L1Loss (pix2pix.py:51, cyclegan.py:51-52); routing: pixel_loss_routed."""
+
+    def forward(self, input, target):
+        if pixel_loss_routed(input, target, self.reduction):
+            return F.PixelLossFn.apply(input, target, PIXEL_LOSS_L1)
         return super().forward(input, target)
 
 
@@ -844,6 +877,7 @@ REPLACEMENTS = {
     "InstanceNorm2d": InstanceNorm2d, "LeakyReLU": LeakyReLU, "ReLU": ReLU, "Tanh": Tanh, "Sigmoid": Sigmoid,
     "Upsample": Upsample, "ZeroPad2d": ZeroPad2d, "ReflectionPad2d": ReflectionPad2d, "Dropout": Dropout,
     "Dropout2d": Dropout2d, "Sequential": Sequential, "Linear": Linear, "BCELoss": BCELoss, "BatchNorm1d": BatchNorm1d,
+    "MSELoss": MSELoss, "L1Loss": L1Loss,
 }
 for _n, _c in REPLACEMENTS.items():
     _c.__name__ = _n

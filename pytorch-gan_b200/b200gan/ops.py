@@ -12,7 +12,7 @@ import torch
 from . import _lib
 from ._lib import (ACT_NONE, ALGO_AUTO, ALGO_SIMT, ALGO_TC, PACK_SIMT_DGRAD, PACK_SIMT_FPROP, PACK_TC_DGRAD,
                    PACK_TC_DGRAD_UP2, PACK_TC_FPROP, PACK_TC_FPROP_UP2, PAD_REFLECT, PAD_ZERO, ConvGeom, Epilogue,
-                   MlpCriticDesc, MlpGenDesc, MlpGenGrads, NbBn, NormDesc, TailDesc)
+                   MlpCriticDesc, MlpGenDesc, MlpGenGrads, NbBn, NormDesc, PixelLossDesc, TailDesc)
 
 CL = torch.channels_last
 
@@ -567,6 +567,76 @@ def bce_bwd(v, t, gout):
     _lib.check(_lib.load().b200gan_bce_bwd(v.data_ptr(), t.data_ptr(), gout.data_ptr(), dv.data_ptr(), v.numel(),
                                            _stream()), "bce_bwd")
     return dv
+
+
+# ---- MSELoss / L1Loss, reduction 'mean' (csrc/pixel_loss/) --------------------------------------------------------------
+def pixel_layout(t):
+    """_lib.LAYOUT_NCHW for a contiguous tensor, LAYOUT_NHWC for a 4-D channels_last one, else None (not dense in either
+    layout: a strided view, an expanded tensor)."""
+    if t.is_contiguous():
+        return _lib.LAYOUT_NCHW
+    if t.dim() == 4 and t.is_contiguous(memory_format=CL):
+        return _lib.LAYOUT_NHWC
+    return None
+
+
+def pixel_loss_desc(a, b, mode):
+    """The kernel's description of loss(a, b): one shape of at most 4 dimensions (padded with leading 1s), 0 < n < 2^31,
+    each operand in its own layout.  None if the pair is not one the kernels take."""
+    if a.shape != b.shape or a.dim() > 4 or not 0 < a.numel() < 2 ** 31:
+        return None
+    la, lb = pixel_layout(a), pixel_layout(b)
+    if la is None or lb is None:
+        return None
+    d = PixelLossDesc()
+    d.mode, d.layout_a, d.layout_b, d.n = mode, la, lb, a.numel()
+    d.N, d.C, d.H, d.W = (1,) * (4 - a.dim()) + tuple(a.shape)
+    return d
+
+
+_pixel_ws = {}
+
+
+def _pixel_loss_workspace(device, nbytes):
+    """The forward's workspace, zeroed once per device: every call leaves its completion ticket at zero again, so no
+    fill kernel runs per loss.  One buffer per device suffices because loss calls never interleave on the stream."""
+    t = _pixel_ws.get(device)
+    if t is None or t.numel() < nbytes:
+        t = torch.zeros(max(nbytes, 16 + 8 * 1024), device=device, dtype=torch.uint8)
+        _pixel_ws[device] = t
+    return t
+
+
+def _pixel_loss_check(a, b, mode):
+    _require_cuda(a, "loss input")
+    _require_cuda(b, "loss target")
+    d = pixel_loss_desc(a, b, mode)
+    if d is None:
+        raise RuntimeError(f"b200gan: pixel loss of {tuple(a.shape)} / {tuple(b.shape)} tensors: one shape of at most 4 "
+                           "dimensions, each NCHW- or channels_last-contiguous, is required")
+    return d
+
+
+def pixel_loss_fwd(a, b, mode):
+    """mean((a - b)^2) (mode PIXEL_LOSS_MSE) or mean(|a - b|) (PIXEL_LOSS_L1) as a 0-dim fp32 tensor; one launch."""
+    d = _pixel_loss_check(a, b, mode)
+    lib = _lib.load()
+    ws = _pixel_loss_workspace(a.device, lib.b200gan_pixel_loss_workspace_bytes(ctypes.byref(d)))
+    loss = torch.empty((), device=a.device, dtype=torch.float32)
+    _lib.check(lib.b200gan_pixel_loss_fwd(ctypes.byref(d), a.data_ptr(), b.data_ptr(), loss.data_ptr(), ws.data_ptr(),
+                                          _stream()), "pixel_loss_fwd")
+    return loss
+
+
+def pixel_loss_bwd(a, b, gout, mode, need_db):
+    """(da, db) for the upstream gradient gout (0-dim, read on the device): da in a's layout, db = -da in b's layout or
+    None; one launch."""
+    d = _pixel_loss_check(a, b, mode)
+    da = torch.empty_like(a)
+    db = torch.empty_like(b) if need_db else None
+    _lib.check(_lib.load().b200gan_pixel_loss_bwd(ctypes.byref(d), a.data_ptr(), b.data_ptr(), gout.data_ptr(),
+                                                  da.data_ptr(), _ptr(db), _stream()), "pixel_loss_bwd")
+    return da, db
 
 
 # ---- MLP critic under autograd: Linear -> LeakyReLU -> Linear -> LeakyReLU -> Linear(-> 1) (csrc/mlp_critic.cu) ------

@@ -159,10 +159,20 @@ def wgan_gp_generator_step(generator, discriminator, opt_g, z):
     return g_loss.detach()
 
 
+def _pixel_losses(*nets):
+    """(mse, l1) for a translator's step: the drop-in MSELoss / L1Loss (csrc/pixel_loss) when the networks are built from
+    drop-in modules, else torch's own functional losses, so that a stock model keeps every op on stock torch."""
+    from . import nn as bnn
+    dropin = tuple(bnn.REPLACEMENTS.values())
+    if any(isinstance(m, dropin) for net in nets for m in net.modules()):
+        return bnn.MSELoss(), bnn.L1Loss()
+    return torch.nn.functional.mse_loss, torch.nn.functional.l1_loss
+
+
 def pix2pix_step(generator, discriminator, opt_g, opt_d, real_a, real_b, lambda_pixel=100.0, reduce_g=None,
                  reduce_d=None):
     """implementations/pix2pix/pix2pix.py:131-172 (MSE GAN loss :50, L1 pixel loss :51,:54)."""
-    mse, l1 = torch.nn.functional.mse_loss, torch.nn.functional.l1_loss
+    mse, l1 = _pixel_losses(generator, discriminator)
     opt_g.zero_grad()                                          # :138
     fake_b = generator(real_a)                                 # :141
     with frozen(discriminator):
@@ -210,7 +220,7 @@ def cyclegan_step(g_ab, g_ba, d_a, d_b, opt_g, opt_d_a, opt_d_b, real_a, real_b,
                   lambda_cyc=10.0, lambda_id=5.0, reduce_g=None, reduce_d_a=None, reduce_d_b=None):
     """implementations/cyclegan/cyclegan.py:163-241: 6 generator passes + 2 D passes for the G loss, then one
     step per discriminator on (real, replayed fake).  buf_* = ReplayBuffer or None (fakes used directly)."""
-    mse, l1 = torch.nn.functional.mse_loss, torch.nn.functional.l1_loss
+    mse, l1 = _pixel_losses(g_ab, g_ba, d_a, d_b)
     opt_g.zero_grad()                                                          # :177
     loss_identity = (l1(g_ba(real_a), real_a) + l1(g_ab(real_b), real_b)) / 2  # :180-183
     fake_b = g_ab(real_a)                                                      # :186
