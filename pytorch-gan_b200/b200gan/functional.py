@@ -99,6 +99,54 @@ def _as_cl(t):
     return t if ops.is_cl(t) else ops.to_cl(t)
 
 
+def _conv_forward(x, weight, bias, chan_scale, spec: ConvSpec, cache: PackCache):
+    """(geometry, output, fused statistics or None) of the conv block `spec` on the channels_last input x"""
+    g, _ = ops.make_geom(tuple(x.shape), tuple(weight.shape), spec.stride, spec.pads, spec.pad_mode, spec.up,
+                         spec.transposed)
+    algo, kind = ops.conv_plan(g, 0, chan_scale)
+    packed = cache.get(g, weight.detach(), kind)
+    stats = None
+    if spec.stats is not None:
+        stats = ops.zero_scratch(x.device, 2 * (g.N * g.K if spec.stats else g.K))
+    y = ops.conv_fprop(g, x, packed, algo, bias=None if bias is None else bias.detach(), act=spec.act,
+                       slope=spec.slope, chan_scale=chan_scale, stats=stats, stats_per_sample=bool(spec.stats),
+                       round_tf32=spec.rtf_out)
+    return g, y, stats
+
+
+def _with_stats(ctx, y, stats):
+    """The outputs of a node whose conv may also produce the statistics of the norm after it"""
+    if stats is None:
+        return y
+    ctx.mark_non_differentiable(stats)
+    ctx.set_materialize_grads(False)  # no zero-filled gradient is launched for the statistics output
+    return y, stats
+
+
+def _conv_dz(dy, y, chan_scale, spec: ConvSpec):
+    """The gradient w.r.t. the conv's raw output: the backward of its fused activation and Dropout2d scale"""
+    if spec.act != ACT_NONE or chan_scale is not None:
+        return ops.epilogue_bwd(dy, y, chan_scale, spec.act, spec.slope, spec.rtf_dz)
+    return dy
+
+
+def _conv_param_grads(g, x, dz, dy, y, chan_scale, spec: ConvSpec, wshape, need_dw, need_db):
+    """(dw, db) of a conv block from dz = _conv_dz(dy, ...); the bias gradient comes out of the weight-gradient kernel"""
+    db = None
+    if need_db and dz is not dy and spec.rtf_dz:
+        # dz was rounded to TF32 for the tensor-core passes; a bias gradient is a sum with heavy cancellation
+        # and must come from the unrounded values
+        db = ops.bias_grad(dy, y, chan_scale, spec.act, spec.slope)
+        need_db = False
+    dw = None
+    if need_dw or need_db:
+        dw, db2 = ops.conv_wgrad(g, x, dz, wshape, need_db, ops.conv_plan(g, 2)[0])
+        db = db2 if need_db else db
+        if not need_dw:
+            dw = None
+    return dw, db
+
+
 class ConvFn(torch.autograd.Function):
     """[Upsample x2] [pad] Conv2d/ConvTranspose2d [+bias] [act] [* Dropout2d scale] (+ BN/IN partial sums)."""
 
@@ -107,57 +155,31 @@ class ConvFn(torch.autograd.Function):
         ops._require_cuda(x, "conv input")
         ops._require_cuda(weight, "conv weight")
         x = _as_cl(x)
-        g, _ = ops.make_geom(tuple(x.shape), tuple(weight.shape), spec.stride, spec.pads, spec.pad_mode, spec.up,
-                             spec.transposed)
-        algo, kind = ops.conv_plan(g, 0, chan_scale)
-        packed = cache.get(g, weight.detach(), kind)
-        stats = None
-        if spec.stats is not None:
-            stats = ops.zero_scratch(x.device, 2 * (g.N * g.K if spec.stats else g.K))
-        y = ops.conv_fprop(g, x, packed, algo, bias=None if bias is None else bias.detach(), act=spec.act,
-                           slope=spec.slope, chan_scale=chan_scale, stats=stats, stats_per_sample=bool(spec.stats),
-                           round_tf32=spec.rtf_out)
+        g, y, stats = _conv_forward(x, weight, bias, chan_scale, spec, cache)
         ctx.spec, ctx.cache, ctx.g = spec, cache, g
         ctx.has_bias = bias is not None
         need_y = spec.act != ACT_NONE
         ctx.save_for_backward(x, weight, y if need_y else None, chan_scale)
-        if stats is not None:
-            ctx.mark_non_differentiable(stats)
-            ctx.set_materialize_grads(False)  # no zero-filled gradient is launched for the statistics output
-            return y, stats
-        return y
+        return _with_stats(ctx, y, stats)
 
     @staticmethod
     def backward(ctx, dy, *unused):
+        x, weight, y, chan_scale = ctx.saved_tensors
+        spec, g, nig = ctx.spec, ctx.g, ctx.needs_input_grad
         if torch.is_grad_enabled():
             # autograd.grad(..., create_graph=True): the gradient penalty of a conv critic (stargan.py:142-161,
             # dragan.py:144-167) differentiates THROUGH this backward -- build it from differentiable nodes
-            if ctx.spec.up != 1 or ctx.spec.pad_mode != PAD_ZERO:
-                raise NotImplementedError("b200gan: double backward through a conv with a folded upsample / reflection "
-                                          "padding")
-            return _conv_backward_differentiable(ctx, dy) + (None, None, None)
-        x, weight, y, chan_scale = ctx.saved_tensors
-        spec, g = ctx.spec, ctx.g
+            dx, dw, db, _, _ = _conv_backward_differentiable(dy, x, weight, y, chan_scale, spec.act, spec.slope, g,
+                                                             nig[0], nig[1], ctx.has_bias and nig[2])
+            return dx, dw, db, None, None, None
         dy = _as_cl(dy)
-        if spec.act != ACT_NONE or chan_scale is not None:
-            dz = ops.epilogue_bwd(dy, y, chan_scale, spec.act, spec.slope, spec.rtf_dz)
-        else:
-            dz = dy
-        dx = dw = db = None
-        if ctx.needs_input_grad[0]:
+        dz = _conv_dz(dy, y, chan_scale, spec)
+        dx = None
+        if nig[0]:
             algo, kind = ops.conv_plan(g, 1)
             dx = ops.conv_dgrad(g, dz, ctx.cache.get(g, weight.detach(), kind), algo)
-        want_db = ctx.has_bias and ctx.needs_input_grad[2]
-        if want_db and dz is not dy and spec.rtf_dz:
-            # dz was rounded to TF32 for the tensor-core passes; a bias gradient is a sum with heavy cancellation
-            # and must come from the unrounded values
-            db = ops.bias_grad(dy, y, chan_scale, spec.act, spec.slope)
-            want_db = False
-        if ctx.needs_input_grad[1] or want_db:
-            dw, db2 = ops.conv_wgrad(g, x, dz, tuple(weight.shape), want_db, ops.conv_plan(g, 2)[0])
-            db = db2 if want_db else db
-            if not ctx.needs_input_grad[1]:
-                dw = None
+        dw, db = _conv_param_grads(g, x, dz, dy, y, chan_scale, spec, tuple(weight.shape), nig[1],
+                                   ctx.has_bias and nig[2])
         return dx, dw, db, None, None, None
 
 
@@ -215,19 +237,22 @@ class ConvWgradFn(torch.autograd.Function):
         return dx, ddz, None, None, None
 
 
-def _conv_backward_differentiable(ctx, dy):
-    """(dx, dw, db) of a conv block [+bias] [act] [* Dropout2d scale] from differentiable nodes, for a backward under
-    autograd.grad(..., create_graph=True).  ctx: a ConvFn context, which saves (x, weight, y, chan_scale) and has
-    .spec (act, slope), .g and .has_bias."""
-    x, weight, y, chan_scale = ctx.saved_tensors
-    nig = ctx.needs_input_grad
-    return _conv_bwd_nodes(dy, x, weight, y, chan_scale, ctx.spec.act, ctx.spec.slope, ctx.g, nig[0], nig[1],
-                           ctx.has_bias and nig[2])
-
-
-def _conv_bwd_nodes(dy, x, weight, y, chan_scale, act, slope, g, need_dx, need_dw, need_db, simt=False):
-    """_conv_backward_differentiable on explicit operands: x is the conv's input (a differentiable recomputation of it
-    when the conv reads a virtual BatchNorm output); dz is rebuilt from (y, act, slope, chan_scale)."""
+def _conv_backward_differentiable(dy, x, weight, y, chan_scale, act, slope, g, need_dx, need_dw, need_db, norm=None,
+                                  simt=False):
+    """(dx, dw, db, dgamma, dbeta) of a [training-mode norm ->] conv block [+bias] [act] [* Dropout2d scale] from
+    differentiable nodes, for a backward under autograd.grad(..., create_graph=True).  x is the block's input; dz is
+    rebuilt from (y, act, slope, chan_scale).  norm: None, or (gamma, beta, NormSpec, need_params) of the norm between
+    x and the conv, whose output no node kept: it is recomputed from x as a differentiable NormFn output (no
+    running-statistics update) and its backward is NormBwdFn."""
+    if g.up != 1 or g.pad_mode != PAD_ZERO:
+        raise NotImplementedError("b200gan: double backward through a conv with a folded upsample / reflection "
+                                  "padding")
+    xin = x
+    if norm is not None:
+        gamma, beta, nspec, need_params = norm
+        _refuse_second_order_act(nspec.act, "a normalisation")
+        xin, mr, ss = _norm_recompute(x, gamma, beta, nspec)
+        need_dx = need_dx or need_params
     if chan_scale is not None and act in (ACT_TANH, ACT_SIGMOID):
         raise NotImplementedError("b200gan: double backward through Dropout2d fused with tanh / sigmoid")
     dz = dy
@@ -242,9 +267,12 @@ def _conv_bwd_nodes(dy, x, weight, y, chan_scale, act, slope, g, need_dx, need_d
     if chan_scale is not None:
         dz = dz * chan_scale.view(chan_scale.shape[0], chan_scale.shape[1], 1, 1)
     dx = ConvDgradFn.apply(dz, weight, g, simt) if need_dx else None
-    dw = ConvWgradFn.apply(x, dz, g, tuple(weight.shape), simt) if need_dw else None
+    dw = ConvWgradFn.apply(xin, dz, g, tuple(weight.shape), simt) if need_dw else None
     db = dz.sum((0, 2, 3)) if need_db else None
-    return dx, dw, db
+    dgamma = dbeta = None
+    if norm is not None and dx is not None:
+        dx, dgamma, dbeta = NormBwdFn.apply(dx, x, gamma, mr, ss, nspec, need_params)
+    return dx, dw, db, dgamma, dbeta
 
 
 # ---- double backward through training-mode norms (SURVEY.md 8f N2: penalties on normalised conv critics) --------------
@@ -254,11 +282,15 @@ def _refuse_second_order_act(act, what):
                                   "has a second-order term of its own)")
 
 
-def _norm_params_grads(dgb, n, c, per_sample):
-    """(dgamma, dbeta) per channel from the [2][G] per-group output of the norm backward"""
+def _norm_params_grads(dgb, shape, per_sample=False):
+    """(dgamma, dbeta) per channel from the [dgamma; dbeta] per-group output of a norm backward on a tensor of `shape`
+    (None: not computed)"""
+    if dgb is None:
+        return None, None
     groups = dgb.numel() // 2
     dgamma, dbeta = dgb[:groups], dgb[groups:]
     if per_sample:  # affine InstanceNorm2d: parameters are shared across samples
+        n, c = shape[0], shape[1]
         dgamma, dbeta = dgamma.view(n, c).sum(0), dbeta.view(n, c).sum(0)
     return dgamma, dbeta
 
@@ -278,9 +310,7 @@ class NormBwdFn(torch.autograd.Function):
                                     scale_shift)
         ctx.spec, ctx.dy = spec, dy
         ctx.save_for_backward(x, gamma, mean_rstd, scale_shift)
-        if not need_params:
-            return dx, None, None
-        return (dx,) + _norm_params_grads(dgb, x.shape[0], x.shape[1], spec.per_sample)
+        return (dx,) + _norm_params_grads(dgb, x.shape, spec.per_sample)
 
     @staticmethod
     @torch.autograd.function.once_differentiable
@@ -318,6 +348,13 @@ def _bn_consts(a, gamma, beta, eps):
 
 
 
+def _norm_forward(x, gamma, beta, stats, running_mean, running_var, nbt, spec: NormSpec):
+    """(y, mean_rstd, scale_shift) of the training-mode norm `spec` on the channels_last input x"""
+    return ops.norm_forward(x, None if gamma is None else gamma.detach(), None if beta is None else beta.detach(),
+                            running_mean, running_var, nbt, spec.per_sample, spec.eps, spec.momentum, spec.act,
+                            spec.slope, stats, spec.rtf_out, return_scale_shift=True)
+
+
 class NormFn(torch.autograd.Function):
     """Training-mode BatchNorm2d / InstanceNorm2d with an optional fused activation."""
 
@@ -326,10 +363,7 @@ class NormFn(torch.autograd.Function):
         """box: None, or a list that receives (mean_rstd, scale_shift) (_norm_recompute)"""
         ops._require_cuda(x, "norm input")
         x = _as_cl(x)
-        y, mean_rstd, scale_shift = ops.norm_forward(
-            x, None if gamma is None else gamma.detach(), None if beta is None else beta.detach(), running_mean,
-            running_var, nbt, spec.per_sample, spec.eps, spec.momentum, spec.act, spec.slope, stats, spec.rtf_out,
-            return_scale_shift=True)
+        y, mean_rstd, scale_shift = _norm_forward(x, gamma, beta, stats, running_mean, running_var, nbt, spec)
         if box is not None:
             box.append((mean_rstd, scale_shift))
         ctx.spec = spec
@@ -353,10 +387,7 @@ class NormFn(torch.autograd.Function):
         x, dy = x.detach(), _as_cl(dy.detach())
         dx, dgb = ops.norm_backward(dy, x, y, mean_rstd, None if gamma is None else gamma.detach(), spec.per_sample,
                                     spec.eps, spec.act, spec.slope, need_params, spec.rtf_dx, scale_shift)
-        dgamma = dbeta = None
-        if need_params:
-            dgamma, dbeta = _norm_params_grads(dgb, x.shape[0], x.shape[1], spec.per_sample)
-        return dx, dgamma, dbeta, None, None, None, None, None, None
+        return (dx,) + _norm_params_grads(dgb, x.shape, spec.per_sample) + (None,) * 6
 
 
 class NormConvFn(torch.autograd.Function):
@@ -371,57 +402,29 @@ class NormConvFn(torch.autograd.Function):
         ops._require_cuda(x, "norm input")
         ops._require_cuda(weight, "conv weight")
         x = _as_cl(x)
-        a, mean_rstd, scale_shift = ops.norm_forward(
-            x, None if gamma is None else gamma.detach(), None if beta is None else beta.detach(), running_mean,
-            running_var, nbt, False, nspec.eps, nspec.momentum, nspec.act, nspec.slope, stats, nspec.rtf_out,
-            return_scale_shift=True)
-        g, _ = ops.make_geom(tuple(a.shape), tuple(weight.shape), cspec.stride, cspec.pads, cspec.pad_mode, cspec.up)
-        algo, kind = ops.conv_plan(g, 0, chan_scale)
-        packed = cache.get(g, weight.detach(), kind)
-        out_stats = None
-        if cspec.stats is not None:
-            out_stats = ops.zero_scratch(x.device, 2 * (g.N * g.K if cspec.stats else g.K))
-        y = ops.conv_fprop(g, a, packed, algo, bias=None if bias is None else bias.detach(), act=cspec.act,
-                           slope=cspec.slope, chan_scale=chan_scale, stats=out_stats,
-                           stats_per_sample=bool(cspec.stats), round_tf32=cspec.rtf_out)
+        a, mean_rstd, scale_shift = _norm_forward(x, gamma, beta, stats, running_mean, running_var, nbt, nspec)
+        g, y, out_stats = _conv_forward(a, weight, bias, chan_scale, cspec, cache)
         ctx.nspec, ctx.cspec, ctx.cache, ctx.g = nspec, cspec, cache, g
         ctx.has_bias = bias is not None
         # the norm output `a` is the conv's weight-gradient operand; the conv's output is kept only for its activation
         ctx.save_for_backward(x, mean_rstd, scale_shift, gamma, a, weight, y if cspec.act != ACT_NONE else None,
                               chan_scale, beta)
-        if out_stats is not None:
-            ctx.mark_non_differentiable(out_stats)
-            ctx.set_materialize_grads(False)
-            return y, out_stats
-        return y
+        return _with_stats(ctx, y, out_stats)
 
     @staticmethod
     def backward(ctx, dy, *unused):
         x, mean_rstd, scale_shift, gamma, a, weight, y, chan_scale, beta = ctx.saved_tensors
         nspec, cspec, g = ctx.nspec, ctx.cspec, ctx.g
         nig = ctx.needs_input_grad
+        need_params = gamma is not None and (nig[1] or nig[2])
         if torch.is_grad_enabled():
-            # create_graph=True: the norm output recomputed as a differentiable NormFn output (no running-statistics
-            # update), the conv's differentiable backward on it, and the norm's backward as NormBwdFn
-            if cspec.up != 1 or cspec.pad_mode != PAD_ZERO:
-                raise NotImplementedError("b200gan: double backward through a conv with a folded upsample / reflection "
-                                          "padding")
-            _refuse_second_order_act(nspec.act, "a normalisation")
-            need_params = gamma is not None and (nig[1] or nig[2])
-            a, mr, ss = _norm_recompute(x, gamma, beta, nspec)
-            da, dw, db = _conv_bwd_nodes(dy, a, weight, y, chan_scale, cspec.act, cspec.slope, g, nig[0] or need_params,
-                                         nig[7], ctx.has_bias and nig[8])
-            dx = dgamma = dbeta = None
-            if da is not None:
-                dx, dgamma, dbeta = NormBwdFn.apply(da, x, gamma, mr, ss, nspec, need_params)
+            dx, dw, db, dgamma, dbeta = _conv_backward_differentiable(
+                dy, x, weight, y, chan_scale, cspec.act, cspec.slope, g, nig[0], nig[7], ctx.has_bias and nig[8],
+                norm=(gamma, beta, nspec, need_params))
             return dx, dgamma, dbeta, None, None, None, None, dw, db, None, None, None, None
         x, a, y, dy = x.detach(), a.detach(), None if y is None else y.detach(), _as_cl(dy.detach())
-        if cspec.act != ACT_NONE or chan_scale is not None:
-            dz = ops.epilogue_bwd(dy, y, chan_scale, cspec.act, cspec.slope, cspec.rtf_dz)
-        else:
-            dz = dy
-        dx = dgamma = dbeta = dw = db = None
-        need_params = gamma is not None and (nig[1] or nig[2])
+        dz = _conv_dz(dy, y, chan_scale, cspec)
+        dx = dgamma = dbeta = None
         if nig[0] or need_params:
             algo, kind = ops.conv_plan(g, 1)
             da, sums = ops.conv_dgrad_norm(g, dz, ctx.cache.get(g, weight.detach(), kind), x, mean_rstd, scale_shift,
@@ -429,21 +432,11 @@ class NormConvFn(torch.autograd.Function):
             dx, dgb = ops.norm_backward_from_sums(da, x, mean_rstd, None if gamma is None else gamma.detach(), sums,
                                                   nspec.eps, nspec.act, nspec.slope, need_params, nspec.rtf_dx,
                                                   scale_shift)
-            if need_params:
-                c = x.shape[1]
-                dgamma, dbeta = dgb[:c], dgb[c:]
+            dgamma, dbeta = _norm_params_grads(dgb, x.shape)
             if not nig[0]:
                 dx = None
-        want_db = ctx.has_bias and nig[8]
-        if want_db and dz is not dy and cspec.rtf_dz:
-            # as in ConvFn: the bias gradient of a rounded dz comes from the unrounded values
-            db = ops.bias_grad(dy, y, chan_scale, cspec.act, cspec.slope)
-            want_db = False
-        if nig[7] or want_db:
-            dw, db2 = ops.conv_wgrad(g, a, dz, tuple(weight.shape), want_db, ops.conv_plan(g, 2)[0])
-            db = db2 if want_db else db
-            if not nig[7]:
-                dw = None
+        dw, db = _conv_param_grads(g, a, dz, dy, y, chan_scale, cspec, tuple(weight.shape), nig[7],
+                                   ctx.has_bias and nig[8])
         return dx, dgamma, dbeta, None, None, None, None, dw, db, None, None, None, None
 
 
@@ -491,9 +484,7 @@ class TailFn(torch.autograd.Function):
         need_bias = ctx.has_bias and ctx.needs_input_grad[8]
         da, dgb, dw, db = ops.tail_bwd(ctx.d, a, mean_rstd, scale_shift, weight.detach().contiguous(), g, need_affine,
                                        need_bias, spec.rtf_dx)
-        c = a.shape[1]
-        dgamma = dgb[:c] if need_affine else None
-        dbeta = dgb[c:] if need_affine else None
+        dgamma, dbeta = _norm_params_grads(dgb, a.shape)
         return da, None, dgamma, dbeta, None, None, None, dw, db, None
 
 
@@ -632,8 +623,18 @@ def _finish_bn(g, a, edge, sums, need_gamma, need_beta):
     mean_rstd, _ = _bn_consts(a, edge.gamma, edge.beta, edge.eps)
     need = edge.gamma is not None and (need_gamma or need_beta)
     da, dgb = ops.norm_backward_from_sums(g, a, mean_rstd, edge.gamma, sums, edge.eps, need_params=need)
-    c = a.shape[1]
-    return da, (dgb[:c] if need and need_gamma else None), (dgb[c:] if need and need_beta else None)
+    dgamma, dbeta = _norm_params_grads(dgb, a.shape)
+    return da, (dgamma if need_gamma else None), (dbeta if need_beta else None)
+
+
+def _chain_params_grads(sums, groups, c, need_gamma, need_beta):
+    """(dgamma, dbeta) of a chain BatchNorm from the [groups][sum g; sum g * ahat] sums of the backward of its
+    consumer, summed over the statistics groups: beta's gradient is the first half, gamma's the second"""
+    if not (need_gamma or need_beta):
+        return None, None
+    # one conversion kernel for both parameter gradients
+    dgb = sums.float() if groups == 1 else sums.view(groups, 2 * c).sum(0).float()
+    return (dgb[c:] if need_gamma else None), (dgb[:c] if need_beta else None)
 
 
 def _refuse_grouped_chain(groups):
@@ -685,18 +686,12 @@ class NbConvFn(torch.autograd.Function):
             # backward is NormBwdFn.  edge.sums is neither read nor written.
             _refuse_grouped_chain(spec.groups)
             ctx.chain.true_grads = True
-            need_params = in_edge is not None and in_gamma is not None and (nig[4] or nig[5])
-            xin, mr, ss = x, None, None
+            norm = None
             if in_edge is not None:
-                xin, mr, ss = _norm_recompute(x, in_gamma, in_beta, NormSpec(eps=in_edge.eps))
-            dxin, dw, db = _conv_bwd_nodes(gy, xin, weight, y, chan_scale, spec.act, spec.slope, g, nig[0] or need_params,
-                                           nig[1], ctx.has_bias and nig[2],
-                                           simt=in_edge is not None or out_edge is not None)
-            gx = dgamma = dbeta = None
-            if in_edge is None:
-                gx = dxin
-            elif dxin is not None:
-                gx, dgamma, dbeta = NormBwdFn.apply(dxin, x, in_gamma, mr, ss, NormSpec(eps=in_edge.eps), need_params)
+                norm = (in_gamma, in_beta, NormSpec(eps=in_edge.eps), in_gamma is not None and (nig[4] or nig[5]))
+            gx, dw, db, dgamma, dbeta = _conv_backward_differentiable(
+                gy, x, weight, y, chan_scale, spec.act, spec.slope, g, nig[0], nig[1], ctx.has_bias and nig[2],
+                norm=norm, simt=in_edge is not None or out_edge is not None)
             return gx, dw, db, None, dgamma, dbeta, None, None, None, None, None, None, None, None
         true_grads = ctx.chain.true_grads
         if true_grads:
@@ -719,12 +714,8 @@ class NbConvFn(torch.autograd.Function):
                 gx, dgamma, dbeta = _finish_bn(gx, x, in_edge, sums, ctx.needs_input_grad[4], ctx.needs_input_grad[5])
             elif in_edge is not None:
                 in_edge.sums = sums
-                c = g.C
-                if ctx.needs_input_grad[4] or ctx.needs_input_grad[5]:
-                    # one conversion kernel for both parameter gradients (summed over the statistics groups)
-                    dgb = sums.float() if in_edge.groups == 1 else sums.view(in_edge.groups, 2 * c).sum(0).float()
-                    dgamma = dgb[c:] if ctx.needs_input_grad[4] else None
-                    dbeta = dgb[:c] if ctx.needs_input_grad[5] else None
+                dgamma, dbeta = _chain_params_grads(sums, in_edge.groups, g.C, ctx.needs_input_grad[4],
+                                                    ctx.needs_input_grad[5])
         return gx, dw, db, None, dgamma, dbeta, None, None, None, None, None, None, None, None
 
 
@@ -758,13 +749,7 @@ class NbTailFn(torch.autograd.Function):
         if ctx.chain.true_grads:
             return _finish_bn(g, a, ctx.edge, sums, nig[1], nig[2]) + (None,) * 7
         ctx.edge.sums = sums
-        c = a.shape[1]
-        dgamma = dbeta = None
-        if ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
-            grp = ctx.edge.groups
-            dgb = sums.float() if grp == 1 else sums.view(grp, 2 * c).sum(0).float()
-            dgamma = dgb[c:] if ctx.needs_input_grad[1] else None
-            dbeta = dgb[:c] if ctx.needs_input_grad[2] else None
+        dgamma, dbeta = _chain_params_grads(sums, ctx.edge.groups, a.shape[1], nig[1], nig[2])
         return g, dgamma, dbeta, None, None, None, None, None, None, None
 
 

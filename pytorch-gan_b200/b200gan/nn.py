@@ -114,6 +114,14 @@ def _dropout2d_scale(x_shape, p, device):
     return noise.bernoulli_(1.0 - p).div_(1.0 - p).view(n, c)
 
 
+def _step_dropout2d_scale(cs, n, device):
+    """The [n, K] scale of the Dropout2d fused into conv step `cs`, or None if it has none in training mode"""
+    d = cs.dropout2d
+    if d is None or not d.training or not d.p > 0.0:
+        return None
+    return _dropout2d_scale((n, cs.conv.out_channels), d.p, device)
+
+
 def _conv_cache(conv):
     cache = conv.__dict__.get("_b200_cache")
     if cache is None:
@@ -141,14 +149,22 @@ def _run_conv(conv, x, up=1, extra_pads=(0, 0, 0, 0), pad_mode=PAD_ZERO, act=ACT
     return F.conv_block(x, conv.weight, conv.bias, chan_scale, spec, _conv_cache(conv))
 
 
+def _running_stats(norm):
+    """(running_mean, running_var, num_batches_tracked, momentum) that a training-mode BatchNorm2d updates; Nones and
+    0.0 if it keeps no running statistics"""
+    if not (norm.track_running_stats and norm.running_mean is not None):
+        return None, None, None, 0.0
+    if norm.momentum is None:
+        raise NotImplementedError("b200gan: BatchNorm2d(momentum=None)")
+    return norm.running_mean, norm.running_var, norm.num_batches_tracked, float(norm.momentum)
+
+
 def _batch_norm_spec(norm, per_sample, act, slope, rtf_out, rtf_dx):
     """(NormSpec, running_mean, running_var, num_batches_tracked) of a norm that normalises with batch statistics."""
     rm = rv = nbt = None
     momentum = 0.0
-    if not per_sample and norm.training and norm.track_running_stats:
-        if norm.momentum is None:
-            raise NotImplementedError("b200gan: BatchNorm2d(momentum=None)")
-        rm, rv, nbt, momentum = norm.running_mean, norm.running_var, norm.num_batches_tracked, float(norm.momentum)
+    if not per_sample and norm.training:
+        rm, rv, nbt, momentum = _running_stats(norm)
     spec = NormSpec(per_sample=per_sample, eps=float(norm.eps), momentum=momentum, act=act, slope=slope,
                     rtf_out=rtf_out, rtf_dx=rtf_dx)
     return spec, rm, rv, nbt
@@ -359,6 +375,11 @@ class _ConvStep:
             return False
         return _tc_like(self.conv, self.up, full)
 
+    def fused_stats(self):
+        """self.stats when the following norm really normalises with batch statistics, else None (an eval-mode
+        BatchNorm2d never consumes -- and so never re-zeroes -- the shared accumulator)"""
+        return self.stats if (self.next_norm is not None and _uses_batch_stats(self.next_norm)) else None
+
 
 class _NormStep:
     def __init__(self, norm, act, slope, takes_stats):
@@ -382,6 +403,11 @@ class _TailStep:
 
 def _no_hooks(m):
     return not (m._forward_hooks or m._forward_pre_hooks or m._backward_hooks)
+
+
+def _plain(m, name):
+    """The stock class `name` or its drop-in, with no hooks that calling the module would run"""
+    return type(m) in (_T[name], REPLACEMENTS[name]) and _no_hooks(m)
 
 
 def _norm_conv_fused(ns, cs, x_shape):
@@ -603,13 +629,9 @@ def mlp_critic_layers(mods, in_features):
     """(Linear 1, Linear 2, Linear 3, slope) if the module list `mods` is exactly the MLP critic of wgan_gp.py:72-78 /
     wgan_div.py:72-78 -- Linear(in_features, H1) -> LeakyReLU(s) -> Linear(H1, H2) -> LeakyReLU(s) -> Linear(H2, 1), all
     with biases, one slope -- which runs as functional.MlpCriticFn; else None.  No side effects."""
-    def plain(m, name):  # the stock class or its drop-in, with no hooks that calling the module would run
-        return (type(m) in (_T[name], REPLACEMENTS[name]) and not m._forward_hooks and not m._forward_pre_hooks
-                and not m._backward_hooks)
-
-    if len(mods) != 5 or not all(plain(mods[i], "Linear") for i in (0, 2, 4)):
+    if len(mods) != 5 or not all(_plain(mods[i], "Linear") for i in (0, 2, 4)):
         return None
-    if not all(plain(mods[i], "LeakyReLU") for i in (1, 3)):
+    if not all(_plain(mods[i], "LeakyReLU") for i in (1, 3)):
         return None
     l1, l2, l3 = mods[0], mods[2], mods[4]
     if any(m.bias is None for m in (l1, l2, l3)) or mods[1].negative_slope != mods[3].negative_slope:
@@ -626,11 +648,7 @@ def mlp_discriminator_layers(mods, in_features):
     gan.py:64-80 / bgan.py:66-80 / aae.py:90-104 -- the critic mlp_critic_layers accepts, with a slope >= 0, followed by
     a Sigmoid -- which runs as functional.MlpDiscriminatorFn; else None.  Stock or drop-in classes only, without hooks.
     No side effects."""
-    if len(mods) != 6:
-        return None
-    sig = mods[5]
-    if (type(sig) not in (_T["Sigmoid"], REPLACEMENTS["Sigmoid"]) or sig._forward_hooks or sig._forward_pre_hooks
-            or sig._backward_hooks):
+    if len(mods) != 6 or not _plain(mods[5], "Sigmoid"):
         return None
     critic = mlp_critic_layers(mods[:5], in_features)
     if critic is None or critic[3] < 0:
@@ -645,30 +663,26 @@ def mlp_generator_layers(mods, in_features):
     functional.MlpGeneratorFn; else None.  Every BatchNorm1d is in training mode, affine, with tracked running statistics and a momentum (not None), all with
     one eps and one momentum: what the kernels compute.  A last Linear with one output stays with the Linear(K, 1) + Tanh
     head kernel.  Stock or drop-in classes only, without hooks.  No side effects."""
-    def plain(m, name):  # the stock class or its drop-in, with no hooks that calling the module would run
-        return (type(m) in (_T[name], REPLACEMENTS[name]) and not m._forward_hooks and not m._forward_pre_hooks
-                and not m._backward_hooks)
-
     layers, slopes, norms, i, width = [], set(), [], 0, in_features
     while i < len(mods):
         lin = mods[i]
-        if not plain(lin, "Linear") or lin.bias is None or lin.in_features != width:
+        if not _plain(lin, "Linear") or lin.bias is None or lin.in_features != width:
             return None
         width, i = lin.out_features, i + 1
         if i + 1 == len(mods):  # the output layer
-            if not plain(mods[i], "Tanh") or width == 1:
+            if not _plain(mods[i], "Tanh") or width == 1:
                 return None
             layers.append((lin, None))
             break
         bn = None
-        if i < len(mods) and plain(mods[i], "BatchNorm1d"):
+        if i < len(mods) and _plain(mods[i], "BatchNorm1d"):
             bn = mods[i]
             if not (bn.training and bn.affine and bn.track_running_stats and bn.running_mean is not None
                     and bn.momentum is not None and bn.num_features == width):
                 return None
             norms.append((bn.eps, bn.momentum))
             i += 1
-        if i >= len(mods) or not plain(mods[i], "LeakyReLU"):
+        if i >= len(mods) or not _plain(mods[i], "LeakyReLU"):
             return None
         slopes.add(mods[i].negative_slope)
         layers.append((lin, bn))
@@ -712,8 +726,8 @@ class Sequential(_T["Sequential"]):
         scales = [None] * len(plan)
         for gq in range(groups):
             for li, (cs, ns, oshape) in enumerate(plan):
-                if cs.dropout2d is not None and cs.dropout2d.training and cs.dropout2d.p > 0.0:
-                    part = _dropout2d_scale((x.shape[0] // groups, cs.conv.out_channels), cs.dropout2d.p, x.device)
+                part = _step_dropout2d_scale(cs, x.shape[0] // groups, x.device)
+                if part is not None:
                     scales[li] = part if scales[li] is None else torch.cat([scales[li], part])
         edge, prev_norm = None, None
         chain = F.ChainPass()
@@ -724,18 +738,12 @@ class Sequential(_T["Sequential"]):
             momentum = 0.0
             if prev_norm is not None:
                 gam, bet = prev_norm.weight, prev_norm.bias
-                if prev_norm.track_running_stats and prev_norm.running_mean is not None:
-                    rm, rv, nbt = prev_norm.running_mean, prev_norm.running_var, prev_norm.num_batches_tracked
-                    momentum = float(prev_norm.momentum)
+                rm, rv, nbt, momentum = _running_stats(prev_norm)
             spec = F.NbSpec(stride=int(conv.stride[0]), pad=int(conv.padding[0]), act=cs.act, slope=cs.slope,
                             momentum=momentum, want_stats=ns is not None, groups=groups)
-            cache = conv.__dict__.get("_b200_cache")
-            if cache is None:
-                cache = PackCache()
-                conv.__dict__["_b200_cache"] = cache
             out_box = []
-            res = F.NbConvFn.apply(x, conv.weight, conv.bias, scale, gam, bet, rm, rv, nbt, edge, out_box, spec, cache,
-                                   chain)
+            res = F.NbConvFn.apply(x, conv.weight, conv.bias, scale, gam, bet, rm, rv, nbt, edge, out_box, spec,
+                                   _conv_cache(conv), chain)
             if ns is not None:
                 x, stats = res
                 norm = ns.norm
@@ -747,12 +755,9 @@ class Sequential(_T["Sequential"]):
             else:
                 x, edge, prev_norm = res, None, None
         if edge is not None:
-            norm = prev_norm
-            rm = rv = nbt = None
-            momentum = 0.0
-            if norm.track_running_stats and norm.running_mean is not None:
-                rm, rv, nbt, momentum = norm.running_mean, norm.running_var, norm.num_batches_tracked, float(norm.momentum)
-            x = F.NbTailFn.apply(x, norm.weight, norm.bias, rm, rv, nbt, edge, momentum, bool(nchw_out), chain)
+            rm, rv, nbt, momentum = _running_stats(prev_norm)
+            x = F.NbTailFn.apply(x, prev_norm.weight, prev_norm.bias, rm, rv, nbt, edge, momentum, bool(nchw_out),
+                                 chain)
         return x
 
     def _forward_2d(self, x):
@@ -816,12 +821,7 @@ class Sequential(_T["Sequential"]):
                 _no_groups("the fused generator tail")
                 if (norm.training and x.shape[1] == conv.in_channels and x.shape[1] == norm.num_features
                         and ops.tail_supported(tuple(x.shape), conv.out_channels, ns.act, ns.slope, cs.act)):
-                    rm = rv = nbt = None
-                    momentum = 0.0
-                    if norm.track_running_stats and norm.running_mean is not None:
-                        if norm.momentum is None:
-                            raise NotImplementedError("b200gan: BatchNorm2d(momentum=None)")
-                        rm, rv, nbt, momentum = norm.running_mean, norm.running_var, norm.num_batches_tracked, float(norm.momentum)
+                    rm, rv, nbt, momentum = _running_stats(norm)
                     spec = F.TailSpec(eps=float(norm.eps), momentum=momentum, act_mid=ns.act, slope=ns.slope,
                                       act_out=cs.act, rtf_dx=ns.rtf_dx)
                     x = F.TailFn.apply(x, stats if ns.takes_stats else None, norm.weight, norm.bias, rm, rv, nbt,
@@ -833,10 +833,8 @@ class Sequential(_T["Sequential"]):
             if queue and _norm_conv_fused(s, queue[0], tuple(x.shape)):
                 # one node whose backward takes the norm's sums from the conv's data-gradient epilogue
                 ns, cs = s, queue.pop(0)
-                scale = None
-                if cs.dropout2d is not None and cs.dropout2d.training and cs.dropout2d.p > 0.0:
-                    scale = _dropout2d_scale((x.shape[0], cs.conv.out_channels), cs.dropout2d.p, x.device)
-                want = cs.stats if (cs.next_norm is not None and _uses_batch_stats(cs.next_norm)) else None
+                scale = _step_dropout2d_scale(cs, x.shape[0], x.device)
+                want = cs.fused_stats()
                 norm, conv = ns.norm, cs.conv
                 nspec, rm, rv, nbt = _batch_norm_spec(norm, False, ns.act, ns.slope, ns.rtf_out, ns.rtf_dx)
                 cspec = ConvSpec(stride=1, pads=tuple(e + int(conv.padding[0]) for e in cs.extra_pads), up=cs.up,
@@ -846,14 +844,10 @@ class Sequential(_T["Sequential"]):
                 x, stats = out if want is not None else (out, None)
                 continue
             if isinstance(s, _ConvStep):
-                cs = None
-                if s.dropout2d is not None and s.dropout2d.training and s.dropout2d.p > 0.0:
+                cs = _step_dropout2d_scale(s, x.shape[0], x.device)
+                if cs is not None:
                     _no_groups("a Dropout2d outside a fused chain")
-                    n = x.shape[0]
-                    cs = _dropout2d_scale((n, s.conv.out_channels), s.dropout2d.p, x.device)
-                # fused statistics only when the following norm really normalises with batch statistics (an eval-mode
-                # BatchNorm2d never consumes -- and so never re-zeroes -- the shared accumulator)
-                want = s.stats if (s.next_norm is not None and _uses_batch_stats(s.next_norm)) else None
+                want = s.fused_stats()
                 out = _run_conv(s.conv, x, s.up, s.extra_pads, s.pad_mode, s.act, s.slope, cs, want, s.rtf_out,
                                 s.rtf_dz)
                 if want is not None:

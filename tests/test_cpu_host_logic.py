@@ -204,3 +204,29 @@ def test_negative_leaky_relu_slope_is_refused():
         bnn._act_of(torch.nn.LeakyReLU(-0.1))
     assert bnn._act_of(torch.nn.LeakyReLU(0.2)) == (bnn.ACT_LRELU, 0.2)
     assert bnn._act_of(torch.nn.LeakyReLU(0.0)) == (bnn.ACT_LRELU, 0.0)
+
+
+@pytest.mark.parametrize("state", ["tracked", "untracked", "buffers_none", "momentum_none", "eval"])
+def test_running_statistics_every_batchnorm_path_updates(state):
+    """What a batch-statistics BatchNorm2d hands its kernels to update -- the same on the stand-alone path, the fused
+    tail and the fused chain: its running buffers and momentum only if it tracks them AND has them.  A norm whose
+    buffers were set to None updates nothing (not even num_batches_tracked); momentum=None with buffers is refused."""
+    from b200gan import nn as bnn
+    bn = bnn.BatchNorm2d(8, 0.8, momentum=None if state == "momentum_none" else 0.1,
+                         track_running_stats=state != "untracked").train(state != "eval")
+    if state == "buffers_none":
+        bn.running_mean = bn.running_var = None
+    if state == "momentum_none":
+        with pytest.raises(NotImplementedError, match="momentum=None"):
+            bnn._running_stats(bn)
+        with pytest.raises(NotImplementedError, match="momentum=None"):
+            bnn._batch_norm_spec(bn, False, 0, 0.0, False, False)
+        return
+    expected = (None, None, None, 0.0)
+    if state in ("tracked", "eval"):
+        expected = (bn.running_mean, bn.running_var, bn.num_batches_tracked, 0.1)
+    assert bnn._running_stats(bn) == expected
+    spec, rm, rv, nbt = bnn._batch_norm_spec(bn, False, 0, 0.0, False, False)
+    if state == "eval":  # an eval-mode norm normalises with batch statistics only without buffers: no update then
+        expected = (None, None, None, 0.0)
+    assert (rm, rv, nbt, spec.momentum) == expected
