@@ -469,6 +469,35 @@ int b200gan_linear1_bwd(const float *x, const float *w, const float *y, const fl
 int b200gan_bce_fwd(const float *v, const float *t, float *loss, int64_t n, void *stream);
 int b200gan_bce_bwd(const float *v, const float *t, const float *gout, float *dv, int64_t n, void *stream);
 
+/* ---- Auxiliary-classifier head and its loss (csrc/head.cu) ----------------------------------------------------- */
+/* nn.Sequential(nn.Linear(K, n_classes), nn.Softmax()) (acgan.py:100, sgan.py:99, infogan.py:111) and
+ * torch.nn.CrossEntropyLoss() (acgan.py:113, sgan.py:112, infogan.py:126) as run-time modes of the head and BCE kernels
+ * above: each entry point launches exactly the one kernel named beside it. */
+/* The head backward keeps dz [N][nout] in shared memory beside 16 bytes of its own: 48 KB in all. */
+enum { B200GAN_CLASS_HEAD_BWD_MAX_ELEMS = 12284, B200GAN_CROSS_ENTROPY_MAX_CLASSES = 1024 };
+/* y [N][nout] = softmax(x w^T + b) over the nout outputs, 2 <= nout <= 32.  x [N][K], w [nout][K] row-major, b [nout]
+ * (may be NULL).  N >= 1.  ONE launch of linear1_fwd_kernel, one 128-thread block per row. */
+int b200gan_class_head_fwd(const float *x, const float *w, const float *b, float *y, int32_t N, int32_t K,
+                           int32_t nout, void *stream);
+/* Backward from the saved output y and dy [N][nout]: dx [N][K] (may be NULL), dw [nout][K], db [nout] (may be NULL)
+ * are OVERWRITTEN.  N * nout <= B200GAN_CLASS_HEAD_BWD_MAX_ELEMS.  ONE launch of linear1_bwd_kernel, ceil(K / 128)
+ * blocks; dw and db are summed in row order (deterministic). */
+int b200gan_class_head_bwd(const float *x, const float *w, const float *y, const float *dy, float *dx, float *dw,
+                           float *db, int32_t N, int32_t K, int32_t nout, void *stream);
+/* Reduction 'mean' over the rows whose int64 class index target[r] != ignore_index: out2[0] = the loss, out2[1] = the
+ * number of such rows (NaN loss when it is 0, as in torch).  A target outside [0, C) that is not ignore_index makes the
+ * loss NaN (torch raises a device assert instead); no logit outside its row is read.  x [N][C], N >= 1,
+ * 1 <= C <= B200GAN_CROSS_ENTROPY_MAX_CLASSES.  Summed in a fixed order in fp64: bit-identical from call to call.  ONE
+ * launch of bce_fwd_kernel, one block of 1024 threads (a warp per row): made for the scripts' batches, it is slow for
+ * large N * C, where the drop-in CrossEntropyLoss keeps the stock path (more than 64 Ki logits). */
+int b200gan_cross_entropy_fwd(const float *x, const int64_t *target, float *out2, int32_t N, int32_t C,
+                              int64_t ignore_index, void *stream);
+/* dx [N][C] (OVERWRITTEN) = gout[0] / out2[1] * (softmax(x[r]) - onehot(target[r])), both read on the device: zero rows
+ * for ignored targets, NaN rows for out-of-range ones.  ONE launch of bce_bwd_kernel, a warp per row (ceil(N / 8)
+ * blocks of 256 threads). */
+int b200gan_cross_entropy_bwd(const float *x, const int64_t *target, const float *out2, const float *gout, float *dx,
+                              int32_t N, int32_t C, int64_t ignore_index, void *stream);
+
 /* ---- MSELoss / L1Loss, reduction 'mean' (csrc/pixel_loss/) --------------------------------------------------------- */
 /* torch.nn.MSELoss() / torch.nn.L1Loss() of an input a and a target b of one logical shape [N][C][H][W] (fewer
  * dimensions padded with leading 1s): the adversarial loss of LSGAN, Pix2Pix and CycleGAN (lsgan.py:102, pix2pix.py:50,

@@ -42,6 +42,9 @@ class MlpCriticDesc(ctypes.Structure):
 
 
 MLP_GEN_MAX_LAYERS, MLP_GEN_MAX_WIDTH, MLP_GEN_MAX_N = 8, 8192, 8192
+CLASS_HEAD_MAX_CLASSES, CLASS_HEAD_BWD_MAX_ELEMS, CROSS_ENTROPY_MAX_CLASSES = 32, 12284, 1024
+# the cross-entropy forward is one block: past this many logits ATen's multi-block log_softmax + nll_loss is faster
+CROSS_ENTROPY_MAX_LOGITS = 1 << 16
 
 
 class MlpGenDesc(ctypes.Structure):
@@ -147,6 +150,10 @@ SIGNATURES = {
     "b200gan_linear1_bwd": (c_i32, [c_vp] * 7 + [c_i32, c_i32, c_i32, c_vp]),
     "b200gan_bce_fwd": (c_i32, [c_vp, c_vp, c_vp, c_i64, c_vp]),
     "b200gan_bce_bwd": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
+    "b200gan_class_head_fwd": (c_i32, [c_vp] * 4 + [c_i32, c_i32, c_i32, c_vp]),
+    "b200gan_class_head_bwd": (c_i32, [c_vp] * 7 + [c_i32, c_i32, c_i32, c_vp]),
+    "b200gan_cross_entropy_fwd": (c_i32, [c_vp, c_vp, c_vp, c_i32, c_i32, c_i64, c_vp]),
+    "b200gan_cross_entropy_bwd": (c_i32, [c_vp] * 5 + [c_i32, c_i32, c_i64, c_vp]),
     "b200gan_pixel_loss_workspace_bytes": (c_sz, [_P(PixelLossDesc)]),
     "b200gan_pixel_loss_fwd": (c_i32, [_P(PixelLossDesc), c_vp, c_vp, c_vp, c_vp, c_vp]),
     "b200gan_pixel_loss_bwd": (c_i32, [_P(PixelLossDesc), c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),

@@ -834,6 +834,65 @@ class BCEMeanFn(torch.autograd.Function):
         return ops.bce_bwd(v, t, gout.contiguous()), None
 
 
+class ClassHeadFn(torch.autograd.Function):
+    """nn.Linear(K, n) + nn.Softmax over the n outputs on a 2-D CUDA tensor, 2 <= n <= 32: the auxiliary-classifier head
+    of acgan.py:100 / sgan.py:99 / infogan.py:111, one kernel per direction (csrc/head.cu).  dx, dW and db are each
+    optional."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias):
+        ops._require_cuda(x, "linear input")
+        y = ops.class_head_fwd(x.contiguous(), weight.detach().contiguous(), None if bias is None else bias.detach())
+        ctx.has_bias = bias is not None
+        # the input itself, not a contiguous copy made here: a create_graph=True backward differentiates through it
+        ctx.save_for_backward(x, weight, y)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, weight, y = ctx.saved_tensors
+        need_dx, need_dw = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+        need_db = ctx.has_bias and ctx.needs_input_grad[2]
+        if not (need_dx or need_dw or need_db):
+            return None, None, None
+        if torch.is_grad_enabled():  # create_graph=True: stay differentiable (plain torch ops on the saved tensors)
+            dz = y * (dy - (dy * y).sum(1, keepdim=True))
+            return (dz @ weight if need_dx else None), (dz.t() @ x if need_dw else None), \
+                (dz.sum(0) if need_db else None)
+        dx, dw, db = ops.class_head_bwd(x.detach().contiguous(), weight.detach().contiguous(), y, dy.contiguous(),
+                                        need_dx, need_db)
+        return dx, (dw if need_dw else None), db
+
+
+class CrossEntropyMeanFn(torch.autograd.Function):
+    """torch.nn.CrossEntropyLoss() (reduction 'mean', class-index targets, no class weights, no label smoothing) of
+    [N, C] logits, forward and backward as one kernel each (csrc/head.cu): the auxiliary loss of acgan.py:113 /
+    sgan.py:112 / infogan.py:126.  The gradient is with respect to the logits only."""
+
+    @staticmethod
+    def forward(ctx, x, target, ignore_index):
+        target = target.contiguous()
+        out = ops.cross_entropy_fwd(x.contiguous(), target, ignore_index)
+        ctx.ignore_index = ignore_index
+        # the input itself, not a contiguous copy made here: a create_graph=True backward differentiates through it
+        ctx.save_for_backward(x, target, out)
+        # out[0] would be a view, which autograd refuses to modify in place (`loss += reg`); alias the storage instead
+        return out.new_empty(0).set_(out.untyped_storage(), out.storage_offset(), ())
+
+    @staticmethod
+    def backward(ctx, gout):
+        x, target, out = ctx.saved_tensors
+        if not ctx.needs_input_grad[0]:
+            return None, None, None
+        if torch.is_grad_enabled():  # create_graph=True: stay differentiable (plain torch ops on the saved tensors)
+            hit = torch.arange(x.shape[1], device=x.device) == target[:, None]
+            keep = (target != ctx.ignore_index)[:, None]
+            d = (torch.softmax(x, 1) - hit.to(x.dtype)) * (gout / out[1])
+            return torch.where(keep, d, torch.zeros_like(d)), None, None
+        return ops.cross_entropy_bwd(x.detach().contiguous(), target, out, gout.detach().contiguous(),
+                                     ctx.ignore_index), None, None
+
+
 class PixelLossFn(torch.autograd.Function):
     """torch.nn.MSELoss() / torch.nn.L1Loss() (reduction 'mean') forward and backward as one kernel each
     (csrc/pixel_loss/): the adversarial, pixel, cycle and identity losses of the image translators

@@ -9,6 +9,8 @@ become single fused nodes; anything unknown is executed leaf by leaf.
 
 There is no CPU / cuDNN fallback for the conv and norm modules: CPU tensors raise.
 """
+import warnings
+
 import torch
 import torch.nn as tnn
 
@@ -23,7 +25,7 @@ _T = {  # the stock classes, captured before any patching
     n: getattr(tnn, n) for n in (
         "Conv2d", "ConvTranspose2d", "BatchNorm2d", "InstanceNorm2d", "LeakyReLU", "ReLU", "Tanh", "Sigmoid",
         "Upsample", "ZeroPad2d", "ReflectionPad2d", "Dropout", "Dropout2d", "Sequential", "Linear", "BCELoss",
-        "BatchNorm1d", "MSELoss", "L1Loss")
+        "BatchNorm1d", "MSELoss", "L1Loss", "Softmax", "CrossEntropyLoss")
 }
 
 
@@ -358,6 +360,69 @@ class L1Loss(_T["L1Loss"]):
     def forward(self, input, target):
         if pixel_loss_routed(input, target, self.reduction):
             return F.PixelLossFn.apply(input, target, PIXEL_LOSS_L1)
+        return super().forward(input, target)
+
+
+class Softmax(_T["Softmax"]):
+    """nn.Softmax, the stock module.  Behind a Linear(K, n) inside a Sequential (class_head_routed, acgan.py:100) it runs
+    in the class-head kernels; anywhere else it is the stock forward."""
+
+
+def _softmax_dim(softmax, ndim):
+    """The dimension a Softmax module normalises over for an ndim-D input: its dim, or for dim=None the implicit choice
+    of torch's own _get_softmax_dim, taken without its deprecation warning."""
+    if softmax.dim is not None:
+        return softmax.dim % ndim if -ndim <= softmax.dim < ndim else None
+    with warnings.catch_warnings():
+        warnings.simplefilter("ignore")
+        return tnn.functional._get_softmax_dim("softmax", ndim, 0)
+
+
+def class_head_routed(linear, softmax, x):
+    """True if `linear` followed by `softmax` on x runs as functional.ClassHeadFn (the auxiliary-classifier head,
+    acgan.py:100 / sgan.py:99 / infogan.py:111): stock or drop-in Linear and Softmax without hooks, a 2-D CUDA fp32 x of
+    at least one row, 2 <= out_features <= 32, fp32 parameters on x's device, the softmax over dimension 1, and
+    N * out_features within the backward's shared-memory bound.  No side effects."""
+    if softmax is None or not (_plain(linear, "Linear") and _plain(softmax, "Softmax")):
+        return False
+    if not (torch.is_tensor(x) and x.dim() == 2 and _on_device(x) and x.dtype == torch.float32):
+        return False
+    n = linear.out_features
+    if not 2 <= n <= _lib.CLASS_HEAD_MAX_CLASSES or x.shape[0] < 1 or x.shape[1] != linear.in_features:
+        return False
+    if x.shape[0] * n > _lib.CLASS_HEAD_BWD_MAX_ELEMS:
+        return False
+    params = [linear.weight] + ([] if linear.bias is None else [linear.bias])
+    if not all(p.device == x.device and p.dtype == torch.float32 for p in params):
+        return False
+    return _softmax_dim(softmax, 2) == 1
+
+
+def cross_entropy_routed(input, target, weight, reduction, label_smoothing):
+    """True if CrossEntropyLoss(input, target) runs on the cross-entropy kernels (functional.CrossEntropyMeanFn): a 2-D
+    CUDA fp32 input [N, C] with N >= 1, 1 <= C <= 1024 and N * C <= 65536 (the forward is one block of 1024 threads: the
+    scripts' batches, not a large-batch classifier), a 1-D int64 class-index target of length N on the same device, no
+    class weights, reduction 'mean' and no label smoothing; any ignore_index.  Everything else -- probability targets,
+    K-dimensional or unbatched inputs, 'sum' / 'none', larger inputs, the CPU -- is the stock module.  No side effects."""
+    if reduction != "mean" or weight is not None or label_smoothing != 0.0:
+        return False
+    if not (torch.is_tensor(input) and torch.is_tensor(target)):
+        return False
+    if input.dim() != 2 or input.dtype != torch.float32 or target.dim() != 1 or target.dtype != torch.int64:
+        return False
+    if not (_on_device(input) and _on_device(target) and input.device == target.device):
+        return False
+    n, c = input.shape
+    return (n >= 1 and 1 <= c <= _lib.CROSS_ENTROPY_MAX_CLASSES and n * c <= _lib.CROSS_ENTROPY_MAX_LOGITS
+            and target.shape[0] == n)
+
+
+class CrossEntropyLoss(_T["CrossEntropyLoss"]):
+    """nn.CrossEntropyLoss (acgan.py:113, sgan.py:112, infogan.py:126); routing: cross_entropy_routed."""
+
+    def forward(self, input, target):
+        if cross_entropy_routed(input, target, self.weight, self.reduction, self.label_smoothing):
+            return F.CrossEntropyMeanFn.apply(input, target, self.ignore_index)
         return super().forward(input, target)
 
 
@@ -783,6 +848,11 @@ class Sequential(_T["Sequential"]):
                     and _act_of(mods[i + 1])[0] in (ACT_SIGMOID, ACT_TANH)):
                 x = F.Linear1Fn.apply(x, m.weight, m.bias, _act_of(mods[i + 1])[0])
                 i += 2
+            elif class_head_routed(m, mods[i + 1] if i + 1 < len(mods) else None, x):
+                if mods[i + 1].dim is None:   # the deprecation warning the stock Softmax raises for an implicit dim
+                    tnn.functional._get_softmax_dim("softmax", x.dim(), 5)
+                x = F.ClassHeadFn.apply(x, m.weight, m.bias)
+                i += 2
             else:
                 x = m(x)
                 i += 1
@@ -871,7 +941,7 @@ REPLACEMENTS = {
     "InstanceNorm2d": InstanceNorm2d, "LeakyReLU": LeakyReLU, "ReLU": ReLU, "Tanh": Tanh, "Sigmoid": Sigmoid,
     "Upsample": Upsample, "ZeroPad2d": ZeroPad2d, "ReflectionPad2d": ReflectionPad2d, "Dropout": Dropout,
     "Dropout2d": Dropout2d, "Sequential": Sequential, "Linear": Linear, "BCELoss": BCELoss, "BatchNorm1d": BatchNorm1d,
-    "MSELoss": MSELoss, "L1Loss": L1Loss,
+    "MSELoss": MSELoss, "L1Loss": L1Loss, "Softmax": Softmax, "CrossEntropyLoss": CrossEntropyLoss,
 }
 for _n, _c in REPLACEMENTS.items():
     _c.__name__ = _n

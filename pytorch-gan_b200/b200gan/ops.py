@@ -569,6 +569,48 @@ def bce_bwd(v, t, gout):
     return dv
 
 
+# ---- Auxiliary-classifier head and its loss: Linear(K, n) + Softmax, CrossEntropyLoss (csrc/head.cu) -------------------
+def class_head_fwd(x, w, b):
+    """softmax(x w^T + b) over the n = w.shape[0] outputs (2 <= n <= 32) of a contiguous [N, K] x; one launch."""
+    n, k = x.shape
+    y = torch.empty((n, w.shape[0]), device=x.device, dtype=torch.float32)
+    _lib.check(_lib.load().b200gan_class_head_fwd(x.data_ptr(), w.data_ptr(), _ptr(b), y.data_ptr(), n, k, w.shape[0],
+                                                  _stream()), "class_head_fwd")
+    return y
+
+
+def class_head_bwd(x, w, y, dy, need_dx, need_db):
+    """(dx or None, dw, db or None) from the saved softmax output y and dy, both [N, n]; one launch."""
+    n, k = x.shape
+    nout = w.shape[0]
+    dx = torch.empty_like(x) if need_dx else None
+    dw = torch.empty((nout, k), device=x.device, dtype=torch.float32)
+    db = torch.empty(nout, device=x.device, dtype=torch.float32) if need_db else None
+    _lib.check(_lib.load().b200gan_class_head_bwd(x.data_ptr(), w.data_ptr(), y.data_ptr(), dy.data_ptr(), _ptr(dx),
+                                                  dw.data_ptr(), _ptr(db), n, k, nout, _stream()), "class_head_bwd")
+    return dx, dw, db
+
+
+def cross_entropy_fwd(x, target, ignore_index):
+    """[loss, count] (fp32, on the device) of CrossEntropyLoss(reduction='mean') of contiguous [N, C] logits and int64
+    class indices [N]; one launch.  out[0] is the loss; the backward reads out[1]."""
+    n, c = x.shape
+    out = torch.empty(2, device=x.device, dtype=torch.float32)
+    _lib.check(_lib.load().b200gan_cross_entropy_fwd(x.data_ptr(), target.data_ptr(), out.data_ptr(), n, c,
+                                                     int(ignore_index), _stream()), "cross_entropy_fwd")
+    return out
+
+
+def cross_entropy_bwd(x, target, out, gout, ignore_index):
+    """d loss / d x for the upstream gradient gout (0-dim, read on the device); one launch."""
+    n, c = x.shape
+    dx = torch.empty_like(x)
+    _lib.check(_lib.load().b200gan_cross_entropy_bwd(x.data_ptr(), target.data_ptr(), out.data_ptr(), gout.data_ptr(),
+                                                     dx.data_ptr(), n, c, int(ignore_index), _stream()),
+               "cross_entropy_bwd")
+    return dx
+
+
 # ---- MSELoss / L1Loss, reduction 'mean' (csrc/pixel_loss/) --------------------------------------------------------------
 def pixel_layout(t):
     """_lib.LAYOUT_NCHW for a contiguous tensor, LAYOUT_NHWC for a 4-D channels_last one, else None (not dense in either

@@ -159,14 +159,48 @@ def wgan_gp_generator_step(generator, discriminator, opt_g, z):
     return g_loss.detach()
 
 
+def _built_from_dropins(*nets):
+    from . import nn as bnn
+    dropin = tuple(bnn.REPLACEMENTS.values())
+    return any(isinstance(m, dropin) for net in nets for m in net.modules())
+
+
 def _pixel_losses(*nets):
     """(mse, l1) for a translator's step: the drop-in MSELoss / L1Loss (csrc/pixel_loss) when the networks are built from
     drop-in modules, else torch's own functional losses, so that a stock model keeps every op on stock torch."""
     from . import nn as bnn
-    dropin = tuple(bnn.REPLACEMENTS.values())
-    if any(isinstance(m, dropin) for net in nets for m in net.modules()):
+    if _built_from_dropins(*nets):
         return bnn.MSELoss(), bnn.L1Loss()
     return torch.nn.functional.mse_loss, torch.nn.functional.l1_loss
+
+
+def acgan_step(generator, discriminator, opt_g, opt_d, real_imgs, labels, z, gen_labels):
+    """implementations/acgan/acgan.py:184-223, with the noise z and the int64 class indices gen_labels drawn by the
+    caller (:187-188).  BCELoss and CrossEntropyLoss (:112-113) are the drop-ins when the networks are built from
+    drop-in modules, else torch's own.  D is frozen during the G step, as in dcgan_step.  Returns the two losses, the
+    fakes and the class posteriors of the real and the fake pass (the script's accuracy readback, :218-220)."""
+    from . import nn as bnn
+    ns = bnn if _built_from_dropins(generator, discriminator) else torch.nn
+    adversarial_loss, auxiliary_loss = ns.BCELoss(), ns.CrossEntropyLoss()
+    n = real_imgs.shape[0]
+    valid = torch.ones(n, 1, device=real_imgs.device)                                        # :173
+    fake = torch.zeros(n, 1, device=real_imgs.device)                                        # :174
+    opt_g.zero_grad()                                                                        # :184
+    gen_imgs = generator(z, gen_labels)                                                      # :191
+    with frozen(discriminator):
+        validity, pred_label = discriminator(gen_imgs)                                       # :194
+        g_loss = 0.5 * (adversarial_loss(validity, valid) + auxiliary_loss(pred_label, gen_labels))  # :195
+        g_loss.backward()                                                                    # :197
+    opt_g.step()                                                                             # :198
+    opt_d.zero_grad()                                                                        # :204
+    real_pred, real_aux = discriminator(real_imgs)                                           # :207
+    d_real_loss = (adversarial_loss(real_pred, valid) + auxiliary_loss(real_aux, labels)) / 2           # :208
+    fake_pred, fake_aux = discriminator(gen_imgs.detach())                                   # :211
+    d_fake_loss = (adversarial_loss(fake_pred, fake) + auxiliary_loss(fake_aux, gen_labels)) / 2        # :212
+    d_loss = (d_real_loss + d_fake_loss) / 2                                                 # :215
+    d_loss.backward()                                                                        # :222
+    opt_d.step()                                                                             # :223
+    return g_loss.detach(), d_loss.detach(), gen_imgs.detach(), real_aux.detach(), fake_aux.detach()
 
 
 def pix2pix_step(generator, discriminator, opt_g, opt_d, real_a, real_b, lambda_pixel=100.0, reduce_g=None,

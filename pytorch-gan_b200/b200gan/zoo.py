@@ -6,6 +6,7 @@ unmodified instead.  Citations: implementations/<name>/...
 """
 import types
 
+import torch
 import torch.nn as tnn
 
 from . import nn as bnn
@@ -86,6 +87,62 @@ class DCGANDiscriminator(tnn.Module):
         out = self.model(img)
         out = out.view(out.shape[0], -1)
         return self.adv_layer(out)
+
+
+class ACGANGenerator(tnn.Module):
+    """acgan/acgan.py:46-73: the DCGAN generator behind a label embedding multiplied into the noise.  nn.Embedding and
+    torch.mul stay stock torch."""
+
+    def __init__(self, img_size=32, latent_dim=100, n_classes=10, channels=1, nn=None):
+        super().__init__()
+        nn = nn or namespace()
+        self.label_emb = nn.Embedding(n_classes, latent_dim)
+        self.init_size = img_size // 4
+        self.l1 = nn.Sequential(nn.Linear(latent_dim, 128 * self.init_size ** 2))
+        self.conv_blocks = nn.Sequential(
+            nn.BatchNorm2d(128),
+            nn.Upsample(scale_factor=2),
+            nn.Conv2d(128, 128, 3, stride=1, padding=1),
+            nn.BatchNorm2d(128, 0.8),
+            nn.LeakyReLU(0.2, inplace=True),
+            nn.Upsample(scale_factor=2),
+            nn.Conv2d(128, 64, 3, stride=1, padding=1),
+            nn.BatchNorm2d(64, 0.8),
+            nn.LeakyReLU(0.2, inplace=True),
+            nn.Conv2d(64, channels, 3, stride=1, padding=1),
+            nn.Tanh(),
+        )
+
+    def forward(self, noise, labels):
+        out = self.l1(torch.mul(self.label_emb(labels), noise))
+        out = out.view(out.shape[0], 128, self.init_size, self.init_size)
+        return self.conv_blocks(out)
+
+
+class ACGANDiscriminator(tnn.Module):
+    """acgan/acgan.py:76-108: the DCGAN discriminator blocks with two heads, Linear(K, 1) + Sigmoid (validity) and
+    Linear(K, n_classes) + Softmax() (the class posterior; the implicit dim resolves to 1)."""
+
+    def __init__(self, img_size=32, channels=1, n_classes=10, nn=None):
+        super().__init__()
+        nn = nn or namespace()
+
+        def block(cin, cout, bn=True):
+            layers = [nn.Conv2d(cin, cout, 3, 2, 1), nn.LeakyReLU(0.2, inplace=True), nn.Dropout2d(0.25)]
+            if bn:
+                layers.append(nn.BatchNorm2d(cout, 0.8))
+            return layers
+
+        self.conv_blocks = nn.Sequential(*block(channels, 16, bn=False), *block(16, 32), *block(32, 64),
+                                         *block(64, 128))
+        ds_size = img_size // 2 ** 4
+        self.adv_layer = nn.Sequential(nn.Linear(128 * ds_size ** 2, 1), nn.Sigmoid())
+        self.aux_layer = nn.Sequential(nn.Linear(128 * ds_size ** 2, n_classes), nn.Softmax())
+
+    def forward(self, img):
+        out = self.conv_blocks(img)
+        out = out.view(out.shape[0], -1)
+        return self.adv_layer(out), self.aux_layer(out)
 
 
 class WGANGPGenerator(tnn.Module):
