@@ -14,6 +14,11 @@ tests/test_cpu_fused_case_table.py holds the table to the sources and to the lib
 """
 from dataclasses import dataclass
 
+import torch
+import torch.nn.functional as F
+
+from b200gan import _lib
+
 NUM_SMS = 132
 OPS = ("fprop", "dz", "wgrad", "dgrad", "plain_dgrad", "tail_fwd", "tail_bwd")
 EDGES = ("none", "stats", "affine")
@@ -257,3 +262,109 @@ HOOK_ONLY = {
     dg(3, 2): "C = 3 is the only width that plans KT = 3, and allow_pt needs C >= 4: PT is always 1",
     dg(3, 4): "C = 3 is the only width that plans KT = 3, and allow_pt needs C >= 4: PT is always 1",
 }
+
+
+# ---- fp64 references (device-agnostic: tests/test_cpu_fused_case_table.py holds them to stock torch) -----------------
+U = 2.0 ** -23
+SLOPE = 0.2
+MOMENTUM = 0.1
+BN_EPS = 0.8          # nn.BatchNorm2d(out, 0.8) of dcgan.py:82
+NBT0 = 7
+BLOCK_PARTIAL = 1032  # values a chain kernel sums in fp32 before its fp64 atomic: at most a tile's 1024 pixels
+ACT_CODE = {"none": _lib.ACT_NONE, "lrelu": _lib.ACT_LRELU, "relu": _lib.ACT_RELU, "tanh": _lib.ACT_TANH,
+            "sigmoid": _lib.ACT_SIGMOID}
+NEG_SLOPE = {"none": 1.0, "lrelu": SLOPE, "relu": 0.0}
+
+
+def group_sums(t, G):
+    """[G][2][C] fp64 sum and sum of squares of t [N, ..., C] over each of G equal runs of images"""
+    t = t.double().reshape(G, -1, t.shape[-1])
+    return torch.stack([t.sum(1), (t * t).sum(1)], 1)
+
+
+def bn_consts(stats, gamma, beta, count, G, C, eps=BN_EPS):
+    """mean, biased var, rstd, scale, shift [G][C] from the batch sums, as nb_bn_consts forms them (in fp64)"""
+    st = stats.double().reshape(G, 2, C)
+    mean = st[:, 0] / count
+    var = (st[:, 1] / count - mean * mean).clamp_min(0)
+    rstd = 1 / torch.sqrt(var + eps)
+    ga = gamma.double() if gamma is not None else torch.ones_like(mean[0])
+    be = beta.double() if beta is not None else torch.zeros_like(mean[0])
+    sc = ga * rstd
+    return mean, var, rstd, sc, be - mean * sc
+
+
+def per_image(t, N):
+    """[G][C] -> [N][1][1][C]: the group's row for every image of the group"""
+    return t.repeat_interleave(N // t.shape[0], 0)[:, None, None, :]
+
+
+def running_ref(rm, rv, mean, var, count, momentum=MOMENTUM):
+    """one torch running-statistics update per group, in batch order"""
+    rm, rv = rm.double(), rv.double()
+    unb = var * count / (count - 1) if count > 1 else var
+    for g in range(mean.shape[0]):
+        rm = (1 - momentum) * rm + momentum * mean[g]
+        rv = (1 - momentum) * rv + momentum * unb[g]
+    return rm, rv
+
+
+def nchw(t):
+    return t.permute(0, 3, 1, 2)
+
+
+def nhwc(t):
+    return t.permute(0, 2, 3, 1)
+
+
+def conv_fwd(x, w, stride, pad):
+    return nhwc(F.conv2d(nchw(x), w, stride=stride, padding=pad))
+
+
+def conv_dgrad(dz, w, xshape, stride, pad):
+    N, H, W, C = xshape
+    return nhwc(torch.nn.grad.conv2d_input((N, C, H, W), w, nchw(dz), stride, pad))
+
+
+def conv_wgrad(x, dz, wshape, stride, pad):
+    return torch.nn.grad.conv2d_weight(nchw(x), wshape, nchw(dz), stride, pad)
+
+
+def bn_bwd_ref(G_, a, mean, rstd, sc, sums, count, cs, act):
+    """nb_dz: dz = scale * (G - sum G / count - ahat * sum G ahat / count) * chan_scale * act'(a), groups per image"""
+    N = a.shape[0]
+    m1, m2 = sums[:, 0] / count, sums[:, 1] / count
+    xh = (a - per_image(mean, N)) * per_image(rstd, N)
+    dA = per_image(sc, N) * (G_ - per_image(m1, N) - xh * per_image(m2, N))
+    return dA * cs * act_grad(act, a)
+
+
+def act_grad(act, a):
+    if act == "lrelu":
+        return torch.where(a > 0, 1.0, SLOPE).double()
+    if act == "relu":
+        return (a > 0).double()
+    return torch.ones_like(a, dtype=torch.float64)
+
+
+
+def act_out64(act, v):
+    return {"none": lambda: v, "tanh": lambda: torch.tanh(v), "sigmoid": lambda: torch.sigmoid(v),
+            "lrelu": lambda: torch.where(v > 0, v, v * SLOPE), "relu": lambda: v.clamp_min(0)}[act]()
+
+
+def act_bound(act, pre, y, bound):
+    """carry an input bound through the activation and its fp32 evaluation (the conv suite's epilogue terms)"""
+    lip = {"none": 1.0, "lrelu": 1.0, "relu": 1.0, "tanh": 1.0, "sigmoid": 0.25}[act]
+    bound = lip * bound + U * y.abs()
+    if act == "tanh":
+        bound = bound + 4 * U * y.abs() + 2.0 ** -126
+    if act == "sigmoid":
+        bound = bound + U * (2 + 2 * pre.abs()) / 4 + 2 * U * y.abs()
+    return bound
+
+
+
+
+def chain_geom(c):
+    return _lib.ConvGeom(c.N, c.H, c.W, c.C, c.K, c.R, c.R, c.stride, 1, 1, 1, 1, _lib.PAD_ZERO, 1, 0, c.P, c.Q)

@@ -13,6 +13,8 @@ table to the kernel source.
 """
 from dataclasses import dataclass, field
 
+import torch
+
 MAX_CLASSES = 32
 BWD_MAX_ELEMS = 12284       # N * n floats of dz beside the kernel's 16 bytes of static shared memory: 48 KB
 CE_MAX_CLASSES = 1024
@@ -114,3 +116,37 @@ CASES = [
     _c("null_gout", "ce", (8, 10), dict(refused_by=("bwd",), null="gout"), error=True, why="gout NULL"),
     _c("null_dx", "ce", (8, 10), dict(refused_by=("bwd",), null="dx"), error=True, why="dx NULL"),
 ]
+
+
+# ---- fp64 references (device-agnostic: tests/test_cpu_class_head.py holds them to torch float64 autograd) ------------
+def head_ref(x, w, b):
+    """softmax(x w^T + b) over dim 1, and the logits"""
+    z = x.double() @ w.double().t() + (0 if b is None else b.double())
+    return torch.softmax(z, 1), z
+
+
+def head_grad_ref(x, w, y, dy):
+    """(dx, dw, db, dz) of Linear + Softmax from the saved output y: dz = y (dy - sum_i y_i dy_i)"""
+    y, dy = y.double(), dy.double()
+    dz = y * (dy - (y * dy).sum(1, keepdim=True))
+    return dz @ w.double(), dz.t() @ x.double(), dz.sum(0), dz
+
+
+def ce_ref(x, target, ignore_index):
+    """CrossEntropyLoss(reduction='mean', ignore_index) over the in-range targets, and the count of rows not ignored"""
+    x = x.double()
+    keep = target != ignore_index
+    lse = torch.logsumexp(x, 1)
+    t = target.clamp(0, x.shape[1] - 1)
+    terms = torch.where(keep, lse - x.gather(1, t[:, None])[:, 0], torch.zeros_like(lse))
+    count = int(keep.sum().item())
+    return terms.sum() / count if count else torch.tensor(float("nan"), dtype=torch.float64), terms, count
+
+
+def ce_grad_ref(x, target, ignore_index, gout, count):
+    """gout / count (softmax(x) - onehot(target)), zero rows where ignored"""
+    x = x.double()
+    p = torch.softmax(x, 1)
+    hit = torch.arange(x.shape[1], device=x.device) == target[:, None]
+    d = (p - hit.double()) * (gout / count)
+    return torch.where((target != ignore_index)[:, None], d, torch.zeros_like(d))

@@ -9,7 +9,10 @@ mlp_critic.cu and holds REGISTERS and GRID to ptxas.
 
 tests/test_gpu_critic_conformance.py runs every case against torch float64.
 """
+import math
 from dataclasses import dataclass
+
+import torch
 
 NUM_SMS = 132
 REGISTERS = {"mlp_critic_fwd_kernel": 39, "mlp_critic_bwd_kernel": 48, "mlp_critic_dbwd_kernel": 64,
@@ -138,3 +141,164 @@ CASES = [
     _c("zero_dims", "step", 33, 0, 33, 31, error=True, why="Din = 0 is refused"),
     _c("no_ws", "step", 33, 31, 33, 31, no_ws=True, error=True, why="no workspace is refused"),
 ]
+
+
+
+# ---- fp64 references with their bounds (device-agnostic: tests/test_cpu_kernel_coverage.py holds them to autograd) ---
+U = 2.0 ** -23
+
+
+def mm(A, eA, B, eB, n):
+    """A @ B in fp64, the bound of an fp32 evaluation with chains of n terms from operands off by eA, eB, and the
+    mean magnitude of one term of the sum"""
+    S = A.abs() @ B.abs()
+    return A @ B, U * (n + 4) * S + eA @ B.abs() + A.abs() @ eB, S / max(A.shape[-1], 1)
+
+
+def mask(h, slope):
+    return torch.where(h > 0, torch.ones_like(h), torch.full_like(h, slope))
+
+
+def z(t):
+    return torch.zeros_like(t)
+
+
+def rowdot_n(K):
+    return math.ceil(K / 32) + 5
+
+
+def critic_fwd_ref(x, W1, b1, W2, b2, W3, b3, slope, m1=None, m2=None):
+    """h1, m1, a1, h2, m2, a2, out; each layer from the previous layer's (given) masks; with bounds of h1, h2, out"""
+    r = {}
+    h1, e1, _ = mm(x, z(x), W1.t(), z(W1).t(), x.shape[1] + 1)
+    r["h1"], r["eh1"] = h1 + b1, e1 + U * 5 * b1.abs()
+    r["m1"] = mask(r["h1"], slope) if m1 is None else m1
+    r["a1"] = r["h1"] * r["m1"]
+    h2, e2, _ = mm(r["a1"], z(r["a1"]), W2.t(), z(W2).t(), W2.shape[1] + 1)
+    r["h2"], r["eh2"] = h2 + b2, e2 + U * 5 * b2.abs()
+    r["m2"] = mask(r["h2"], slope) if m2 is None else m2
+    r["a2"] = r["h2"] * r["m2"]
+    out, eo, _ = mm(r["a2"], z(r["a2"]), W3.t(), z(W3).t(), rowdot_n(W3.shape[1]) + 1)
+    r["out"], r["eout"] = out.reshape(-1) + b3, eo.reshape(-1) + U * 5 * b3.abs()
+    return r
+
+
+def critic_bwd_ref(dout, x, W1, W2, W3, m1, a1, m2, a2):
+    N = x.shape[0]
+    d = dout.reshape(-1, 1)
+    U2 = d * W3.reshape(1, -1) * m2
+    eU2 = 2 * U * U2.abs()
+    r = {"U2": (U2, eU2)}
+    r["dW3"] = tuple(v.reshape(1, -1) for v in mm(a2.t(), z(a2).t(), d, z(d), N))
+    r["db3"] = (d.sum().reshape(1), U * (N + 4) * d.abs().sum().reshape(1))
+    r["dW2"] = mm(U2.t(), eU2.t(), a1, z(a1), N)
+    v, e, _ = mm(U2, eU2, W2, z(W2), W2.shape[0])
+    U1 = v * m1
+    eU1 = e * m1.abs() + U * U1.abs()
+    r["U1"] = (U1, eU1)
+    r["db2"] = (U2.sum(0), U * (N + 4) * U2.abs().sum(0) + eU2.sum(0))
+    r["dW1"] = mm(U1.t(), eU1.t(), x, z(x), N)
+    r["dx"] = mm(U1, eU1, W1, z(W1), W1.shape[0])
+    r["db1"] = (U1.sum(0), U * (N + 4) * U1.abs().sum(0) + eU1.sum(0))
+    return r
+
+
+def critic_dbwd_ref(u, dout, U1, U2, m1, m2, W1, W2, W3):
+    N = u.shape[0]
+    r = {"dW1": mm(U1.t(), z(U1).t(), u, z(u), N)}
+    v, e, _ = mm(u, z(u), W1.t(), z(W1).t(), W1.shape[1])
+    t, et = v * m1, e * m1.abs() + U * (v * m1).abs()
+    r["dW2"] = mm(U2.t(), z(U2).t(), t, et, N)
+    v, e, _ = mm(t, et, W2.t(), z(W2).t(), W2.shape[1])
+    s, es = v * m2, e * m2.abs() + U * (v * m2).abs()
+    d = dout.reshape(-1, 1)
+    r["dW3"] = tuple(v.reshape(1, -1) for v in mm(s.t(), es.t(), d, z(d), N))
+    r["ddout"] = tuple(v.reshape(-1) for v in mm(s, es, W3.reshape(-1, 1), z(W3).reshape(-1, 1), rowdot_n(s.shape[1])))
+    r["t"], r["s"] = (t, et), (s, es)
+    return r
+
+
+def critic_step_ref(real, fake, alpha, W1, b1, W2, b2, W3, b3, slope, lam, M1=None, M2=None):
+    """the critic iteration: losses [d_loss, lambda * gp] and the gradient of d_loss w.r.t. every parameter, each as
+    (value, bound); M1 / M2 [3N][H]: the masks of the stacked rows (None: the fp64 signs)"""
+    N, Din = real.shape
+    R = 3 * N
+    a = alpha.reshape(-1, 1)
+    X = torch.cat([real, fake, a * real + (1 - a) * fake])
+    eX = torch.cat([z(real), z(fake), 3 * U * (a.abs() * real.abs() + (1 - a).abs() * fake.abs())])
+    f = critic_fwd_ref(X, W1, b1, W2, b2, W3, b3, slope, M1, M2)
+    M1, M2 = f["m1"], f["m2"]
+    eh1 = f["eh1"] + eX @ W1.abs().t()
+    ea1 = eh1 * M1.abs() + U * f["a1"].abs()
+    eh2 = f["eh2"] + ea1 @ W2.abs().t()
+    ea2 = eh2 * M2.abs() + U * f["a2"].abs()
+    eout = f["eout"] + (ea2 @ W3.abs().t()).reshape(-1)
+    r = {"h1": (f["h1"], eh1), "h2": (f["h2"], eh2), "M1": M1, "M2": M2}
+    # dout = (-1/N, +1/N, 1) per row group, as the kernel forms it in fp32
+    dout = torch.cat([torch.full((N,), -1.0 / N), torch.full((N,), 1.0 / N), torch.ones(N)])
+    dout = dout.float().double().to(real.device).reshape(-1, 1)
+    out = f["out"][:2 * N]
+    wterms = out * dout[:2 * N, 0]
+    U2 = dout * W3.reshape(1, -1) * M2
+    eU2 = 2 * U * U2.abs()
+    v, e, _ = mm(U2, eU2, W2, z(W2), W2.shape[0])
+    U1, eU1 = v * M1, e * M1.abs() + U * (v * M1).abs()
+    g1, eg1 = U1[2 * N:], eU1[2 * N:]
+    gx, egx, _ = mm(g1, eg1, W1, z(W1), W1.shape[0])
+    s = (gx * gx).sum(1)
+    es = U * (rowdot_n(Din) + 4) * s + 2 * (gx.abs() * egx).sum(1)
+    rn = torch.sqrt(s)
+    pos = rn > 0
+    safe = torch.where(pos, rn, torch.ones_like(rn))
+    er = torch.where(pos, es / (2 * safe) + U * rn, torch.zeros_like(rn))
+    k = lam * 2.0 / N
+    coef = torch.where(pos, k * (rn - 1) / safe, torch.zeros_like(rn))
+    ecoef = torch.where(pos, abs(k) * er / (safe * safe) + 4 * U * coef.abs(), torch.zeros_like(rn))
+    pterms = lam * (rn - 1) ** 2 / N
+    epterms = abs(lam) / N * 2 * (rn - 1).abs() * er + 4 * U * pterms
+    gp = pterms.sum()
+    egp = epterms.sum() + U * (N + 4) * pterms.abs().sum()
+    ew = (eout[:2 * N] * dout[:2 * N, 0].abs()).sum() + 2 * U * wterms.abs().sum()
+    loss = wterms.sum() + gp
+    eloss = ew + egp + U * (3 * N + 4) * (wterms.abs().sum() + pterms.abs().sum())
+    r["losses"] = (torch.stack([loss, gp]), torch.stack([eloss, egp]))
+    c = coef.reshape(-1, 1)
+    ec = ecoef.reshape(-1, 1)
+    g1s = c * g1
+    eg1s = c.abs() * eg1 + ec * g1.abs() + U * g1s.abs()
+    Ucat, eUcat = torch.cat([U1[:2 * N], g1s]), torch.cat([eU1[:2 * N], eg1s])
+    Xcat, eXcat = torch.cat([X[:2 * N], gx]), torch.cat([z(X[:2 * N]), egx])
+    r["dW1"] = mm(Ucat.t(), eUcat.t(), Xcat, eXcat, R)
+    acc, eacc, _ = mm(gx, egx, W1.t(), z(W1).t(), Din)
+    Mp = M1[2 * N:]
+    t = acc * c * Mp
+    et = (eacc * c.abs() + acc.abs() * ec) * Mp.abs() + 2 * U * t.abs()
+    A1cat, eA1cat = torch.cat([f["a1"][:2 * N], t]), torch.cat([ea1[:2 * N], et])
+    r["dW2"] = mm(U2.t(), eU2.t(), A1cat, eA1cat, R)
+    v, e, _ = mm(t, et, W2.t(), z(W2).t(), W2.shape[1])
+    sp, esp = v * M2[2 * N:], e * M2[2 * N:].abs() + U * (v * M2[2 * N:]).abs()
+    A2cat, eA2cat = torch.cat([f["a2"][:2 * N], sp]), torch.cat([ea2[:2 * N], esp])
+    r["dW3"] = tuple(v.reshape(1, -1) for v in mm(A2cat.t(), eA2cat.t(), dout, z(dout), R))
+    r["db1"] = (U1[:2 * N].sum(0), U * (2 * N + 4) * U1[:2 * N].abs().sum(0) + eU1[:2 * N].sum(0))
+    r["db2"] = (U2[:2 * N].sum(0), U * (2 * N + 4) * U2[:2 * N].abs().sum(0) + eU2[:2 * N].sum(0))
+    r["db3"] = (dout[:2 * N].sum().reshape(1), U * (2 * N + 4) * dout[:2 * N].abs().sum().reshape(1))
+    r["coef"], r["ecoef"] = coef, ecoef
+    # the workspace rows the kernel's last GEMMs read: U1 (penalty rows scaled), X3 (penalty rows gx), U2, A1
+    # (penalty rows t), A2 (penalty rows (t W2^T) * m2)
+    r["ws"] = {"U1": (Ucat, eUcat), "X3": (Xcat, eXcat), "U2": (U2, eU2), "A1": (A1cat, eA1cat), "A2": (A2cat, eA2cat)}
+    r["dout"] = dout
+    return r
+
+
+F32 = torch.float32
+
+
+def check_mask(what, m, h, eh, slope):
+    """the kernel's mask equals the fp64 sign of h wherever |h| exceeds its bound, and is 1 or slope everywhere"""
+    m = m.double().view_as(h)
+    ok = (m == 1) | (m == torch.tensor(slope, dtype=F32).item())
+    assert ok.all(), f"{what}: mask value {m[~ok][0].item()} is neither 1 nor the slope"
+    sure = h.abs() > eh
+    bad = sure & (m != mask(h, torch.tensor(slope, dtype=F32).item()))
+    assert not bad.any(), f"{what}: mask differs from the sign of h at {tuple(bad.nonzero()[0].tolist())}, " \
+                          f"h {h[bad][0].item():.3e}, bound {eh[bad][0].item():.3e}"

@@ -9,7 +9,10 @@ REGISTERS and GRID to ptxas, and the fp64 references to torch float64 autograd.
 
 tests/test_gpu_mlp_generator_conformance.py runs every case against its fp64 reference.
 """
+import math
 from dataclasses import dataclass
+
+import torch
 
 NUM_SMS = 132
 REGISTERS = {"mlp_gen_fwd_kernel": 48, "mlp_gen_bwd_kernel": 80}
@@ -112,3 +115,136 @@ CASES = [
     _c("wide", "bwd", 8, (31, MAX_WIDTH + 1, 17), (1,), error=True, why="a width over the limit is refused"),
     _c("no_ws", "bwd", 33, SMALL, (1, 1), no_ws=True, error=True, why="no workspace is refused"),
 ]
+
+
+# ---- inputs and fp64 references (device-agnostic: tests/test_cpu_mlp_generator.py holds them to autograd) ----------
+U = 2.0 ** -23
+EPS, MOMENTUM = 0.8, 0.1     # BatchNorm1d(o, 0.8) of wgan_gp.py:49 / gan.py:45, torch's default momentum
+F32 = torch.float32
+
+
+def f32(v):
+    return torch.tensor(v, dtype=F32).item()
+
+
+def make(c, seed=0):
+    """the case's fp32 inputs on the CPU: z, W{l}, b{l}, and per norm layer gamma, beta, rm, rv, nbt; dout"""
+    g = torch.Generator().manual_seed(seed)
+    rn = lambda *s, scale=1.0: torch.randn(*s, generator=g) * scale  # noqa: E731
+    N, w = max(c.N, 1), c.widths
+    P = {"z": rn(N, w[0])}
+    for l in range(c.L):
+        P[f"W{l}"] = rn(w[l + 1], w[l], scale=1 / math.sqrt(w[l]))
+        P[f"b{l}"] = rn(w[l + 1], scale=0.2)
+        if c.has_norm[l]:
+            P[f"gamma{l}"] = 1 + rn(w[l + 1], scale=0.2)
+            P[f"beta{l}"] = rn(w[l + 1], scale=0.2)
+            P[f"rm{l}"] = rn(w[l + 1], scale=0.1)
+            P[f"rv{l}"] = 1 + torch.rand(w[l + 1], generator=g)
+            P[f"nbt{l}"] = torch.tensor([7], dtype=torch.int64)
+    P["dout"] = rn(N, w[-1])
+    return P
+
+
+def mask(a, slope):
+    return torch.where(a > 0, torch.ones_like(a), torch.full_like(a, slope))
+
+
+def gen_fwd_ref(P, c, acts=None):
+    """fp64 forward of case c from its (fp32) inputs P.  Per layer: x (the layer's input), h, and for a norm layer mean,
+    var, rstd, xhat, the updated running statistics; y, a; and out.  acts: the kernel's activations, each layer then
+    starts from the kernel's previous layer."""
+    D = {k: v.double() for k, v in P.items() if v.is_floating_point()}
+    slope, N = f32(c.slope), D["z"].shape[0]
+    x, layers = D["z"], []
+    for l in range(c.L):
+        r = {"x": x, "h": x @ D[f"W{l}"].t() + D[f"b{l}"]}
+        if l == c.L - 1:
+            r["out"] = torch.tanh(r["h"])
+        else:
+            y = r["h"]
+            if c.has_norm[l]:
+                mean = y.mean(0)
+                var = ((y - mean) ** 2).mean(0)
+                r.update(mean=mean, var=var, rstd=1 / torch.sqrt(var + f32(EPS)))
+                r["xhat"] = (y - mean) * r["rstd"]
+                y = r["xhat"] * D[f"gamma{l}"] + D[f"beta{l}"]
+                m = f32(MOMENTUM)
+                r["rm"] = (1 - m) * D[f"rm{l}"] + m * mean
+                r["rv"] = (1 - m) * D[f"rv{l}"] + m * var * N / (N - 1)
+            r["y"], r["a"] = y, y * mask(y, slope)
+            x = r["a"] if acts is None or acts[l] is None else acts[l].double()
+        layers.append(r)
+    return layers
+
+
+def saved_of(c, layers):
+    """the saved region (include/b200gan.h: a_l, then xhat and rstd of each norm layer) from a forward's layers"""
+    hid = [layers[l] for l in range(c.L - 1)]
+    parts = [r["a"] for r in hid] + [r["xhat"] for r, n in zip(hid, c.has_norm) if n] + \
+        [r["rstd"] for r, n in zip(hid, c.has_norm) if n]
+    return torch.cat([p.reshape(-1) for p in parts]) if parts else torch.zeros(0, dtype=torch.float64)
+
+
+def split_saved(c, saved, N):
+    """saved -> (acts, xhats, rstds), per hidden layer (None for layers without a norm)"""
+    w, o = c.widths, 0
+    acts, xh, rs = [], [None] * (c.L - 1), [None] * (c.L - 1)
+    for l in range(c.L - 1):
+        acts.append(saved[o:o + N * w[l + 1]].view(N, w[l + 1]))
+        o += N * w[l + 1]
+    for l in range(c.L - 1):
+        if c.has_norm[l]:
+            xh[l] = saved[o:o + N * w[l + 1]].view(N, w[l + 1])
+            o += N * w[l + 1]
+    for l in range(c.L - 1):
+        if c.has_norm[l]:
+            rs[l] = saved[o:o + w[l + 1]]
+            o += w[l + 1]
+    return acts, xh, rs
+
+
+def mmr(A, eA, B, n):
+    """A @ B in fp64 for an operand A off by eA and an exact B: the bound of the fp32 GEMM's own rounding, plus the
+    operand errors carried as independent ones (root-sum-square); and the mean magnitude of one term"""
+    S = A.abs() @ B.abs()
+    return A @ B, U * (n + 4) * S + torch.sqrt((eA * eA) @ (B * B)), S / max(A.shape[-1], 1)
+
+
+def rss(e, dim=0):
+    return torch.sqrt((e * e).sum(dim))
+
+
+def gen_bwd_ref(c, dout, out, z_, W, gamma, acts, xhat, rstd):
+    """fp64 backward for dout with bounds: name -> (value, bound[, mean magnitude of one term]) for dz, dW{l}, db{l},
+    dgamma{l}, dbeta{l}; every operand but the gradient itself is exact (the kernel reads the same fp32 values).  The
+    gradient's own error is carried from layer to layer as independent per-element errors (mmr, rss): the worst case of
+    correlated errors grows by the row sums of |W| per layer and is vacuous after five layers.  Each carried bound is
+    itself a worst case of its layer's rounding, far above the error a kernel makes."""
+    slope, N = f32(c.slope), dout.shape[0]
+    g = dout * (1 - out * out)
+    eg = U * (3 * g.abs() + 2 * dout.abs() * out * out)
+    r = {}
+    for l in range(c.L - 1, -1, -1):
+        ain = z_ if l == 0 else acts[l - 1]
+        r[f"dW{l}"] = mmr(g.t(), eg.t(), ain, N)
+        r[f"db{l}"] = (g.sum(0), U * (N + 4) * g.abs().sum(0) + rss(eg))
+        da, eda, _ = mmr(g, eg, W[l], W[l].shape[0])
+        if l == 0:
+            r["dz"] = (da, eda)
+            break
+        mk = mask(ain, slope)
+        dy, edy = da * mk, eda * mk.abs() + U * (da * mk).abs()
+        if c.has_norm[l - 1]:
+            xh, k = xhat[l - 1], gamma[l - 1] * rstd[l - 1]
+            s1, s2 = dy.sum(0), (dy * xh).sum(0)
+            es1 = U * (N + 4) * dy.abs().sum(0) + rss(edy)
+            es2 = U * (N + 4) * (dy * xh).abs().sum(0) + rss(edy * xh)
+            r[f"dbeta{l - 1}"], r[f"dgamma{l - 1}"] = (s1, es1), (s2, es2)
+            inner = dy - s1 / N - xh * s2 / N
+            g = k * inner
+            eg = k.abs() * (edy + es1 / N + xh.abs() * es2 / N
+                            + 6 * U * (dy.abs() + (s1 / N).abs() + (xh * s2 / N).abs())) + 2 * U * g.abs()
+        else:
+            g, eg = dy, edy
+    return r

@@ -8,9 +8,17 @@ of at most 256 groups in gridDim.z.  Written from the launchers in pytorch-gan_b
 tests/test_cpu_norm_case_table.py checks it against the kernels the source declares and launches;
 tests/test_gpu_norm_conformance.py runs every case against torch float64.
 """
+import ctypes
 from dataclasses import dataclass
 
+import torch
+
+from b200gan import _lib
+from conformance import Arena
+
 ACTS = ("none", "lrelu", "relu", "tanh", "sigmoid")
+KERNELS = {"norm_stats_kernel", "norm_finalize_kernel", "norm_apply_kernel", "norm_bwd_reduce_kernel",
+           "norm_bwd_apply_kernel", "norm_bwd_params_kernel"}     # what norm.cu declares
 
 
 @dataclass(frozen=True)
@@ -65,3 +73,110 @@ class Case:
 
 # every geometry with every activation; round_tf32 alternates so that each activation runs with it on and off
 CASES = tuple(Case(g, a, (i + j) % 2 == 1) for i, g in enumerate(GEOMS) for j, a in enumerate(ACTS))
+
+
+# ---- runs and references -------------------------------------------------------------------------------------------
+SLOPE = 0.2
+MOMENTUM = 0.1
+NBT0 = 7
+ACT_CODE = {"none": _lib.ACT_NONE, "lrelu": _lib.ACT_LRELU, "relu": _lib.ACT_RELU, "tanh": _lib.ACT_TANH,
+            "sigmoid": _lib.ACT_SIGMOID}
+
+
+class Run:
+    """one case on guarded buffers: stats -> finalize -> apply, then the backward"""
+
+    def __init__(self, case, seed=0):
+        self.c, g = case, case.geom
+        self.lib = _lib.load()
+        self.G = g.N * g.C if g.per_sample else g.C
+        self.numel = g.N * g.H * g.W * g.C
+        self.eps = 1e-5 if g.per_sample else 0.8
+        gen = torch.Generator().manual_seed(seed)
+        self.x = (torch.randn(g.N, g.H * g.W, g.C, generator=gen) * 2 + 0.5).cuda()
+        self.dy = torch.randn(g.N, g.H * g.W, g.C, generator=gen).cuda()
+        self.gamma = (1 + 0.5 * torch.randn(g.C, generator=gen)).cuda()
+        self.beta = (0.3 * torch.randn(g.C, generator=gen)).cuda()
+        self.rm0 = (0.1 * torch.randn(g.C, generator=gen)).cuda()
+        self.rv0 = (1 + torch.rand(g.C, generator=gen)).cuda()
+        f32, f64 = torch.float32, torch.float64
+        specs = [("x", self.numel + g.offset, f32, "in"), ("dy", self.numel, f32, "in"),
+                 ("y", self.numel, f32, "out"), ("mean_rstd", 2 * self.G, f32, "out"),
+                 ("scale_shift", 2 * self.G, f32, "out"), ("dx", self.numel, f32, "out"),
+                 ("stats", 2 * self.G, f64, "ws"), ("sums", 2 * self.G, f64, "ws")]
+        if g.affine:
+            specs += [("gamma", g.C, f32, "in"), ("beta", g.C, f32, "in"), ("dgb", 2 * self.G, f32, "out")]
+        if not g.per_sample:
+            specs += [("running_mean", g.C, f32, "ws"), ("running_var", g.C, f32, "ws"), ("nbt", 1, torch.int64, "in")]
+        self.arena = Arena(specs)
+        lead = torch.full((g.offset,), float("nan"), device="cuda")
+        self.data = dict(x=torch.cat([lead, self.x.reshape(-1)]), dy=self.dy, gamma=self.gamma, beta=self.beta,
+                         nbt=torch.tensor([NBT0], device="cuda"))
+        self.d = _lib.NormDesc(g.N, g.H * g.W, g.C, int(g.per_sample), self.eps, MOMENTUM, ACT_CODE[case.act], SLOPE,
+                               int(case.rtf))
+
+    def prepare(self):
+        a = self.arena
+        a.prepare(self.data)
+        a.t["stats"].zero_()
+        a.t["sums"].zero_()
+        if "running_mean" in a.t:
+            a.t["running_mean"].copy_(self.rm0)
+            a.t["running_var"].copy_(self.rv0)
+
+    def ptr(self, name):
+        p = self.arena.ptr(name)
+        return p + 4 * self.c.geom.offset if name == "x" else p
+
+    def outputs(self):
+        return self.arena.outputs()
+
+    def call(self, st):
+        """forward then backward on stream st; the first failing return code, or 0"""
+        lib, d, p, act = self.lib, ctypes.byref(self.d), self.ptr, self.c.act
+        for rc in (lambda: lib.b200gan_norm_stats(d, p("x"), p("stats"), st),
+                   lambda: lib.b200gan_norm_finalize(d, p("stats"), p("gamma"), p("beta"), p("mean_rstd"),
+                                                     p("scale_shift"), p("running_mean"), p("running_var"), p("nbt"),
+                                                     st),
+                   lambda: lib.b200gan_norm_apply(d, p("x"), p("scale_shift"), p("y"), st),
+                   lambda: lib.b200gan_norm_bwd(d, p("dy"), p("x"), p("y") if act in ("tanh", "sigmoid") else None,
+                                                p("mean_rstd"), p("scale_shift") if act in ("lrelu", "relu") else None,
+                                                p("gamma"), p("sums"), p("dx"), p("dgb"), st)):
+            code = rc()
+            if code:
+                return code
+        return 0
+
+
+def mask(act, pre):
+    if act == "lrelu":
+        return torch.where(pre > 0, torch.ones_like(pre), torch.full_like(pre, SLOPE))
+    if act == "relu":
+        return (pre > 0).to(pre.dtype)
+    return torch.ones_like(pre)
+
+
+def closed_form(x, dy, gamma, beta, u, ugamma, ubeta, eps, act, per_sample, ap=None):
+    """(dL/d(dy), dL/dx, dL/d(gamma) per channel or None) on NCHW tensors, any dtype; gamma/beta None = non-affine,
+    ugamma/ubeta None = 0; ap: the activation's mask, else computed from the normalised x"""
+    n, c = x.shape[:2]
+    dims = (2, 3) if per_sample else (0, 2, 3)
+    m = x[0, 0].numel() * (1 if per_sample else n)
+    ch = (1, c, 1, 1)
+    mean = x.mean(dims, keepdim=True)
+    r = 1 / torch.sqrt(((x - mean) ** 2).mean(dims, keepdim=True) + eps)
+    xh = (x - mean) * r
+    ga = gamma.view(ch) if gamma is not None else 1.0
+    be = beta.view(ch) if beta is not None else 0.0
+    ap = mask(act, ga * xh + be) if ap is None else ap
+    g = dy * ap
+    A, B = g.sum(dims, keepdim=True) / m, (g * xh).sum(dims, keepdim=True) / m
+    U, T, Q = u.sum(dims, keepdim=True), (u * xh).sum(dims, keepdim=True), (u * g).sum(dims, keepdim=True)
+    ug = ugamma.view(ch) if ugamma is not None else 0.0
+    ub = ubeta.view(ch) if ubeta is not None else 0.0
+    gdy = ap * (ga * r * (u - U / m - xh * T / m) + ug * xh + ub)
+    gx = ug * r * (g - A - xh * B) - (ga * r * r / m) * (xh * (Q - A * U - 3 * B * T) + T * (g - A) + B * (m * u - U))
+    ggamma = None
+    if gamma is not None:
+        ggamma = (r * (Q - A * U - B * T)).sum(0).view(c)
+    return gdy, gx, ggamma

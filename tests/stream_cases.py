@@ -9,7 +9,11 @@ and adam_multi's ADAM_CHUNK blocks per tensor in launches of at most ADAM_MAX_TE
 tests/test_cpu_kernel_coverage.py holds the kernel names to the sources; tests/test_gpu_stream_conformance.py runs
 every case against torch float64 (bit for bit where the kernel only moves data).
 """
+import math
 from dataclasses import dataclass, field
+
+import torch
+import torch.nn.functional as F
 
 NUM_SMS = 132
 ADAM_CHUNK = 256 * 16
@@ -190,3 +194,90 @@ CASES = [
        why="a NULL pointer in the second launch's tensors is refused before the first launch runs"),
     _c("count_neg", "adam", (-1,), error=True, why="count < 0 is refused"),
 ]
+
+
+
+# ---- fp64 references (device-agnostic: tests/test_cpu_kernel_coverage.py holds them to stock torch) -----------------
+U = 2.0 ** -23
+SLOPE = 0.2
+ADAM = dict(lr=2e-4, b1=0.5, b2=0.999, eps=1e-8)   # dcgan.py:134-135
+F32 = torch.float32
+
+
+def bce_ref(v, t):
+    """torch.nn.BCELoss(): mean of -(t log v + (1 - t) log(1 - v)), logs clamped at -100; and its terms"""
+    v, t = v.double(), t.double()
+    lp, lq = torch.log(v).clamp_min(-100), torch.log1p(-v).clamp_min(-100)
+    terms = (t - 1) * lq - t * lp
+    return terms.mean(), terms, lp, lq
+
+
+def bce_grad_ref(v, t, gout):
+    """d loss / d v = gout / n * (v - t) / max((1 - v) v, 1e-12) (the clamp of torch's binary_cross_entropy_backward)"""
+    v, t = v.double(), t.double()
+    eps = torch.tensor(1e-12, dtype=F32).item()
+    return gout / v.numel() * (v - t) / ((1 - v) * v).clamp_min(eps)
+
+
+def pad_ref(x_nhwc, pads, mode):
+    t, l, b, r = pads
+    y = F.pad(x_nhwc.permute(0, 3, 1, 2), (l, r, t, b), mode="reflect" if mode == "reflect" else "constant")
+    return y.permute(0, 2, 3, 1)
+
+
+def pad_grad_ref(dy_nhwc, xshape, pads, mode):
+    x = torch.zeros(xshape, dtype=dy_nhwc.dtype, device=dy_nhwc.device, requires_grad=True)
+    (g,) = torch.autograd.grad(pad_ref(x, pads, mode), x, dy_nhwc)
+    return g
+
+
+def upsample_ref(x_nhwc):
+    return x_nhwc.repeat_interleave(2, 1).repeat_interleave(2, 2)
+
+
+def upsample_grad_ref(dy_nhwc):
+    N, H2, W2, C = dy_nhwc.shape
+    return dy_nhwc.reshape(N, H2 // 2, 2, W2 // 2, 2, C).sum((2, 4))
+
+
+def adam_consts(step0, lr=ADAM["lr"], b1=ADAM["b1"], b2=ADAM["b2"], eps=ADAM["eps"]):
+    """the kernel's fp32 casts of the Python-double terms of _single_tensor_adam, as doubles"""
+    f = lambda v: torch.tensor(v, dtype=F32).item()
+    t = step0 + 1.0
+    return dict(nss=f(-(lr / (1.0 - b1 ** t))), bc2=f(math.sqrt(1.0 - b2 ** t)), b1=f(b1), omb1=f(1.0 - b1), b2=f(b2),
+                omb2=f(1.0 - b2), eps=f(eps))
+
+
+def adam_ref(p, g, m, v, step0, gscale=1.0):
+    """one Adam step in fp64 on the kernel's constants; returns p, m, v and their bounds (roundings per step:
+    m 2, v 3, the denominator 3 (sqrt, divide, add), the update 3 (divide, multiply, add))"""
+    k = adam_consts(step0)
+    p, g, m, v = p.double(), g.double() * gscale, m.double(), v.double()
+    m1 = k["b1"] * m + k["omb1"] * g
+    v1 = k["b2"] * v + k["omb2"] * g * g
+    sq = torch.sqrt(v1)
+    den = sq / k["bc2"] + k["eps"]
+    p1 = p + k["nss"] * (m1 / den)
+    em = 2 * U * (k["b1"] * m.abs() + k["omb1"] * g.abs())
+    ev = 3 * U * (k["b2"] * v.abs() + k["omb2"] * g * g)
+    eden = torch.where(sq > 0, ev / (2 * sq.clamp_min(1e-300)), ev.sqrt()) / k["bc2"] + 3 * U * den
+    ep = abs(k["nss"]) * (em / den + m1.abs() * eden / (den * den) + 2 * U * m1.abs() / den) + U * p1.abs()
+    return (p1, ep), (m1, em), (v1, ev)
+
+
+def act64(name, v):
+    return {"none": lambda: v, "lrelu": lambda: torch.where(v > 0, v, v * SLOPE), "relu": lambda: v.clamp_min(0),
+            "tanh": lambda: torch.tanh(v), "sigmoid": lambda: torch.sigmoid(v)}[name]()
+
+
+def act32_exact(name, x):
+    """none / LeakyReLU / ReLU in fp32, as apply_act evaluates them"""
+    return {"none": lambda: x, "lrelu": lambda: torch.where(x > 0, x, x * SLOPE),
+            "relu": lambda: x.clamp_min(0)}[name]()
+
+
+def grad32_exact(name, y):
+    """act_grad_from_out of none / LeakyReLU / ReLU in fp32"""
+    one = torch.ones_like(y)
+    return {"none": lambda: one, "lrelu": lambda: torch.where(y > 0, one, one * SLOPE),
+            "relu": lambda: (y > 0).to(y.dtype)}[name]()

@@ -10,6 +10,11 @@ tests/test_gpu_fused_conformance.py runs every case against torch float64.
 """
 from dataclasses import dataclass
 
+import torch
+
+from chain_cases import NEG_SLOPE, SLOPE, act_out64, conv_dgrad, conv_fwd, conv_wgrad
+from conformance import tf32_rna
+
 ACT_MID = ("none", "lrelu", "relu")
 ACT_OUT = ("none", "tanh", "sigmoid")
 
@@ -62,3 +67,59 @@ CASES = [
     _c("k4", 2, 64, 4, 8, 16, error=True, why="K = 4 > 3"),
     _c("mid_tanh", 2, 64, 1, 8, 16, act_mid="tanh", error=True, why="act_mid must be none, LeakyReLU or ReLU"),
 ]
+
+
+# ---- fp64 references (device-agnostic: tests/test_cpu_fused_case_table.py holds them to stock torch) -----------------
+def act_mid32(act, v):
+    """the tail's LeakyReLU / ReLU in fp32, as the kernel computes it"""
+    if act == "lrelu":
+        return torch.where(v > 0, v, v * SLOPE)
+    if act == "relu":
+        return v.clamp_min(0)
+    return v
+
+def tail_fwd_ref(a, ss, w, bias, act_mid, act_out):
+    """tail.cu forward: operands as the kernel feeds wgmma (RNA TF32); returns out, the linear part and A"""
+    C = a.shape[-1]
+    pre = (a.double() * ss[:C].double() + ss[C:].double()).float()     # fmaf(a, sc, sh)
+    x = tf32_rna(act_mid32(act_mid, pre)).double()
+    wr = tf32_rna(w).double()
+    conv = conv_fwd(x, wr, 1, 1)
+    A = conv_fwd(x.abs(), wr.abs(), 1, 1)
+    b = bias.double() if bias is not None else torch.zeros(w.shape[0], dtype=torch.float64, device=a.device)
+    return act_out64(act_out, conv + b), conv + b, A, b
+
+
+def tail_bwd_ref(a, mr, ss, w, g, act_mid, neg_branch):
+    """tail.cu backward with the activation's derivative on `neg_branch` (bool mask: take the negative side)"""
+    C, K = a.shape[-1], w.shape[0]
+    a64 = a.double()
+    sc, sh, mean, rstd = ss[:C].double(), ss[C:].double(), mr[:C].double(), mr[C:].double()
+    pre = a64 * sc + sh
+    neg = NEG_SLOPE[act_mid]
+    y = torch.where(neg_branch, pre * neg, pre)
+    dy = conv_dgrad(g.double(), w.double(), a.shape, 1, 1)
+    dz = torch.where(neg_branch, dy * neg, dy)
+    xh = (a64 - mean) * rstd
+    total = a.numel() // C
+    s1, s2 = dz.sum((0, 1, 2)), (dz * xh).sum((0, 1, 2))
+    da = sc * (dz - s1 / total - xh * (s2 / total))
+    dw = conv_wgrad(y, g.double(), (K, C, 3, 3), 1, 1)
+    return dict(da=da, s1=s1, s2=s2, dw=dw, db=g.double().sum((0, 1, 2)), y=y, dz=dz, xh=xh, pre=pre, dy=dy)
+
+
+# ---- the modules of the GPU parity tests (test_gpu_tail.py, test_gpu_tail_ranges.py) --------------------------------
+def mods(ns, c, k, mid, out):
+    """Conv2d(8, c) -> BatchNorm2d(c, 0.8) [-> LeakyReLU / ReLU] -> Conv2d(c, k, 3, 1, 1) [-> Tanh / Sigmoid] from the
+    namespace ns"""
+    layers = [ns.Conv2d(8, c, 3, 1, 1), ns.BatchNorm2d(c, 0.8)]
+    if mid == "lrelu":
+        layers.append(ns.LeakyReLU(0.2, inplace=True))
+    elif mid == "relu":
+        layers.append(ns.ReLU(inplace=True))
+    layers.append(ns.Conv2d(c, k, 3, stride=1, padding=1))
+    if out == "tanh":
+        layers.append(ns.Tanh())
+    elif out == "sigmoid":
+        layers.append(ns.Sigmoid())
+    return ns.Sequential(*layers)

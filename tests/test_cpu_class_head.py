@@ -1,35 +1,19 @@
 """The auxiliary-classifier head (Linear(K, n) + Softmax, functional.ClassHeadFn) and CrossEntropyLoss
 (functional.CrossEntropyMeanFn) without a GPU: which calls route to the kernels and which go to the stock forward, the
-Softmax dim=None warning, the class names and the patch, the fp64 references of tests/test_gpu_class_head_conformance.py
-against torch float64 autograd, the case table against csrc/head.cu and ptxas, the rule that every __global__ kernel
-under csrc/ -- in a .cu file or a header, at any depth -- has a case, and tests/scripts/mini_acgan under the launcher on
-the CPU, patched against stock."""
-import glob
+Softmax dim=None warning, the class names and the patch, the fp64 references of tests/class_head_cases.py against torch
+float64 autograd, the case table against csrc/head.cu and ptxas, and tests/scripts/mini_acgan under the launcher on the
+CPU, patched against stock."""
 import os
 import re
-import shutil
-import subprocess
-import tempfile
 import warnings
 
 import pytest
 import torch
 
-import chain_cases as ch
 import class_head_cases as hc
-import conv_cases as cc
-import critic_cases as cr
-import generator_cases as gc
-import norm_cases as nc
 import stream_cases as sc
-import tail_cases as tl
-import test_gpu_class_head_conformance as hcc
-import test_gpu_pixel_loss_conformance as pl
 from b200gan import nn as bnn
-from test_cpu_conv_case_table import CSRC
-from test_cpu_fused_case_table import declared
-from test_cpu_kernel_coverage import COVERED_BY_TEST, table_kernels
-from test_cpu_mlp_discriminator_plan import _functions
+from conformance import CSRC, declared, functions, needs_nvcc, ptxas_report, source
 
 HEAD_CU = os.path.join(CSRC, "head.cu")
 
@@ -266,9 +250,9 @@ def test_head_references_are_torch_float64():
     xx, ww, bb = (t.clone().requires_grad_(True) for t in (x, w, b))
     y = torch.softmax(xx @ ww.t() + bb, 1)
     gx, gw, gb = torch.autograd.grad(y, (xx, ww, bb), dy)
-    y_ref, _ = hcc.head_ref(x, w, b)
+    y_ref, _ = hc.head_ref(x, w, b)
     torch.testing.assert_close(y_ref, y.detach(), rtol=1e-14, atol=1e-16)
-    dx, dw, db, _ = hcc.head_grad_ref(x, w, y.detach(), dy)
+    dx, dw, db, _ = hc.head_grad_ref(x, w, y.detach(), dy)
     for got, want in ((dx, gx), (dw, gw), (db, gb)):
         torch.testing.assert_close(got, want, rtol=1e-12, atol=1e-15)
 
@@ -282,10 +266,10 @@ def test_cross_entropy_references_are_torch_float64(ignore_index):
     xx = x.clone().requires_grad_(True)
     loss = torch.nn.functional.cross_entropy(xx, t, ignore_index=ignore_index)
     gx, = torch.autograd.grad(loss, xx, torch.tensor(1.5, dtype=torch.float64))
-    ref, _, count = hcc.ce_ref(x, t, ignore_index)
+    ref, _, count = hc.ce_ref(x, t, ignore_index)
     assert count == int((t != ignore_index).sum())
     torch.testing.assert_close(ref, loss.detach(), rtol=1e-14, atol=0)
-    torch.testing.assert_close(hcc.ce_grad_ref(x, t, ignore_index, 1.5, count), gx, rtol=1e-12, atol=1e-16)
+    torch.testing.assert_close(hc.ce_grad_ref(x, t, ignore_index, 1.5, count), gx, rtol=1e-12, atol=1e-16)
 
 
 @pytest.fixture
@@ -293,16 +277,16 @@ def stubbed(monkeypatch):
     """the launch wrappers replaced by the fp64 references, so that the autograd nodes run on the CPU"""
     from b200gan import ops
     monkeypatch.setattr(ops, "_require_cuda", lambda *a: None)
-    monkeypatch.setattr(ops, "class_head_fwd", lambda x, w, b: hcc.head_ref(x, w, b)[0])
+    monkeypatch.setattr(ops, "class_head_fwd", lambda x, w, b: hc.head_ref(x, w, b)[0])
     monkeypatch.setattr(ops, "cross_entropy_fwd", lambda x, t, ig: torch.stack(
-        [hcc.ce_ref(x, t, ig)[0], torch.tensor(float(hcc.ce_ref(x, t, ig)[2]), dtype=torch.float64)]).to(x.dtype))
+        [hc.ce_ref(x, t, ig)[0], torch.tensor(float(hc.ce_ref(x, t, ig)[2]), dtype=torch.float64)]).to(x.dtype))
 
     def head_bwd(x, w, y, dy, need_dx, need_db):
-        dx, dw, db, _ = hcc.head_grad_ref(x, w, y, dy)
+        dx, dw, db, _ = hc.head_grad_ref(x, w, y, dy)
         return (dx if need_dx else None), dw, (db if need_db else None)
     monkeypatch.setattr(ops, "class_head_bwd", head_bwd)
     monkeypatch.setattr(ops, "cross_entropy_bwd",
-                        lambda x, t, out, gout, ig: hcc.ce_grad_ref(x, t, ig, gout, out[1]).to(x.dtype))
+                        lambda x, t, out, gout, ig: hc.ce_grad_ref(x, t, ig, gout, out[1]).to(x.dtype))
 
 
 @pytest.mark.parametrize("layout", ["contiguous", "transposed"])
@@ -396,8 +380,8 @@ def test_table_covers_its_edges():
 def test_head_cu_keeps_its_four_kernels_and_the_entry_points_launch_only_theirs():
     assert declared(HEAD_CU) == {k for c in sc.CASES if c.op in ("linear1", "bce") for k in c.kernels} == \
         {k for c in hc.CASES for k in c.kernels}
-    src = re.sub(r"//[^\n]*", "", open(HEAD_CU).read())
-    fns = _functions(src)
+    src = source(HEAD_CU)
+    fns = functions(src)
     want = {"b200gan_class_head_fwd": "linear1_fwd_kernel", "b200gan_class_head_bwd": "linear1_bwd_kernel",
             "b200gan_cross_entropy_fwd": "bce_fwd_kernel", "b200gan_cross_entropy_bwd": "bce_bwd_kernel",
             "b200gan_linear1_fwd": "linear1_fwd_kernel", "b200gan_linear1_bwd": "linear1_bwd_kernel",
@@ -408,34 +392,12 @@ def test_head_cu_keeps_its_four_kernels_and_the_entry_points_launch_only_theirs(
     assert "template" not in src, "head.cu's kernels stay non-template: the traced names are compared exactly"
 
 
-def test_every_kernel_at_any_depth_has_a_case():
-    """every __global__ under csrc/ -- in a .cu file or a .cuh header, in a subdirectory too -- is named by a case table
-    (the class-head table included) or a dedicated test"""
-    found = {k: os.path.relpath(p, CSRC) for ext in ("*.cu", "*.cuh")
-             for p in glob.glob(os.path.join(CSRC, "**", ext), recursive=True) for k in declared(p)}
-    assert "linear1_fwd_kernel" in found and "pixel_loss_fwd_kernel" in found and len(found) > 30
-    covered = set(COVERED_BY_TEST) | {k for c in pl.CASES for k, _ in c.kernels()}
-    for cases in (cc.CASES, ch.CASES, tl.CASES, nc.CASES, cr.CASES, sc.CASES, gc.CASES, hc.CASES):
-        covered |= table_kernels(cases)
-    missing = set(found) - covered
-    assert not missing, f"kernels without a conformance case: {sorted((found[k], k) for k in missing)}"
-
-
-@pytest.mark.skipif(not os.path.exists("/usr/local/cuda/bin/nvcc") and not shutil.which("nvcc"), reason="no nvcc")
+@needs_nvcc
 def test_head_kernels_do_not_spill():
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    if not os.path.exists(nvcc):
-        nvcc = shutil.which("nvcc")
-    import build as b200_build
-    with tempfile.TemporaryDirectory() as d:
-        r = subprocess.run([nvcc, *b200_build.FLAGS, "-Xptxas=-v", "-c", HEAD_CU, "-o", os.path.join(d, "h.o")],
-                           capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-2000:]
-    names = set()
-    for chunk in r.stderr.split("Compiling entry function")[1:]:
-        names.add(re.match(r" '_ZN7b200gan\d+(\w+?)E", chunk).group(1))
-        assert re.search(r"0 bytes stack frame, 0 bytes spill stores, 0 bytes spill loads", chunk), chunk[:400]
-    assert names == declared(HEAD_CU)
+    rep = ptxas_report(HEAD_CU)
+    for name, r in rep.items():
+        assert r["stack"] == r["spills"] == 0, f"{name}: {r}"
+    assert set(rep) == declared(HEAD_CU)
 
 
 # ---- the reference-idiom script on the CPU -----------------------------------------------------------------------------

@@ -2,15 +2,12 @@
 sources declare.  Needs the built library, not a GPU: b200gan_conv2d_supported is host logic."""
 import ctypes
 import os
-import re
 
 import pytest
 
 import conv_cases as cc
 from b200gan import _lib
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, "pytorch-gan_b200", "csrc")
+from conformance import CSRC, declared
 
 
 def geom(c):
@@ -43,23 +40,17 @@ def test_tc_support_matches_table(case):
     assert case.pas == cc.FPROP or not case.epi
 
 
-def declared_kernels(path, only=None):
-    src = re.sub(r"//[^\n]*", "", open(path).read())
-    names = set(re.findall(r"__global__\s+void\s+(?:__launch_bounds__\([^)]*\)\s*)?(\w+)\s*\(", src))
-    return names if only is None else names & set(only)
-
-
 def test_table_covers_every_conv_kernel():
-    declared = set()
+    kernels = set()
     for f in cc.COVERED_SOURCES:
-        declared |= declared_kernels(os.path.join(CSRC, f))
-    nb = declared_kernels(os.path.join(CSRC, "narrow_block.cu"), cc.NARROW_BLOCK_KERNELS)
+        kernels |= declared(os.path.join(CSRC, f))
+    nb = declared(os.path.join(CSRC, "narrow_block.cu")) & set(cc.NARROW_BLOCK_KERNELS)
     assert nb == set(cc.NARROW_BLOCK_KERNELS), "narrow_block.cu no longer declares " + \
         str(set(cc.NARROW_BLOCK_KERNELS) - nb)
-    declared |= nb
-    assert len(declared) == 18, f"source parse found {sorted(declared)}"
+    kernels |= nb
+    assert len(kernels) == 18, f"source parse found {sorted(kernels)}"
     covered = {cc.base_name(k) for c in cc.CASES for k in c.kernels}
-    missing = declared - covered
+    missing = kernels - covered
     assert not missing, f"convolution kernels without a conformance case: {sorted(missing)}"
-    unknown = covered - declared - cc.HELPER_KERNELS
+    unknown = covered - kernels - cc.HELPER_KERNELS
     assert not unknown, f"the table names kernels the sources do not declare: {sorted(unknown)}"

@@ -1,7 +1,6 @@
 """The fused-path case tables (tests/chain_cases.py, tests/tail_cases.py) against the library's eligibility predicates
-and the kernels csrc/narrow_block.cu and csrc/tail.cu declare and launch, and the fp64 references of
-tests/test_gpu_fused_conformance.py against stock torch float64.  Needs the built library, not a GPU: the predicates
-are host logic (num_sms() is 132 without a device)."""
+and the kernels csrc/narrow_block.cu and csrc/tail.cu declare and launch, and the tables' fp64 references against stock
+torch float64.  Needs the built library, not a GPU: the predicates are host logic (num_sms() is 132 without a device)."""
 import ctypes
 import os
 import re
@@ -13,22 +12,11 @@ import torch.nn.functional as F
 import chain_cases as ch
 import conv_cases as cc
 import tail_cases as tl
-import test_gpu_fused_conformance as ref
 from b200gan import _lib
-from test_cpu_conv_case_table import CSRC
+from conformance import CSRC, declared, source
 
 NB_CU = os.path.join(CSRC, "narrow_block.cu")
 TAIL_CU = os.path.join(CSRC, "tail.cu")
-
-
-def declared(path):
-    """__global__ names, also behind a __launch_bounds__ whose arguments hold a call"""
-    return set(re.findall(r"__global__\s+void\s+(?:__launch_bounds__\((?:[^()]|\([^()]*\))*\)\s*)?(\w+)\s*\(",
-                          _src(path)))
-
-
-def _src(path):
-    return re.sub(r"//[^\n]*", "", open(path).read())
 
 
 def test_case_ids_unique_and_explained():
@@ -46,7 +34,7 @@ def test_case_ids_unique_and_explained():
                          ids=lambda c: c.id)
 def test_chain_rows_against_the_predicates(case):
     lib = _lib.load()
-    g = ref.chain_geom(case)
+    g = ch.chain_geom(case)
     if case.op == "plain_dgrad":
         # a staged data gradient through the conv entry: not a chain layer, no tensor-core route
         assert lib.b200gan_nb_supported(ctypes.byref(g)) == 0
@@ -65,7 +53,7 @@ def test_grouped_minimum_batches():
     for c in ch.CASES:
         if c.groups in (3, 4) and c.op in ("fprop", "dgrad") and not c.error:
             smaller = [n for n in range(c.groups, c.N, c.groups)
-                       if lib.b200gan_nb_groups_supported(ctypes.byref(ref.chain_geom(
+                       if lib.b200gan_nb_groups_supported(ctypes.byref(ch.chain_geom(
                            ch.Case(c.name, c.op, n, c.C, c.K, c.H, c.W, c.R, c.stride))), c.groups)]
             assert not smaller, f"{c.id}: N = {smaller[0]} also runs with {c.groups} groups"
 
@@ -73,8 +61,8 @@ def test_grouped_minimum_batches():
 @pytest.mark.parametrize("case", tl.CASES, ids=lambda c: c.id)
 def test_tail_rows_against_the_predicate(case):
     lib = _lib.load()
-    d = _lib.TailDesc(case.N, case.H, case.W, case.C, case.K, ref.ACT_CODE[case.act_mid], ref.SLOPE,
-                      ref.ACT_CODE[case.act_out])
+    d = _lib.TailDesc(case.N, case.H, case.W, case.C, case.K, ch.ACT_CODE[case.act_mid], ch.SLOPE,
+                      ch.ACT_CODE[case.act_out])
     assert lib.b200gan_tail_supported(ctypes.byref(d)) == (0 if case.error else 1), case.id
 
 
@@ -91,7 +79,7 @@ def test_every_fused_kernel_has_a_case():
 
 def _launch_cases(macro):
     """the (KT, PT) list of an NB_*_INSTANCES X-macro, which both the launch and the refusal check expand"""
-    src = _src(NB_CU)
+    src = source(NB_CU)
     m = re.search(r"#define " + macro + r"\(X\)((?:[^\n]*\\\n)*[^\n]*)", src)
     assert m, f"no {macro} in narrow_block.cu"
     assert f"{macro}(NB_IS_INSTANCE)" in src and re.search(macro + r"\(NB_\w+_CASE\)", src), \
@@ -115,7 +103,7 @@ def test_every_planned_instance_is_covered_or_hook_only():
 
 
 def test_every_tail_instance_is_covered():
-    src = _src(TAIL_CU)
+    src = source(TAIL_CU)
     fwd = {f"tail_fprop_tc_kernel<{a}, {b}>" for a, b in re.findall(r"launch_tail_fprop<(\d+),\s*(\d+)>\(p", src)}
     assert len(fwd) == 6, fwd
     ks = sorted({int(k) for k in re.findall(r"launch_tail_bwd<C4,\s*(\d+)>", src)})
@@ -130,7 +118,7 @@ def test_every_tail_instance_is_covered():
 
 def test_planner_candidates_are_launch_cases_or_refused():
     """nb_plan's candidates (its kts lists x PT in {1, 2, 4}) either have an instance or make the launcher refuse"""
-    src = _src(NB_CU)
+    src = source(NB_CU)
     plan = src[src.index("static NbPlan nb_plan("):src.index("static NbPlan nb_plan_fprop")]
     kts = {int(v) for v in re.findall(r"kts\[\d\]\s*=\s*(\d+)", plan)}
     assert kts == {16, 8, 4, 1}, kts
@@ -164,15 +152,15 @@ def _bn_case(G, N=6, C=5, H=3, W=4, seed=0):
 def test_grouped_batchnorm_reference_is_separate_batch_norm_calls(G):
     a, gamma, beta, count = _bn_case(G)
     N, C = a.shape[0], a.shape[-1]
-    mean, var, rstd, sc, sh = ref.bn_consts(ref.group_sums(a, G), gamma, beta, count, G, C)
-    x = a * ref.per_image(sc, N) + ref.per_image(sh, N)
+    mean, var, rstd, sc, sh = ch.bn_consts(ch.group_sums(a, G), gamma, beta, count, G, C)
+    x = a * ch.per_image(sc, N) + ch.per_image(sh, N)
     rm0, rv0 = torch.linspace(-0.2, 0.3, C, dtype=torch.float64), torch.linspace(0.5, 1.5, C, dtype=torch.float64)
-    rm, rv = ref.running_ref(rm0, rv0, mean, var, count)
+    rm, rv = ch.running_ref(rm0, rv0, mean, var, count)
     trm, trv = rm0.clone(), rv0.clone()
     outs = []
     for g in range(G):   # the reference's separate forward passes, in batch order
-        part = ref.nchw(a[g * (N // G):(g + 1) * (N // G)])
-        outs.append(ref.nhwc(F.batch_norm(part, trm, trv, gamma, beta, True, ref.MOMENTUM, ref.BN_EPS)))
+        part = ch.nchw(a[g * (N // G):(g + 1) * (N // G)])
+        outs.append(ch.nhwc(F.batch_norm(part, trm, trv, gamma, beta, True, ch.MOMENTUM, ch.BN_EPS)))
     torch.testing.assert_close(x, torch.cat(outs), rtol=1e-12, atol=1e-12)
     torch.testing.assert_close(rm, trm, rtol=1e-12, atol=1e-12)
     torch.testing.assert_close(rv, trv, rtol=1e-12, atol=1e-12)
@@ -185,28 +173,28 @@ def test_dz_reference_is_batchnorm_backward(G):
     gen = torch.Generator().manual_seed(2)
     G_ = torch.randn(a.shape, generator=gen, dtype=torch.float64)
     cs = torch.rand(N, 1, 1, C, generator=gen, dtype=torch.float64) * 2 - 0.5
-    mean, var, rstd, sc, sh = ref.bn_consts(ref.group_sums(a, G), gamma, beta, count, G, C)
-    xh = (a - ref.per_image(mean, N)) * ref.per_image(rstd, N)
+    mean, var, rstd, sc, sh = ch.bn_consts(ch.group_sums(a, G), gamma, beta, count, G, C)
+    xh = (a - ch.per_image(mean, N)) * ch.per_image(rstd, N)
     sums = torch.stack([G_.reshape(G, -1, C).sum(1), (G_ * xh).reshape(G, -1, C).sum(1)], 1)
-    dz = ref.bn_bwd_ref(G_, a, mean, rstd, sc, sums, count, cs, "lrelu")
+    dz = ch.bn_bwd_ref(G_, a, mean, rstd, sc, sums, count, cs, "lrelu")
     av = a.clone().requires_grad_(True)
-    parts = [F.batch_norm(ref.nchw(av[g * (N // G):(g + 1) * (N // G)]), None, None, gamma, beta, True, 0.0,
-                          ref.BN_EPS) for g in range(G)]
-    (da,) = torch.autograd.grad(ref.nhwc(torch.cat(parts)), av, G_)
-    torch.testing.assert_close(dz, da * cs * torch.where(a > 0, 1.0, ref.SLOPE).double(), rtol=1e-10, atol=1e-12)
+    parts = [F.batch_norm(ch.nchw(av[g * (N // G):(g + 1) * (N // G)]), None, None, gamma, beta, True, 0.0,
+                          ch.BN_EPS) for g in range(G)]
+    (da,) = torch.autograd.grad(ch.nhwc(torch.cat(parts)), av, G_)
+    torch.testing.assert_close(dz, da * cs * torch.where(a > 0, 1.0, ch.SLOPE).double(), rtol=1e-10, atol=1e-12)
 
 
 def test_conv_references_are_autograd_of_conv2d():
     gen = torch.Generator().manual_seed(3)
     x = torch.randn(2, 9, 9, 4, generator=gen, dtype=torch.float64)
     w = torch.randn(8, 4, 3, 3, generator=gen, dtype=torch.float64)
-    xv, wv = ref.nchw(x).clone().requires_grad_(True), w.clone().requires_grad_(True)
+    xv, wv = ch.nchw(x).clone().requires_grad_(True), w.clone().requires_grad_(True)
     y = F.conv2d(xv, wv, stride=2, padding=1)
-    torch.testing.assert_close(ref.conv_fwd(x, w, 2, 1), ref.nhwc(y), rtol=1e-12, atol=1e-12)
+    torch.testing.assert_close(ch.conv_fwd(x, w, 2, 1), ch.nhwc(y), rtol=1e-12, atol=1e-12)
     dz = torch.randn(y.shape, generator=gen, dtype=torch.float64)
     gx, gw = torch.autograd.grad(y, (xv, wv), dz)
-    torch.testing.assert_close(ref.conv_dgrad(ref.nhwc(dz), w, x.shape, 2, 1), ref.nhwc(gx), rtol=1e-12, atol=1e-12)
-    torch.testing.assert_close(ref.conv_wgrad(x, ref.nhwc(dz), w.shape, 2, 1), gw, rtol=1e-12, atol=1e-12)
+    torch.testing.assert_close(ch.conv_dgrad(ch.nhwc(dz), w, x.shape, 2, 1), ch.nhwc(gx), rtol=1e-12, atol=1e-12)
+    torch.testing.assert_close(ch.conv_wgrad(x, ch.nhwc(dz), w.shape, 2, 1), gw, rtol=1e-12, atol=1e-12)
 
 
 @pytest.mark.parametrize("act_mid", ["none", "lrelu", "relu"])
@@ -226,17 +214,17 @@ def test_tail_references_are_the_stock_module(act_mid):
     sc = gamma * rstd
     mr, ss = torch.cat([mean, rstd]), torch.cat([sc, beta - mean * sc])
     av, gv, bv, wv, biv = (t.clone().requires_grad_(True) for t in (a, gamma, beta, w, bias))
-    x = F.batch_norm(ref.nchw(av), None, None, gv, bv, True, 0.0, 1e-5)
-    x = {"none": x, "lrelu": F.leaky_relu(x, ref.SLOPE), "relu": F.relu(x)}[act_mid]
+    x = F.batch_norm(ch.nchw(av), None, None, gv, bv, True, 0.0, 1e-5)
+    x = {"none": x, "lrelu": F.leaky_relu(x, ch.SLOPE), "relu": F.relu(x)}[act_mid]
     y = F.conv2d(x, wv, biv, padding=1)
-    da, dgamma, dbeta, dw, db = torch.autograd.grad(y, (av, gv, bv, wv, biv), ref.nchw(g))
-    r = ref.tail_bwd_ref(a, mr, ss, w, g, act_mid, (a * ss[:C] + ss[C:]) <= 0)
+    da, dgamma, dbeta, dw, db = torch.autograd.grad(y, (av, gv, bv, wv, biv), ch.nchw(g))
+    r = tl.tail_bwd_ref(a, mr, ss, w, g, act_mid, (a * ss[:C] + ss[C:]) <= 0)
     for got, want in ((r["da"], da), (r["s2"], dgamma), (r["s1"], dbeta), (r["dw"], dw),
                       (r["db"], db)):
         torch.testing.assert_close(got, want, rtol=1e-9, atol=1e-11)
     # forward: the wgmma operand rounding is the kernel's, the rest is the module's
-    out = ref.conv_fwd(ref.nhwc(x.detach()), w, 1, 1) + bias
-    want, *_ = ref.tail_fwd_ref(a.float(), ss.float(), w.float(), bias.float(), act_mid, "tanh")
+    out = ch.conv_fwd(ch.nhwc(x.detach()), w, 1, 1) + bias
+    want, *_ = tl.tail_fwd_ref(a.float(), ss.float(), w.float(), bias.float(), act_mid, "tanh")
     torch.testing.assert_close(want, torch.tanh(out), rtol=0, atol=5e-3)
 
 
@@ -338,7 +326,7 @@ def test_rows_are_what_the_planner_picks(case):
     elif case.op == "wgrad":
         got = None, wgrad_grid(case)
         lib = _lib.load()
-        nws = lib.b200gan_nb_wgrad_workspace_floats(ctypes.byref(ref.chain_geom(case)))
+        nws = lib.b200gan_nb_wgrad_workspace_floats(ctypes.byref(ch.chain_geom(case)))
         # the library sizes the slabs from the same plan: gx slabs of K * C * R * S floats
         if case.ws or ch.WG_RED in case.kernels:   # a NULL workspace (ws False) takes the atomics whatever the plan
             assert (nws > 0) == (ch.WG_RED in case.kernels), f"{case.id}: workspace floats {nws}"

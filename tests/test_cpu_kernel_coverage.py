@@ -1,47 +1,34 @@
 """Every __global__ kernel of the library has an fp64 conformance case, and the references of the critic and stream
-suites agree with stock torch float64.  Needs the built library (the suites import it), not a GPU.
+suites agree with stock torch float64.  Needs the built library (the case tables import it), not a GPU.
 
-A kernel is covered when a case table names it: conv (tests/conv_cases.py), chain, tail, norm, critic or stream; the
-few kernels a dedicated test covers instead are listed in COVERED_BY_TEST with that test.  A new kernel without a
-case fails here.
+A kernel is covered when a case table of the registry (conformance.case_tables) names it; the few kernels a dedicated
+test covers instead are listed in COVERED_BY_TEST with that test.  A new kernel without a case fails here.
 """
-import glob
 import os
-import re
-import shutil
-import subprocess
-import tempfile
 
 import pytest
 import torch
 import torch.nn.functional as F
 
-import chain_cases as ch
-import conv_cases as cc
 import critic_cases as cr
-import norm_cases as nc
 import stream_cases as sc
-import tail_cases as tl
-import test_gpu_critic_conformance as cref
-import test_gpu_stream_conformance as sref
-from test_cpu_conv_case_table import CSRC
-from test_cpu_fused_case_table import declared
+from conformance import CSRC, case_tables, declared, declared_under_csrc, needs_nvcc, ptxas_report, table_kernels
 
 COVERED_BY_TEST = {
     "pack_multi_kernel": "tests/test_gpu_conv_conformance.py::test_pack_weights_multi_30_jobs (bit-exact, 30 jobs)",
 }
 
 
-def table_kernels(cases):
-    return {cc.base_name(k) for c in cases for k in c.kernels}
-
-
 def test_every_kernel_has_a_case():
-    kernels = {k: os.path.basename(p) for p in glob.glob(os.path.join(CSRC, "*.cu")) for k in declared(p)}
+    """every __global__ under csrc/ -- in a .cu file or a .cuh header, at any depth -- is named by a registered case
+    table or by COVERED_BY_TEST"""
+    kernels = declared_under_csrc()
     assert len(kernels) > 30, f"parsed only {len(kernels)} __global__ kernels"
+    for d in (e.name for e in os.scandir(CSRC) if e.is_dir()):
+        assert any(f.startswith(d + os.sep) for f in kernels.values()), f"no kernel parsed under csrc/{d}"
     covered = set()
-    for cases in (cc.CASES, ch.CASES, tl.CASES, nc.CASES, cr.CASES, sc.CASES):
-        covered |= table_kernels(cases)
+    for cases, names in case_tables().values():
+        covered |= table_kernels(cases, names)
     missing = set(kernels) - covered - set(COVERED_BY_TEST)
     assert not missing, f"kernels without a conformance case: {sorted((kernels[k], k) for k in missing)}"
     stale = set(COVERED_BY_TEST) - set(kernels)
@@ -84,23 +71,13 @@ def test_critic_edges_are_in_the_table():
     assert any(c.zero_w3 for c in step) and any(c.zero_row >= 0 for c in step)
 
 
-@pytest.mark.skipif(not os.path.exists("/usr/local/cuda/bin/nvcc") and not shutil.which("nvcc"), reason="no nvcc")
+@needs_nvcc
 def test_critic_grid_follows_from_the_registers():
     """the cooperative grid is num_sms * min(2, blocks per SM); the blocks per SM follow from ptxas's registers"""
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    if not os.path.exists(nvcc):
-        nvcc = shutil.which("nvcc")
-    import build as b200_build
-    with tempfile.TemporaryDirectory() as d:
-        r = subprocess.run([nvcc, *b200_build.FLAGS, "-Xptxas=-v", "-c", os.path.join(CSRC, "mlp_critic.cu"), "-o",
-                            os.path.join(d, "mc.o")], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-2000:]
-    regs = {}
-    for chunk in r.stderr.split("Compiling entry function")[1:]:
-        name = re.match(r" '_ZN7b200gan\d+(\w+?)E", chunk).group(1)
-        regs[name] = int(re.search(r"Used (\d+) registers", chunk).group(1))
+    rep = ptxas_report(os.path.join(CSRC, "mlp_critic.cu"))
+    regs = {k: r["registers"] for k, r in rep.items()}
     assert regs == cr.REGISTERS, f"ptxas {regs}, table {cr.REGISTERS}"
-    assert re.findall(r"(\d+) bytes smem", r.stderr) == [str(cr.SMEM_BYTES)] * 4
+    assert [r["smem"] for r in rep.values()] == [cr.SMEM_BYTES] * 4
     per_sm = min(cr.blocks_per_sm(v) for v in regs.values())
     assert cr.GRID == (cr.NUM_SMS * min(2, per_sm), 1, 1)
     assert all(c.grid == cr.GRID for c in cr.CASES if not c.error)
@@ -124,18 +101,18 @@ def test_critic_references_are_sequential_autograd(slope):
     Wd = [w.detach() for w in W]
     x = torch.randn(5, 7, generator=g, dtype=torch.float64, requires_grad=True)
     out = net(x).reshape(-1)
-    f = cref.critic_fwd_ref(x.detach(), *Wd, slope)
+    f = cr.critic_fwd_ref(x.detach(), *Wd, slope)
     torch.testing.assert_close(f["out"], out.detach(), rtol=1e-12, atol=1e-12)
     dout = torch.randn(5, generator=g, dtype=torch.float64, requires_grad=True)
     gx, = torch.autograd.grad(out, x, dout, create_graph=True)
     grads = torch.autograd.grad(out, [x] + W, dout, retain_graph=True)
-    b = cref.critic_bwd_ref(dout.detach(), x.detach(), Wd[0], Wd[2], Wd[4].reshape(-1), f["m1"], f["a1"], f["m2"],
+    b = cr.critic_bwd_ref(dout.detach(), x.detach(), Wd[0], Wd[2], Wd[4].reshape(-1), f["m1"], f["a1"], f["m2"],
                             f["a2"])
     for name, want in zip(("dx", "dW1", "db1", "dW2", "db2", "dW3", "db3"), grads):
         torch.testing.assert_close(b[name][0].reshape(want.shape), want, rtol=1e-10, atol=1e-12, msg=name)
     u = torch.randn(5, 7, generator=g, dtype=torch.float64)
     dd = torch.autograd.grad(gx, [W[0], W[2], W[4], dout], u, allow_unused=True)
-    r = cref.critic_dbwd_ref(u, dout.detach(), b["U1"][0], b["U2"][0], f["m1"], f["m2"], Wd[0], Wd[2],
+    r = cr.critic_dbwd_ref(u, dout.detach(), b["U1"][0], b["U2"][0], f["m1"], f["m2"], Wd[0], Wd[2],
                              Wd[4].reshape(-1))
     for name, want in zip(("dW1", "dW2", "dW3", "ddout"), dd):
         want = torch.zeros_like(r[name][0]) if want is None else want
@@ -173,14 +150,14 @@ def test_critic_step_reference_is_the_wgan_gp_iteration(kind):
     d_loss = -torch.mean(net(real)) + torch.mean(net(fake)) + lam * gp
     want = torch.autograd.grad(d_loss, W, retain_graph=True)
     Wd = [w.detach() for w in W]
-    r = cref.critic_step_ref(real, fake, alpha.reshape(-1), *Wd, slope, lam)
+    r = cr.critic_step_ref(real, fake, alpha.reshape(-1), *Wd, slope, lam)
     # the reference weighs the real / fake rows by the kernel's fp32 -1/N and 1/N: relative differences of ~2^-24
     torch.testing.assert_close(r["losses"][0], torch.stack([d_loss, lam * gp]).detach(), rtol=1e-6, atol=1e-12)
     for name, w in zip(("dW1", "db1", "dW2", "db2", "dW3", "db3"), want):
         torch.testing.assert_close(r[name][0].reshape(w.shape), w, rtol=1e-6, atol=1e-7, msg=name)
     if kind in ("zero_w3", "zero_row"):
         pen = torch.autograd.grad(lam * gp, W, allow_unused=True)
-        r0 = cref.critic_step_ref(real, fake, alpha.reshape(-1), *Wd, slope, 0.0)
+        r0 = cr.critic_step_ref(real, fake, alpha.reshape(-1), *Wd, slope, 0.0)
         assert r["coef"].eq(0).sum() >= (6 if kind == "zero_w3" else 1)
         for name, p in zip(("dW1", "db1", "dW2", "db2", "dW3", "db3"), pen):
             # torch's norm backward passes 0 at a zero norm: the penalty contributes no gradient through that sample
@@ -201,7 +178,7 @@ def test_adam_reference_is_torch_adam(step0, gscale):
     m0 = torch.randn(1000, generator=g, dtype=torch.float64) * 0.1
     v0 = torch.rand(1000, generator=g, dtype=torch.float64) * 0.01
     p = torch.nn.Parameter(p0.clone())
-    opt = torch.optim.Adam([p], lr=sref.ADAM["lr"], betas=(sref.ADAM["b1"], sref.ADAM["b2"]), eps=sref.ADAM["eps"],
+    opt = torch.optim.Adam([p], lr=sc.ADAM["lr"], betas=(sc.ADAM["b1"], sc.ADAM["b2"]), eps=sc.ADAM["eps"],
                            foreach=False)
     if step0:
         opt.state[p] = {"step": torch.tensor(float(step0)), "exp_avg": m0.clone(), "exp_avg_sq": v0.clone()}
@@ -209,7 +186,7 @@ def test_adam_reference_is_torch_adam(step0, gscale):
         m0, v0 = torch.zeros_like(m0), torch.zeros_like(v0)
     p.grad = grad * gscale
     opt.step()
-    (p1, _), (m1, _), (v1, _) = sref.adam_ref(p0, grad, m0, v0, step0, gscale)
+    (p1, _), (m1, _), (v1, _) = sc.adam_ref(p0, grad, m0, v0, step0, gscale)
     st = opt.state[p]
     # the reference keeps the kernel's fp32 casts of the hyper-parameter terms: relative differences of ~2^-24
     torch.testing.assert_close(m1, st["exp_avg"], rtol=1e-6, atol=0)
@@ -225,8 +202,8 @@ def test_bce_reference_is_binary_cross_entropy():
     vv = v.clone().requires_grad_(True)
     loss = F.binary_cross_entropy(vv, t)
     (dv,) = torch.autograd.grad(loss * 1.5, vv)
-    torch.testing.assert_close(sref.bce_ref(v, t)[0], loss.detach(), rtol=1e-12, atol=0)
-    torch.testing.assert_close(sref.bce_grad_ref(v, t, 1.5), dv, rtol=1e-6, atol=0)   # the clamp is 1e-12 in fp32
+    torch.testing.assert_close(sc.bce_ref(v, t)[0], loss.detach(), rtol=1e-12, atol=0)
+    torch.testing.assert_close(sc.bce_grad_ref(v, t, 1.5), dv, rtol=1e-6, atol=0)   # the clamp is 1e-12 in fp32
 
 
 @pytest.mark.parametrize("pads,mode", [((1, 1, 0, 0), "zero"), ((1, 1, 1, 1), "reflect"), ((3, 3, 3, 3), "reflect"),
@@ -237,17 +214,17 @@ def test_pad_reference_is_the_stock_module(pads, mode):
     g = torch.Generator().manual_seed(5)
     x = torch.randn(2, 5, 6, 3, generator=g, dtype=torch.float64, requires_grad=True)
     y = m(x.permute(0, 3, 1, 2)).permute(0, 2, 3, 1)
-    torch.testing.assert_close(sref.pad_ref(x.detach(), pads, mode), y.detach(), rtol=0, atol=0)
+    torch.testing.assert_close(sc.pad_ref(x.detach(), pads, mode), y.detach(), rtol=0, atol=0)
     dy = torch.randn(y.shape, generator=g, dtype=torch.float64)
     (dx,) = torch.autograd.grad(y, x, dy)
-    torch.testing.assert_close(sref.pad_grad_ref(dy, x.shape, pads, mode), dx, rtol=1e-15, atol=1e-15)
+    torch.testing.assert_close(sc.pad_grad_ref(dy, x.shape, pads, mode), dx, rtol=1e-15, atol=1e-15)
 
 
 def test_upsample_reference_is_interpolate():
     g = torch.Generator().manual_seed(6)
     x = torch.randn(2, 5, 7, 3, generator=g, dtype=torch.float64, requires_grad=True)
     y = F.interpolate(x.permute(0, 3, 1, 2), scale_factor=2, mode="nearest").permute(0, 2, 3, 1)
-    torch.testing.assert_close(sref.upsample_ref(x.detach()), y.detach(), rtol=0, atol=0)
+    torch.testing.assert_close(sc.upsample_ref(x.detach()), y.detach(), rtol=0, atol=0)
     dy = torch.randn(y.shape, generator=g, dtype=torch.float64)
     (dx,) = torch.autograd.grad(y, x, dy)
-    torch.testing.assert_close(sref.upsample_grad_ref(dy), dx, rtol=1e-15, atol=1e-15)
+    torch.testing.assert_close(sc.upsample_grad_ref(dy), dx, rtol=1e-15, atol=1e-15)

@@ -10,8 +10,7 @@ import torch
 
 import critic_cases as cr
 from b200gan import nn as bnn
-from test_cpu_conv_case_table import CSRC
-from test_cpu_fused_case_table import declared
+from conformance import CSRC, declared, functions
 
 MC_CU = os.path.join(CSRC, "mlp_critic.cu")
 
@@ -100,19 +99,6 @@ def test_the_discriminator_on_the_cpu_is_the_stock_module():
 
 
 # ---- the entry points and the kernels they launch --------------------------------------------------------------------
-def _functions(src):
-    """name -> body of every function definition (static helpers and extern "C" entry points) in src"""
-    src = re.sub(r"//[^\n]*", "", src)
-    out = {}
-    for m in re.finditer(r"\n(?:static|extern \"C\")[^;{]*?\b(\w+)\s*\([^;{]*\)\s*\{", src):
-        depth, i = 1, m.end()
-        while depth:
-            depth += {"{": 1, "}": -1}.get(src[i], 0)
-            i += 1
-        out[m.group(1)] = src[m.end():i - 1]
-    return out
-
-
 def _launched(fns, name, seen=()):
     body = fns[name]
     assert "<<<" not in body, name
@@ -125,7 +111,7 @@ def _launched(fns, name, seen=()):
 
 def test_mlp_critic_cu_declares_only_the_critic_kernels_and_the_disc_entry_points_launch_them():
     assert declared(MC_CU) == set(cr.KERNEL.values())
-    fns = _functions(open(MC_CU).read())
+    fns = functions(open(MC_CU).read())
     assert {"b200gan_mlp_disc_fwd", "b200gan_mlp_disc_bwd", "b200gan_mlp_disc_bwd_workspace_floats"} <= set(fns)
     assert _launched(fns, "b200gan_mlp_disc_fwd") == {cr.KERNEL["fwd"]}
     assert _launched(fns, "b200gan_mlp_disc_bwd") == {cr.KERNEL["bwd"]}

@@ -1,29 +1,15 @@
 """The MLP generator (csrc/mlp_generator/mlp_generator.cu, functional.MlpGeneratorFn) without a GPU: the fp64
-references of tests/test_gpu_mlp_generator_conformance.py against torch float64 autograd for every case of
-tests/generator_cases.py, which module lists the drop-in Sequential routes to the kernels, the BatchNorm1d drop-in on
-the CPU, the rule that every __global__ kernel under csrc/ (at any depth) has a case, and ptxas's registers and spills."""
-import glob
+references of tests/generator_cases.py against torch float64 autograd for every case of the table, which module lists
+the drop-in Sequential routes to the kernels, the BatchNorm1d drop-in on the CPU, and ptxas's registers and spills."""
+import math
 import os
-import re
-import shutil
-import subprocess
-import tempfile
 
 import pytest
 import torch
 
-import chain_cases as ch
-import conv_cases as cc
-import critic_cases as cr
 import generator_cases as gc
-import norm_cases as nc
-import stream_cases as sc
-import tail_cases as tl
-import test_gpu_mlp_generator_conformance as gref
 from b200gan import nn as bnn
-from test_cpu_conv_case_table import CSRC
-from test_cpu_fused_case_table import declared
-from test_cpu_kernel_coverage import COVERED_BY_TEST, table_kernels
+from conformance import CSRC, declared, needs_nvcc, ptxas_report, table_kernels
 
 GEN_CU = os.path.join(CSRC, "mlp_generator", "mlp_generator.cu")
 
@@ -43,24 +29,24 @@ def _stock(c, P):
             break
         if c.has_norm[l]:
             # the kernel's eps and momentum are fp32
-            bn = tnn.BatchNorm1d(c.widths[l + 1], gref.f32(gref.EPS), momentum=gref.f32(gref.MOMENTUM)).double()
+            bn = tnn.BatchNorm1d(c.widths[l + 1], gc.f32(gc.EPS), momentum=gc.f32(gc.MOMENTUM)).double()
             with torch.no_grad():
                 for name, key in (("weight", "gamma"), ("bias", "beta"), ("running_mean", "rm"), ("running_var", "rv"),
                                   ("num_batches_tracked", "nbt")):
                     getattr(bn, name).copy_(P[f"{key}{l}"].reshape(()) if key == "nbt" else P[f"{key}{l}"])
             mods.append(bn)
-        mods.append(tnn.LeakyReLU(gref.f32(c.slope), inplace=True))
+        mods.append(tnn.LeakyReLU(gc.f32(c.slope), inplace=True))
     return tnn.Sequential(*mods)
 
 
 @pytest.mark.parametrize("case", [c for c in gc.CASES if not c.error and (c.op == "fwd" or c.only is None)],
                          ids=lambda c: c.id)
 def test_references_are_torch_float64_autograd(case):
-    c, P = case, gref.make(case, seed=0)
+    c, P = case, gc.make(case, seed=0)
     net = _stock(c, P)
     z = P["z"].double().requires_grad_(True)
     out = net(z)
-    layers = gref.gen_fwd_ref(P, c)
+    layers = gc.gen_fwd_ref(P, c)
     torch.testing.assert_close(layers[-1]["out"], out.detach(), rtol=1e-12, atol=1e-12)
     bns = [m for m in net if isinstance(m, torch.nn.BatchNorm1d)]
     for l, bn in zip([l for l in range(c.L - 1) if c.has_norm[l]], bns):
@@ -72,8 +58,8 @@ def test_references_are_torch_float64_autograd(case):
     want = dict(zip(["dz"] + [n for l in range(c.L) for n in (f"dW{l}", f"db{l}") +
                               ((f"dgamma{l}", f"dbeta{l}") if c.has_norm[l] else ())],
                     torch.autograd.grad(out, [z] + params, dout)))
-    acts, xh, rs = gref.split_saved(c, gref.saved_of(c, layers), c.N)
-    r = gref.gen_bwd_ref(c, dout, layers[-1]["out"], P["z"].double(), [P[f"W{l}"].double() for l in range(c.L)],
+    acts, xh, rs = gc.split_saved(c, gc.saved_of(c, layers), c.N)
+    r = gc.gen_bwd_ref(c, dout, layers[-1]["out"], P["z"].double(), [P[f"W{l}"].double() for l in range(c.L)],
                          [P[f"gamma{l}"].double() if c.has_norm[l] else None for l in range(c.L)], acts, xh, rs)
     assert set(r) == set(c.all_outputs()) == set(want)
     for name, w in want.items():
@@ -90,24 +76,12 @@ def test_generator_table_covers_its_edges():
         assert any(c.N == 64 and c.widths == gc.WGAN for c in ok) and any(c.widths == gc.GAN for c in ok), op
         assert any(any(w % 32 for w in c.widths) for c in ok) and any(c.N == 2 for c in ok), op
         assert any(c.L == 1 for c in ok) and {0.0, 0.2, 1.0} <= {c.slope for c in ok}, op
-        assert any(gref.math.ceil(c.N / 32) * gref.math.ceil(max(c.widths) / 32) > 2 * gc.GRID[0] for c in ok), op
+        assert any(math.ceil(c.N / 32) * math.ceil(max(c.widths) / 32) > 2 * gc.GRID[0] for c in ok), op
         err = {c.name for c in gc.CASES if c.op == op and c.error}
         assert {"n1", "wide", "no_ws"} <= err, op
     single = gc.Case("", "bwd", 0, gc.SMALL, (1, 1)).all_outputs()
     assert {f"{o}_only" for o in single} <= {c.name for c in gc.CASES if c.op == "bwd"}
     assert any(not c.keep for c in gc.CASES if c.op == "fwd" and not c.error)
-
-
-def test_every_kernel_at_any_depth_has_a_case():
-    """every __global__ under csrc/, in a subdirectory too, is named by a case table (or a dedicated test)"""
-    found = {k: os.path.relpath(p, CSRC) for p in glob.glob(os.path.join(CSRC, "**", "*.cu"), recursive=True)
-             for k in declared(p)}
-    assert "mlp_gen_fwd_kernel" in found and len(found) > 30
-    covered = set(COVERED_BY_TEST)
-    for cases in (cc.CASES, ch.CASES, tl.CASES, nc.CASES, cr.CASES, sc.CASES, gc.CASES):
-        covered |= table_kernels(cases)
-    missing = set(found) - covered
-    assert not missing, f"kernels without a conformance case: {sorted((found[k], k) for k in missing)}"
 
 
 def test_build_compiles_every_source_at_any_depth():
@@ -116,23 +90,14 @@ def test_build_compiles_every_source_at_any_depth():
     assert all(os.path.isfile(os.path.join(CSRC, f)) for f in b200_build._files())
 
 
-@pytest.mark.skipif(not os.path.exists("/usr/local/cuda/bin/nvcc") and not shutil.which("nvcc"), reason="no nvcc")
+@needs_nvcc
 def test_generator_kernels_do_not_spill_and_the_grid_follows_from_the_registers():
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    if not os.path.exists(nvcc):
-        nvcc = shutil.which("nvcc")
-    import build as b200_build
-    with tempfile.TemporaryDirectory() as d:
-        r = subprocess.run([nvcc, *b200_build.FLAGS, "-Xptxas=-v", "-c", GEN_CU, "-o", os.path.join(d, "g.o")],
-                           capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-2000:]
-    regs = {}
-    for chunk in r.stderr.split("Compiling entry function")[1:]:
-        name = re.match(r" '_ZN7b200gan\d+(\w+?)E", chunk).group(1)
-        regs[name] = int(re.search(r"Used (\d+) registers", chunk).group(1))
-        assert re.search(r"0 bytes stack frame, 0 bytes spill stores, 0 bytes spill loads", chunk), chunk[:400]
+    rep = ptxas_report(GEN_CU)
+    for name, r in rep.items():
+        assert r["stack"] == r["spills"] == 0, f"{name}: {r}"
+    regs = {k: r["registers"] for k, r in rep.items()}
     assert regs == gc.REGISTERS, f"ptxas {regs}, table {gc.REGISTERS}"
-    assert re.findall(r"(\d+) bytes smem", r.stderr) == [str(gc.SMEM_BYTES)] * 2
+    assert [r["smem"] for r in rep.values()] == [gc.SMEM_BYTES] * 2
     per_sm = min(gc.blocks_per_sm(v) for v in regs.values())
     assert gc.GRID == (gc.NUM_SMS * min(2, per_sm), 1, 1)
     assert all(c.grid == gc.GRID for c in gc.CASES if not c.error)

@@ -3,19 +3,17 @@ import os
 import re
 
 import norm_cases as nc
-from test_cpu_conv_case_table import CSRC, declared_kernels
+from conformance import CSRC, declared, source
 
 NORM_CU = os.path.join(CSRC, "norm.cu")
-KERNELS = {"norm_stats_kernel", "norm_finalize_kernel", "norm_apply_kernel", "norm_bwd_reduce_kernel",
-           "norm_bwd_apply_kernel", "norm_bwd_params_kernel"}
 
 
 def test_norm_cu_declares_one_kernel_per_pass():
-    assert declared_kernels(NORM_CU) == KERNELS
+    assert declared(NORM_CU) == nc.KERNELS
 
 
 def test_table_covers_every_instance_and_the_sliced_grid():
-    src = re.sub(r"//[^\n]*", "", open(NORM_CU).read())
+    src = source(NORM_CU)
     launched = set(re.findall(r"\b(norm_\w+_kernel<\d+>)", src))
     assert launched, "no templated launch found in norm.cu"
     covered = {k for c in nc.CASES for k in c.kernels if "<" in k}

@@ -12,54 +12,15 @@ Incoming u = dL/d(dx), ugamma, ubeta; U = sum u, T = sum u xhat, Q = sum u g:
 Nothing assumes sum xhat^2 = m, which fails for DCGAN's eps = 0.8.
 """
 import os
-import re
-import shutil
-import subprocess
-import tempfile
 
 import pytest
 import torch
 import torch.nn.functional as tf
 
-from test_cpu_conv_case_table import CSRC, declared_kernels
-from test_cpu_norm_case_table import KERNELS
+from conformance import CSRC, declared, needs_nvcc, ptxas_report
+from norm_cases import KERNELS, SLOPE, closed_form
 
 NORM_CU = os.path.join(CSRC, "norm.cu")
-SLOPE = 0.2
-
-
-def mask(act, pre):
-    if act == "lrelu":
-        return torch.where(pre > 0, torch.ones_like(pre), torch.full_like(pre, SLOPE))
-    if act == "relu":
-        return (pre > 0).to(pre.dtype)
-    return torch.ones_like(pre)
-
-
-def closed_form(x, dy, gamma, beta, u, ugamma, ubeta, eps, act, per_sample, ap=None):
-    """(dL/d(dy), dL/dx, dL/d(gamma) per channel or None) on NCHW tensors, any dtype; gamma/beta None = non-affine,
-    ugamma/ubeta None = 0; ap: the activation's mask, else computed from the normalised x"""
-    n, c = x.shape[:2]
-    dims = (2, 3) if per_sample else (0, 2, 3)
-    m = x[0, 0].numel() * (1 if per_sample else n)
-    ch = (1, c, 1, 1)
-    mean = x.mean(dims, keepdim=True)
-    r = 1 / torch.sqrt(((x - mean) ** 2).mean(dims, keepdim=True) + eps)
-    xh = (x - mean) * r
-    ga = gamma.view(ch) if gamma is not None else 1.0
-    be = beta.view(ch) if beta is not None else 0.0
-    ap = mask(act, ga * xh + be) if ap is None else ap
-    g = dy * ap
-    A, B = g.sum(dims, keepdim=True) / m, (g * xh).sum(dims, keepdim=True) / m
-    U, T, Q = u.sum(dims, keepdim=True), (u * xh).sum(dims, keepdim=True), (u * g).sum(dims, keepdim=True)
-    ug = ugamma.view(ch) if ugamma is not None else 0.0
-    ub = ubeta.view(ch) if ubeta is not None else 0.0
-    gdy = ap * (ga * r * (u - U / m - xh * T / m) + ug * xh + ub)
-    gx = ug * r * (g - A - xh * B) - (ga * r * r / m) * (xh * (Q - A * U - 3 * B * T) + T * (g - A) + B * (m * u - U))
-    ggamma = None
-    if gamma is not None:
-        ggamma = (r * (Q - A * U - B * T)).sum(0).view(c)
-    return gdy, gx, ggamma
 
 
 def torch_double_backward(x, dy, gamma, beta, u, ugamma, ubeta, eps, act, per_sample):
@@ -110,29 +71,18 @@ def test_closed_form_matches_torch_float64_double_backward(per_sample, affine, e
 
 
 def test_norm_cu_still_declares_exactly_the_six_kernels():
-    assert declared_kernels(NORM_CU) == KERNELS
+    assert declared(NORM_CU) == KERNELS
 
 
-@pytest.mark.skipif(not os.path.exists("/usr/local/cuda/bin/nvcc") and not shutil.which("nvcc"), reason="no nvcc")
+@needs_nvcc
 def test_norm_backward_kernels_keep_their_register_and_shared_memory_budgets():
     """Every norm.cu instance: no stack frame, no spills.  The VEC 4 backward instances stay at or below 80 registers
     (3 blocks of 256 threads per SM); the reduce instances keep their 2048 / 8192 B of shared memory."""
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    if not os.path.exists(nvcc):
-        nvcc = shutil.which("nvcc")
-    import build as b200_build
-    with tempfile.TemporaryDirectory() as d:
-        r = subprocess.run([nvcc, *b200_build.FLAGS, "-Xptxas=-v", "-c", NORM_CU, "-o", os.path.join(d, "n.o")],
-                           capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-2000:]
-    regs, smem = {}, {}
-    for chunk in r.stderr.split("Compiling entry function")[1:]:
-        m = re.match(r" '_ZN7b200gan\d+(\w+?)(?:ILi(\d)EE)?E", chunk)
-        name = m.group(1) + (f"<{m.group(2)}>" if m.group(2) else "")
-        assert re.search(r"0 bytes stack frame, 0 bytes spill stores, 0 bytes spill loads", chunk), f"{name}: {chunk[:400]}"
-        regs[name] = int(re.search(r"Used (\d+) registers", chunk).group(1))
-        s = re.search(r"(\d+) bytes smem", chunk)
-        smem[name] = int(s.group(1)) if s else 0
+    rep = ptxas_report(NORM_CU)
+    for name, r in rep.items():
+        assert r["stack"] == r["spills"] == 0, f"{name}: {r}"
+    regs = {k: r["registers"] for k, r in rep.items()}
+    smem = {k: r["smem"] for k, r in rep.items()}
     assert regs["norm_bwd_reduce_kernel<4>"] <= 80 and regs["norm_bwd_apply_kernel<4>"] <= 80, regs
     assert smem["norm_bwd_reduce_kernel<1>"] == 2048 and smem["norm_bwd_reduce_kernel<4>"] == 8192, smem
     assert smem["norm_bwd_apply_kernel<1>"] == smem["norm_bwd_apply_kernel<4>"] == 0, smem

@@ -1,32 +1,17 @@
 """MSELoss / L1Loss on the pixel-loss kernels (csrc/pixel_loss/, functional.PixelLossFn) without a GPU:
 which calls the drop-in modules route to the kernels and which go to the stock forward, the class names and the patch,
-the fp64 references of tests/test_gpu_pixel_loss_conformance.py against torch float64 autograd, the case table against
-the kernel source and ptxas, and the rule that every __global__ kernel under csrc/ -- in a .cu file or a header, at any
-depth -- has a case."""
-import glob
+the fp64 references of tests/pixel_loss_cases.py against torch float64 autograd, and the case table against the kernel
+source and ptxas."""
 import os
 import re
-import shutil
-import subprocess
-import tempfile
 import warnings
 
 import pytest
 import torch
 
-import chain_cases as ch
-import conv_cases as cc
-import critic_cases as cr
-import generator_cases as gc
-import norm_cases as nc
-import stream_cases as sc
-import tail_cases as tl
-import test_gpu_pixel_loss_conformance as pl
+import pixel_loss_cases as pl
 from b200gan import nn as bnn
-from test_cpu_conv_case_table import CSRC
-from test_cpu_fused_case_table import declared
-from test_cpu_kernel_coverage import COVERED_BY_TEST, table_kernels
-from test_cpu_mlp_discriminator_plan import _functions
+from conformance import CSRC, declared, functions, needs_nvcc, ptxas_report, source
 
 PL_CU = os.path.join(CSRC, "pixel_loss", "pixel_loss.cu")
 PL_CUH = os.path.join(CSRC, "pixel_loss", "pixel_loss_kernels.cuh")
@@ -212,8 +197,8 @@ def test_the_header_declares_the_two_kernels_and_the_entry_points_launch_only_th
     assert declared(PL_CUH) == set(pl.KERNEL.values()) == {k for c in pl.CASES for k, _ in c.kernels()}
     assert declared(PL_CU) == set()
     assert '#include "pixel_loss_kernels.cuh"' in open(PL_CU).read()
-    src = re.sub(r"//[^\n]*", "", open(PL_CU).read())
-    fns = _functions(src)
+    src = source(PL_CU)
+    fns = functions(src)
     assert {"b200gan_pixel_loss_fwd", "b200gan_pixel_loss_bwd", "b200gan_pixel_loss_workspace_bytes"} <= set(fns)
 
     def launched(name, seen=()):
@@ -229,40 +214,17 @@ def test_the_header_declares_the_two_kernels_and_the_entry_points_launch_only_th
     assert len(re.findall(r"<<<", src)) == 2
 
 
-def test_every_kernel_in_a_source_or_header_at_any_depth_has_a_case():
-    """every __global__ under csrc/ -- in a .cu file or a .cuh header, in a subdirectory too -- is named by a case table
-    (the pixel-loss table included) or a dedicated test"""
-    found = {k: os.path.relpath(p, CSRC) for ext in ("*.cu", "*.cuh")
-             for p in glob.glob(os.path.join(CSRC, "**", ext), recursive=True) for k in declared(p)}
-    assert "mlp_gen_fwd_kernel" in found and "pixel_loss_fwd_kernel" in found and len(found) > 30
-    covered = set(COVERED_BY_TEST) | {k for c in pl.CASES for k, _ in c.kernels()}
-    for cases in (cc.CASES, ch.CASES, tl.CASES, nc.CASES, cr.CASES, sc.CASES, gc.CASES):
-        covered |= table_kernels(cases)
-    missing = set(found) - covered
-    assert not missing, f"kernels without a conformance case: {sorted((found[k], k) for k in missing)}"
-
-
 def test_build_compiles_the_subdirectory():
     import build as b200_build
     assert os.path.join("pixel_loss", "pixel_loss.cu") in b200_build.sources()
 
 
-@pytest.mark.skipif(not os.path.exists("/usr/local/cuda/bin/nvcc") and not shutil.which("nvcc"), reason="no nvcc")
+@needs_nvcc
 def test_kernels_do_not_spill_and_keep_their_registers():
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    if not os.path.exists(nvcc):
-        nvcc = shutil.which("nvcc")
-    import build as b200_build
-    with tempfile.TemporaryDirectory() as d:
-        r = subprocess.run([nvcc, *b200_build.FLAGS, "-Xptxas=-v", "-c", PL_CU, "-o", os.path.join(d, "p.o")],
-                           capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-2000:]
-    regs, smem = {}, {}
-    for chunk in r.stderr.split("Compiling entry function")[1:]:
-        name = re.match(r" '_ZN7b200gan\d+(\w+?)E", chunk).group(1)
-        regs[name] = int(re.search(r"Used (\d+) registers", chunk).group(1))
-        m = re.search(r"(\d+) bytes smem", chunk)
-        smem[name] = int(m.group(1)) if m else 0
-        assert re.search(r"0 bytes stack frame, 0 bytes spill stores, 0 bytes spill loads", chunk), chunk[:400]
+    rep = ptxas_report(PL_CU)
+    for name, r in rep.items():
+        assert r["stack"] == r["spills"] == 0, f"{name}: {r}"
+    regs = {k: r["registers"] for k, r in rep.items()}
+    smem = {k: r["smem"] for k, r in rep.items()}
     assert regs == pl.REGISTERS, f"ptxas {regs}, table {pl.REGISTERS}"
     assert smem == pl.SMEM_BYTES, f"ptxas {smem}, table {pl.SMEM_BYTES}"

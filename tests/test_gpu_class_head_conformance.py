@@ -1,17 +1,17 @@
 """Every case of tests/class_head_cases.py -- the class-head mode of linear1_{fwd,bwd}_kernel and the cross-entropy mode
 of bce_{fwd,bwd}_kernel (csrc/head.cu) -- element by element against torch float64.
 
-Each case calls the C ABI on the guarded buffers of the convolution conformance test (Arena): inputs between NaN
-guards, outputs started as NaN, sentinels around everything the library writes.
+Each case calls the C ABI on the guarded buffers of tests/conformance.py (Arena) and runs its protocol: inputs between
+NaN guards, outputs started as NaN, sentinels around everything the library writes.
 
 Checks:
   - every output against fp64 with a bound from the arithmetic, 2^-23 (n + s) A as in the stream suite: A the same sum
     over |terms|, n the length of the kernel's longest fp32 chain and s the roundings outside it; the softmax carries
     the logits' bound through its derivative;
-  - the traced kernels and grids of the table (a sacrificial first profiler session, and a marker launch);
-  - two eager runs and a CUDA-graph replay, bit for bit;
-  - refusals: each entry point the case names returns B200GAN_E_BAD_ARG and writes nothing;
-  - the linear1 and BCE rows of the stream table, unchanged, through the stream suite's own per-case test.
+  - the traced kernels and grids of the table;
+  - a CUDA-graph replay, bit for bit;
+  - refusals: each entry point the case names returns B200GAN_E_BAD_ARG and writes nothing, the others accept the call.
+The linear1 and BCE rows of the stream table, which share these kernels, run in tests/test_gpu_stream_conformance.py.
 """
 import math
 
@@ -19,50 +19,15 @@ import pytest
 import torch
 
 import class_head_cases as hc
-import stream_cases as sc
-import test_gpu_stream_conformance as st
 from b200gan import _lib
-from test_gpu_conv_conformance import Arena, check_elementwise, traced_kernels
+from class_head_cases import ce_grad_ref, ce_ref, head_grad_ref, head_ref
+from conformance import Arena, check_elementwise, not_vacuous, run_case
 
 pytestmark = pytest.mark.gpu
 
 U = 2.0 ** -23
 TINY = 2.0 ** -126      # fp32's smallest normal: what an underflowing expf may lose
 F32, I64 = torch.float32, torch.int64
-
-
-# ---- fp64 references (device-agnostic: tests/test_cpu_class_head.py holds them to torch float64 autograd) ------------
-def head_ref(x, w, b):
-    """softmax(x w^T + b) over dim 1, and the logits"""
-    z = x.double() @ w.double().t() + (0 if b is None else b.double())
-    return torch.softmax(z, 1), z
-
-
-def head_grad_ref(x, w, y, dy):
-    """(dx, dw, db, dz) of Linear + Softmax from the saved output y: dz = y (dy - sum_i y_i dy_i)"""
-    y, dy = y.double(), dy.double()
-    dz = y * (dy - (y * dy).sum(1, keepdim=True))
-    return dz @ w.double(), dz.t() @ x.double(), dz.sum(0), dz
-
-
-def ce_ref(x, target, ignore_index):
-    """CrossEntropyLoss(reduction='mean', ignore_index) over the in-range targets, and the count of rows not ignored"""
-    x = x.double()
-    keep = target != ignore_index
-    lse = torch.logsumexp(x, 1)
-    t = target.clamp(0, x.shape[1] - 1)
-    terms = torch.where(keep, lse - x.gather(1, t[:, None])[:, 0], torch.zeros_like(lse))
-    count = int(keep.sum().item())
-    return terms.sum() / count if count else torch.tensor(float("nan"), dtype=torch.float64), terms, count
-
-
-def ce_grad_ref(x, target, ignore_index, gout, count):
-    """gout / count (softmax(x) - onehot(target)), zero rows where ignored"""
-    x = x.double()
-    p = torch.softmax(x, 1)
-    hit = torch.arange(x.shape[1], device=x.device) == target[:, None]
-    d = (p - hit.double()) * (gout / count)
-    return torch.where((target != ignore_index)[:, None], d, torch.zeros_like(d))
 
 
 # ---- runs ------------------------------------------------------------------------------------------------------------
@@ -98,7 +63,7 @@ class Run:
         self.arena.prepare(self.data)
 
     def outputs(self):
-        return {k: v.clone() for k, v in self.arena.t.items() if self.arena.layout[k][3] != "in"}
+        return self.arena.outputs()
 
     # ---- Linear(K, n) + Softmax
     def setup_head(self, specs, d, o):
@@ -142,7 +107,7 @@ class Run:
         ey = y_ref * (ez + (y_ref * ez).sum(1, keepdim=True) + U * (zm + (y_ref * zm).sum(1, keepdim=True)) + 12 * U) + \
             TINY
         worst = check_elementwise(what + " y", self.t("y"), y_ref, ey, "(r, j)")
-        st.not_vacuous(what + " y", ey - TINY, y_ref)
+        not_vacuous(what + " y", ey - TINY, y_ref)
         yk = self.t("y").view(N, n)
         dx_ref, dw_ref, db_ref, dz = head_grad_ref(self.x, self.w, yk, self.dy)
         yd = yk.double()
@@ -229,88 +194,29 @@ class Run:
         return check_elementwise(what + " dx", dx[ok], d_ref[ok], bound[ok], "(r, j)")
 
     def call(self, s):
-        return getattr(self, "fwd_" + self.c.op)(s) or getattr(self, "bwd_" + self.c.op)(s)
+        if not self.c.error:
+            return getattr(self, "fwd_" + self.c.op)(s) or getattr(self, "bwd_" + self.c.op)(s)
+        # a refusal: each entry point the case names must refuse it; one it does not name accepts the call, and what
+        # that wrote is reset, so that the refusals are seen to write nothing
+        codes = []
+        for side in ("fwd", "bwd"):
+            rc = getattr(self, f"{side}_{self.c.op}")(s)
+            torch.cuda.synchronize()
+            if side in self.c.opt["refused_by"]:
+                codes.append(rc)
+            else:
+                assert rc == 0, f"{self.c.id}: {side} rc {rc}: {self.lib.b200gan_last_error().decode()}"
+                self.prepare()
+        return next((rc for rc in codes if rc != -2), -2)
 
     def check(self, what):
         return getattr(self, "check_" + self.c.op)(what)
 
 
 # ---- the per-case test ---------------------------------------------------------------------------------------------
-FAMILY = {k for c in hc.CASES for k in c.kernels}
-
-
-def check_route(run):
-    """the case's kernels in launch order with their grids, from one profiler session opened by a marker launch"""
-    c = run.c
-    marker = torch.zeros(1, device="cuda")
-    seen = []
-    for _ in range(3):   # a lost record does not repeat; a route that differs from the table does
-        run.prepare()
-        seen = [(n, tuple(g)) for n, g in traced_kernels(lambda: (marker.zero_(), run.call(
-            torch.cuda.current_stream().cuda_stream))) if n in FAMILY]
-        if [n for n, _ in seen] == list(c.kernels):
-            break
-    assert seen == c.launches, f"{c.id}: trace {seen}, table {c.launches}"
+FAMILY = tuple({k for c in hc.CASES for k in c.kernels})
 
 
 @pytest.mark.parametrize("case", hc.CASES, ids=lambda c: c.id)
 def test_class_head_case(case):
-    run = Run(case)
-    lib = run.lib
-    run.prepare()
-    before = run.outputs()
-    s = torch.cuda.current_stream().cuda_stream
-    if case.error:
-        for side in ("fwd", "bwd"):
-            rc = getattr(run, f"{side}_{case.op}")(s)
-            torch.cuda.synchronize()
-            if side in case.opt["refused_by"]:
-                assert rc == -2, f"{case.id}: {side} expected B200GAN_E_BAD_ARG, rc {rc}"
-            else:
-                assert rc == 0, f"{case.id}: {side} rc {rc}: {lib.b200gan_last_error().decode()}"
-                run.prepare()
-        run.arena.check_guards(case.id)
-        after = run.outputs()
-        for k, v in before.items():
-            assert torch.equal(v.view(torch.int32), after[k].view(torch.int32)), f"{case.id}: refused call wrote {k}"
-        return
-    rc = run.call(s)
-    torch.cuda.synchronize()
-    assert rc == 0, f"{case.id}: rc {rc}: {lib.b200gan_last_error().decode()}"
-    run.arena.check_guards(case.id)
-    eager = run.outputs()
-    worst = run.check(case.id + " eager")
-
-    run.prepare()
-    assert run.call(s) == 0
-    torch.cuda.synchronize()
-    for k, v in run.outputs().items():
-        assert torch.equal(v.view(torch.int32), eager[k].view(torch.int32)), f"{case.id}: a second run differs in {k}"
-
-    check_route(run)
-
-    side = torch.cuda.Stream()
-    run.prepare()
-    torch.cuda.synchronize()
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph, stream=side):
-        rc = run.call(side.cuda_stream)
-    assert rc == 0, f"{case.id}: rc {rc} under capture: {lib.b200gan_last_error().decode()}"
-    run.prepare()
-    torch.cuda.synchronize()
-    graph.replay()
-    torch.cuda.synchronize()
-    run.arena.check_guards(case.id + " graph")
-    for k, v in run.outputs().items():
-        assert torch.equal(v.view(torch.int32), eager[k].view(torch.int32)), f"{case.id}: graph replay differs in {k}"
-    print(f"\n{case.id}: worst |err|/bound {worst:.3g}, launches {case.launches}")
-
-
-UNCHANGED = [c for c in sc.CASES if c.id in ("linear1-dcgan", "linear1-k129", "linear1-nulls", "linear1-n4096",
-                                             "bce-n128", "bce-clamps", "bce-over_cap")]
-
-
-@pytest.mark.parametrize("case", UNCHANGED, ids=lambda c: c.id)
-def test_linear1_and_bce_entry_points_keep_their_behaviour(case):
-    """the nout == 1 head and the BCE loss, which share the kernels with the new modes, still pass their stream cases"""
-    st.test_stream_case(case)
+    run_case(Run(case), case.id, case.launches, refuse=(-2,) if case.error else (), family=FAMILY)

@@ -1,12 +1,8 @@
 """Every convolution route of tests/conv_cases.py, element by element against an fp64 reference.
 
-Each case calls the C ABI directly on buffers carved from one allocation, [guard | tensor | guard], every tensor
-256-byte aligned behind a 4 KB guard:
-  - input guards hold NaN: a read past an input that feeds arithmetic shows up as NaN in the output;
-  - outputs and workspaces start as NaN: an element the kernel never writes fails, and stale workspace contents
-    cannot pass for zeros;
-  - output / workspace / statistics guards hold a sentinel bit pattern that must survive the call;
-  - statistics start at known non-zero values: the header promises accumulation, not overwrite.
+Each case calls the C ABI directly on the guarded buffers of tests/conformance.py (Arena) and runs its protocol; the
+statistics start at known non-zero values, since the header promises accumulation, not overwrite.  The route is a set:
+every traced kernel is one the table names, and every kernel it names is traced.
 The reference is torch float64 on the GPU, fed the operands the kernel feeds its arithmetic (packed wgmma weights
 rounded to TF32 with RNA, raw activations truncated to TF32 by wgmma; SIMT kernels use fp32 as is).  A, the same
 operation on absolute values, scales an error bound that follows from the arithmetic, not from a fit:
@@ -17,10 +13,7 @@ rounding the reference does not reproduce (the x2 upsample fold's fp32 tap sums 
 through the epilogue with its Lipschitz constants.
 """
 import ctypes
-import json
 import math
-import os
-import tempfile
 
 import numpy as np
 import pytest
@@ -29,92 +22,14 @@ import torch.nn.functional as F
 
 import conv_cases as cc
 from b200gan import _lib
+from conformance import (STATS_FILL, Arena, check_elementwise, first_grid, not_vacuous, np_rna, run_case, tf32_rna,
+                         tf32_trunc)
 
 pytestmark = pytest.mark.gpu
 
-GUARD_BYTES = 4096
-ALIGN_BYTES = 256
-SENTINEL = 0x7FC0DEAD          # a NaN bit pattern no kernel produces
-STATS_FILL = (3.0, 5.0)        # prefill of stats[0..G) and stats[G..2G)
 U = 2.0 ** -23
 EPS_UP2_FOLD = 2.0 ** -11 + 3 * 2.0 ** -24
 SLOPE = 0.2
-
-
-# ---- TF32 models -------------------------------------------------------------------------------------------------
-def tf32_trunc(t):
-    """what wgmma does to a raw fp32 operand: the low 13 mantissa bits are ignored"""
-    return (t.contiguous().view(torch.int32) & ~0x1FFF).view(torch.float32)
-
-
-def tf32_rna(t):
-    """cvt.rna.tf32.f32: round to nearest, ties away from zero (the packed weights, round_tf32 outputs)"""
-    return ((t.contiguous().view(torch.int32) + 0x1000) & ~0x1FFF).view(torch.float32)
-
-
-def np_rna(a):
-    a = np.ascontiguousarray(a, dtype=np.float32)
-    return ((a.view(np.int32) + 0x1000) & ~0x1FFF).view(np.float32)
-
-
-# ---- buffers -----------------------------------------------------------------------------------------------------
-class Arena:
-    """Tensors carved from one device allocation, each between two guards of GUARD_BYTES."""
-
-    def __init__(self, specs):
-        # specs: list of (name, numel, dtype, role) with role in {"in", "out", "ws", "stats"}
-        self.specs = specs
-        off = 0
-        self.layout = {}
-        for name, numel, dtype, role in specs:
-            isz = torch.empty((), dtype=dtype).element_size()
-            off += GUARD_BYTES
-            nbytes = -(-max(numel, 1) * isz // ALIGN_BYTES) * ALIGN_BYTES
-            self.layout[name] = (off, numel, dtype, role, nbytes)
-            off += nbytes
-        off += GUARD_BYTES
-        self.buf = torch.empty(off // 4, dtype=torch.int32, device="cuda")
-        self.t = {}
-        for name, (o, numel, dtype, role, nbytes) in self.layout.items():
-            raw = self.buf[o // 4:(o + nbytes) // 4]
-            self.t[name] = raw.view(dtype)[:numel]
-
-    def guards(self, name):
-        o, numel, dtype, role, nbytes = self.layout[name]
-        isz = torch.empty((), dtype=dtype).element_size()
-        lo = self.buf[(o - GUARD_BYTES) // 4:o // 4]
-        tail_start = o + numel * isz
-        hi = self.buf[-(-tail_start // 4):(o + nbytes + GUARD_BYTES) // 4]
-        return lo, hi
-
-    def prepare(self, data):
-        """guards, NaN / prefill of outputs and workspaces; data: name -> tensor for the inputs"""
-        nan32 = torch.tensor(float("nan"), dtype=torch.float32).view(torch.int32).item()
-        self.buf.fill_(nan32)
-        for name, (o, numel, dtype, role, nbytes) in self.layout.items():
-            lo, hi = self.guards(name)
-            if role != "in":
-                lo.fill_(SENTINEL)
-                hi.fill_(SENTINEL)
-            if role == "in":
-                self.t[name].copy_(data[name].reshape(-1))
-            elif role == "stats":
-                g = numel // 2
-                self.t[name][:g] = STATS_FILL[0]
-                self.t[name][g:] = STATS_FILL[1]
-            else:
-                self.t[name].fill_(float("nan"))
-
-    def check_guards(self, what):
-        for name, (o, numel, dtype, role, nbytes) in self.layout.items():
-            if role == "in":
-                continue
-            for side, g in zip(("front", "back"), self.guards(name)):
-                bad = (g != SENTINEL).nonzero()
-                assert bad.numel() == 0, f"{what}: {name} guard ({side}) overwritten at word {bad[0].item()}"
-
-    def ptr(self, name):
-        return self.t[name].data_ptr() if name in self.t else None
 
 
 # ---- the case as tensors -----------------------------------------------------------------------------------------
@@ -226,15 +141,11 @@ class Run:
         return lib.b200gan_conv2d_wgrad(ctypes.byref(self.g), a.ptr("x"), a.ptr("dy"), a.ptr("dw"), a.ptr("db"),
                                         a.ptr("ws"), self.algo, stream_handle)
 
-    def run_eager(self):
-        self.prepare()
-        st = torch.cuda.current_stream()
-        rc = self.call(st.cuda_stream)
-        torch.cuda.synchronize()
-        return rc
-
     def outputs(self):
-        return {k: v.clone() for k, v in self.arena.t.items() if self.arena.layout[k][3] != "in"}
+        return self.arena.outputs()
+
+    def check(self, what):
+        return check_outputs(self, self.outputs(), what)
 
 
 # ---- fp64 reference ------------------------------------------------------------------------------------------------
@@ -339,104 +250,7 @@ def epilogue_ref(run, conv, bound):
     return y, bound
 
 
-def first_failure(err, bound, layout):
-    ratio = err / bound.clamp_min(1e-300)
-    bad = (err > bound) | torch.isnan(err)
-    idx = bad.nonzero()
-    worst = ratio[~torch.isnan(ratio)].max().item() if ratio.numel() else 0.0
-    return (tuple(idx[0].tolist()) if idx.numel() else None), worst
-
-
-def check_elementwise(what, y, ref, bound, layout):
-    y64 = y.double().view_as(ref)
-    assert not torch.isnan(y64).any(), f"{what}: NaN at {layout} {tuple(torch.isnan(y64).nonzero()[0].tolist())} " \
-                                       "(an element never written, or a guard read)"
-    err = (y64 - ref).abs()
-    at, worst = first_failure(err, bound, layout)
-    assert at is None, f"{what}: |err| {err[at].item():.3e} > bound {bound[at].item():.3e} at {layout} {at}; " \
-                       f"worst |err|/bound {worst:.3g}"
-    return worst
-
-
-def check_not_vacuous(run, bound, ref_fn):
-    """median bound < the fp64 contribution of one filter tap (wgrad: of one image)"""
-    c = run.c
-    med = bound.median().item()
-    contrib = ref_fn().abs()
-    med_c = contrib[contrib > 0].median().item() if (contrib > 0).any() else 0.0
-    assert med < med_c, f"{c.id}: vacuous bound: median bound {med:.3e} >= median one-tap contribution {med_c:.3e}"
-
-
-# ---- profiler ------------------------------------------------------------------------------------------------------
-def short_name(name):
-    name = name.replace("(anonymous namespace)::", "")
-    if name.startswith("void "):
-        name = name[5:]
-    head = name.split("(", 1)[0]
-    return head.rsplit("::", 1)[-1] if "<" not in head else head[:head.index("<")].rsplit("::", 1)[-1] + \
-        head[head.index("<"):]
-
-
-_PROFILER_WARM = []
-
-
-def traced_kernels(fn):
-    from torch.profiler import ProfilerActivity, profile
-    if not _PROFILER_WARM:  # the first CUDA activity session of a process can come back empty
-        with profile(activities=[ProfilerActivity.CUDA]):
-            torch.ones(1, device="cuda").add_(1)
-            torch.cuda.synchronize()
-        _PROFILER_WARM.append(True)
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        fn()
-        torch.cuda.synchronize()
-    with tempfile.TemporaryDirectory() as d:
-        path = os.path.join(d, "trace.json")
-        prof.export_chrome_trace(path)
-        with open(path) as fh:
-            trace = json.load(fh)
-    out = []
-    for ev in trace.get("traceEvents", []):
-        if ev.get("cat") == "kernel":
-            out.append((short_name(ev["name"]), tuple(ev.get("args", {}).get("grid", ()))))
-    return out
-
-
-def kernel_matches(expected, seen):
-    return seen == expected if "<" in expected else cc.base_name(seen) == expected
-
-
-def check_route(run):
-    c = run.c
-    seen = []
-    # a CUDA activity session now and then comes back without some kernel records; the call is the same every time,
-    # so a route that differs from the table fails every attempt, while a lost record does not repeat
-    for _ in range(3):
-        run.prepare()
-        seen = traced_kernels(lambda: run.call(torch.cuda.current_stream().cuda_stream))
-        names = [n for n, _ in seen]
-        for n in names:
-            assert any(kernel_matches(e, n) for e in c.kernels), f"{c.id}: unexpected kernel {n} (table: {c.kernels})"
-        if all(any(kernel_matches(e, n) for n in names) for e in c.kernels):
-            break
-    if not seen:
-        return "the profiler recorded no CUDA kernel activity on this machine"
-    for e in c.kernels:
-        assert any(kernel_matches(e, n) for n in names), f"{c.id}: expected kernel {e}, trace has {names}"
-    if c.grid is not None and torch.cuda.get_device_properties(0).multi_processor_count == cc.NUM_SMS:
-        grids = [g for n, g in seen if kernel_matches(c.kernels[0], n)]
-        assert grids, f"{c.id}: no grid recorded for {c.kernels[0]}"
-        for got in grids:
-            for want, have in zip(c.grid, got):
-                assert want is None or want == have, f"{c.id}: grid {got}, table {c.grid}"
-    return None
-
-
 # ---- the per-case test ---------------------------------------------------------------------------------------------
-WORST = {}
-
-
 def check_outputs(run, outs, what):
     """every output of the call against the fp64 reference; returns the worst |err|/bound"""
     c = run.c
@@ -453,10 +267,10 @@ def check_outputs(run, outs, what):
             assert ((y.view(torch.int32) & 0x1FFF) == 0).all(), f"{what}: round_tf32 output not TF32-representable"
         if "stats" in outs:
             check_stats(run, y, outs["stats"], what)
-        check_not_vacuous(run, bound, lambda: conv_pass_ref(c, x, dy, one_tap(c, w)).double())
+        not_vacuous(what, bound, conv_pass_ref(c, x, dy, one_tap(c, w)).abs())
     elif c.pas == cc.DGRAD:
         worst = check_elementwise(what, outs["dx"], ref, bound, "(n, h, w, c)")
-        check_not_vacuous(run, bound, lambda: conv_pass_ref(c, x, dy, one_tap(c, w)))
+        not_vacuous(what, bound, conv_pass_ref(c, x, dy, one_tap(c, w)).abs())
     else:
         worst = check_elementwise(what, outs["dw"], ref, bound, "(param index)")
         db_ref = run.inp["dy"].double().sum((0, 1, 2))
@@ -464,7 +278,7 @@ def check_outputs(run, outs, what):
         n = c.N * c.P * c.Q
         check_elementwise(what + " db", outs["db"], db_ref, U * (n + 1100) * db_A, "(k,)")
         if c.N > 1:
-            check_not_vacuous(run, bound, lambda: conv_pass_ref(replace_n(c), x[:1], dy[:1], w))
+            not_vacuous(what, bound, conv_pass_ref(replace_n(c), x[:1], dy[:1], w).abs())
     return worst
 
 
@@ -503,45 +317,10 @@ def check_stats(run, y, stats, what):
 @pytest.mark.parametrize("case", cc.CASES, ids=lambda c: c.id)
 def test_conv_case(case):
     run = Run(case)
-    lib = run.lib
-    rc = run.run_eager()
-    if case.error:
-        assert rc == -2, f"{case.id}: expected B200GAN_E_BAD_ARG, rc = {rc}"
-        return
-    assert rc == 0, f"{case.id}: rc {rc}: {lib.b200gan_last_error().decode()}"
-    run.arena.check_guards(case.id)
-    eager = run.outputs()
-    worst = check_outputs(run, eager, case.id + " eager")
-
-    # route: kernel names and, where the table names one, the grid
-    skip_reason = check_route(run)
-
-    # CUDA graph on a side stream, replayed once; a launch on the legacy stream fails the capture
-    side = torch.cuda.Stream()
-    run.prepare()
-    torch.cuda.synchronize()
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph, stream=side):
-        rc = run.call(side.cuda_stream)
-    assert rc == 0, f"{case.id}: rc {rc} under capture: {lib.b200gan_last_error().decode()}"
-    run.prepare()
-    torch.cuda.synchronize()
-    graph.replay()
-    torch.cuda.synchronize()
-    run.arena.check_guards(case.id + " graph")
-    replay = run.outputs()
-    if case.deterministic:
-        for k, v in replay.items():
-            if k in ("stats", "db", "ws"):
-                continue
-            same = v.view(torch.int32) == eager[k].view(torch.int32)
-            assert same.all(), f"{case.id}: graph replay differs from the eager call in {k} at " \
-                               f"{tuple(same.logical_not().nonzero()[0].tolist())} (route marked deterministic)"
-    worst = max(worst, check_outputs(run, replay, case.id + " graph"))
-    WORST[case.id] = worst
-    print(f"\n{case.id}: worst |err|/bound {worst:.3g}")
-    if skip_reason:
-        pytest.skip(skip_reason)
+    # fp64 statistics and db are summed atomically; a route not marked deterministic repeats nothing bit for bit
+    varies = ("stats", "db", "ws") if case.deterministic else tuple(run.arena.t)
+    run_case(run, case.id, first_grid(case.kernels, case.grid), refuse=(-2,) if case.error else (), varies=varies,
+             ordered=False, num_sms=cc.NUM_SMS)
 
 
 # ---- rounding probe --------------------------------------------------------------------------------------------------

@@ -1,6 +1,6 @@
 """Every case of tests/chain_cases.py and tests/tail_cases.py, element by element against torch float64.
 
-Each case calls the C ABI directly on the guarded buffers of the convolution conformance test (Arena): inputs
+Each case calls the C ABI directly on the guarded buffers of tests/conformance.py (Arena) and runs its protocol: inputs
 between NaN guards, outputs started as NaN, sentinels around everything the library writes.  The fp64 statistics
 and sums buffers start at non-zero values, so a kernel that accumulates into them instead of overwriting them (the
 header's "OVERWRITTEN" contracts) fails; num_batches_tracked starts at 7.
@@ -21,180 +21,25 @@ import math
 
 import pytest
 import torch
-import torch.nn.functional as F
 
 import chain_cases as ch
 import tail_cases as tl
 from b200gan import _lib
-from test_gpu_conv_conformance import Arena, tf32_rna, traced_kernels
+from chain_cases import (ACT_CODE, BLOCK_PARTIAL, BN_EPS, MOMENTUM, NBT0, NEG_SLOPE, SLOPE, U, act_bound, act_grad,
+                         act_out64, bn_bwd_ref, bn_consts, chain_geom, conv_dgrad, conv_fwd, conv_wgrad, group_sums,
+                         per_image, running_ref)
+from conformance import Arena, check_elementwise, first_grid, run_case
+from tail_cases import tail_bwd_ref, tail_fwd_ref
 
 pytestmark = pytest.mark.gpu
 
-U = 2.0 ** -23
-SLOPE = 0.2
-MOMENTUM = 0.1
-BN_EPS = 0.8          # nn.BatchNorm2d(out, 0.8) of dcgan.py:82
-NBT0 = 7
-BLOCK_PARTIAL = 1032  # values a chain kernel sums in fp32 before its fp64 atomic: at most a tile's 1024 pixels
-ACT_CODE = {"none": _lib.ACT_NONE, "lrelu": _lib.ACT_LRELU, "relu": _lib.ACT_RELU, "tanh": _lib.ACT_TANH,
-            "sigmoid": _lib.ACT_SIGMOID}
-NEG_SLOPE = {"none": 1.0, "lrelu": SLOPE, "relu": 0.0}
-
-
-# ---- fp64 references (device-agnostic: tests/test_cpu_fused_case_table.py holds them to stock torch) -----------------
-def group_sums(t, G):
-    """[G][2][C] fp64 sum and sum of squares of t [N, ..., C] over each of G equal runs of images"""
-    t = t.double().reshape(G, -1, t.shape[-1])
-    return torch.stack([t.sum(1), (t * t).sum(1)], 1)
-
-
-def bn_consts(stats, gamma, beta, count, G, C, eps=BN_EPS):
-    """mean, biased var, rstd, scale, shift [G][C] from the batch sums, as nb_bn_consts forms them (in fp64)"""
-    st = stats.double().reshape(G, 2, C)
-    mean = st[:, 0] / count
-    var = (st[:, 1] / count - mean * mean).clamp_min(0)
-    rstd = 1 / torch.sqrt(var + eps)
-    ga = gamma.double() if gamma is not None else torch.ones_like(mean[0])
-    be = beta.double() if beta is not None else torch.zeros_like(mean[0])
-    sc = ga * rstd
-    return mean, var, rstd, sc, be - mean * sc
-
-
-def per_image(t, N):
-    """[G][C] -> [N][1][1][C]: the group's row for every image of the group"""
-    return t.repeat_interleave(N // t.shape[0], 0)[:, None, None, :]
-
-
-def running_ref(rm, rv, mean, var, count, momentum=MOMENTUM):
-    """one torch running-statistics update per group, in batch order"""
-    rm, rv = rm.double(), rv.double()
-    unb = var * count / (count - 1) if count > 1 else var
-    for g in range(mean.shape[0]):
-        rm = (1 - momentum) * rm + momentum * mean[g]
-        rv = (1 - momentum) * rv + momentum * unb[g]
-    return rm, rv
-
-
-def nchw(t):
-    return t.permute(0, 3, 1, 2)
-
-
-def nhwc(t):
-    return t.permute(0, 2, 3, 1)
-
-
-def conv_fwd(x, w, stride, pad):
-    return nhwc(F.conv2d(nchw(x), w, stride=stride, padding=pad))
-
-
-def conv_dgrad(dz, w, xshape, stride, pad):
-    N, H, W, C = xshape
-    return nhwc(torch.nn.grad.conv2d_input((N, C, H, W), w, nchw(dz), stride, pad))
-
-
-def conv_wgrad(x, dz, wshape, stride, pad):
-    return torch.nn.grad.conv2d_weight(nchw(x), wshape, nchw(dz), stride, pad)
-
-
-def bn_bwd_ref(G_, a, mean, rstd, sc, sums, count, cs, act):
-    """nb_dz: dz = scale * (G - sum G / count - ahat * sum G ahat / count) * chan_scale * act'(a), groups per image"""
-    N = a.shape[0]
-    m1, m2 = sums[:, 0] / count, sums[:, 1] / count
-    xh = (a - per_image(mean, N)) * per_image(rstd, N)
-    dA = per_image(sc, N) * (G_ - per_image(m1, N) - xh * per_image(m2, N))
-    return dA * cs * act_grad(act, a)
-
-
-def act_grad(act, a):
-    if act == "lrelu":
-        return torch.where(a > 0, 1.0, SLOPE).double()
-    if act == "relu":
-        return (a > 0).double()
-    return torch.ones_like(a, dtype=torch.float64)
-
-
-def act_mid32(act, v):
-    """the tail's LeakyReLU / ReLU in fp32, as the kernel computes it"""
-    if act == "lrelu":
-        return torch.where(v > 0, v, v * SLOPE)
-    if act == "relu":
-        return v.clamp_min(0)
-    return v
-
-
-def act_out64(act, v):
-    return {"none": lambda: v, "tanh": lambda: torch.tanh(v), "sigmoid": lambda: torch.sigmoid(v),
-            "lrelu": lambda: torch.where(v > 0, v, v * SLOPE), "relu": lambda: v.clamp_min(0)}[act]()
-
-
-def act_bound(act, pre, y, bound):
-    """carry an input bound through the activation and its fp32 evaluation (the conv suite's epilogue terms)"""
-    lip = {"none": 1.0, "lrelu": 1.0, "relu": 1.0, "tanh": 1.0, "sigmoid": 0.25}[act]
-    bound = lip * bound + U * y.abs()
-    if act == "tanh":
-        bound = bound + 4 * U * y.abs() + 2.0 ** -126
-    if act == "sigmoid":
-        bound = bound + U * (2 + 2 * pre.abs()) / 4 + 2 * U * y.abs()
-    return bound
-
-
-def tail_fwd_ref(a, ss, w, bias, act_mid, act_out):
-    """tail.cu forward: operands as the kernel feeds wgmma (RNA TF32); returns out, the linear part and A"""
-    C = a.shape[-1]
-    pre = (a.double() * ss[:C].double() + ss[C:].double()).float()     # fmaf(a, sc, sh)
-    x = tf32_rna(act_mid32(act_mid, pre)).double()
-    wr = tf32_rna(w).double()
-    conv = conv_fwd(x, wr, 1, 1)
-    A = conv_fwd(x.abs(), wr.abs(), 1, 1)
-    b = bias.double() if bias is not None else torch.zeros(w.shape[0], dtype=torch.float64, device=a.device)
-    return act_out64(act_out, conv + b), conv + b, A, b
-
-
-def tail_bwd_ref(a, mr, ss, w, g, act_mid, neg_branch):
-    """tail.cu backward with the activation's derivative on `neg_branch` (bool mask: take the negative side)"""
-    C, K = a.shape[-1], w.shape[0]
-    a64 = a.double()
-    sc, sh, mean, rstd = ss[:C].double(), ss[C:].double(), mr[:C].double(), mr[C:].double()
-    pre = a64 * sc + sh
-    neg = NEG_SLOPE[act_mid]
-    y = torch.where(neg_branch, pre * neg, pre)
-    dy = conv_dgrad(g.double(), w.double(), a.shape, 1, 1)
-    dz = torch.where(neg_branch, dy * neg, dy)
-    xh = (a64 - mean) * rstd
-    total = a.numel() // C
-    s1, s2 = dz.sum((0, 1, 2)), (dz * xh).sum((0, 1, 2))
-    da = sc * (dz - s1 / total - xh * (s2 / total))
-    dw = conv_wgrad(y, g.double(), (K, C, 3, 3), 1, 1)
-    return dict(da=da, s1=s1, s2=s2, dw=dw, db=g.double().sum((0, 1, 2)), y=y, dz=dz, xh=xh, pre=pre, dy=dy)
-
 
 # ---- checks ---------------------------------------------------------------------------------------------------------
-def check(what, got, ref, bound, alt=None):
-    """|got - ref| <= bound element by element; where `alt` is not NaN, matching alt instead is accepted"""
-    got = got.double().reshape(ref.shape)
-    assert not torch.isnan(got).any(), f"{what}: NaN at {tuple(torch.isnan(got).nonzero()[0].tolist())} " \
-                                       "(an element never written, or a guard read)"
-    err = (got - ref).abs()
-    if alt is not None:
-        err = torch.where(torch.isnan(alt), err, torch.minimum(err, (got - alt).abs()))
-    bad = (err > bound).nonzero()
-    if bad.numel():
-        at = tuple(bad[0].tolist())
-        raise AssertionError(f"{what}: |err| {err[at].item():.3e} > bound {bound[at].item():.3e} at {at}; got "
-                             f"{got[at].item():.9g}, fp64 {ref[at].item():.9g}")
-    ratio = err / bound.clamp_min(1e-300)
-    return ratio.max().item() if ratio.numel() else 0.0
-
-
 def check_sums(what, got, ref, bound):
-    return check(what + " (an OVERWRITTEN buffer: accumulating onto its old contents fails)", got, ref, bound)
+    return check_elementwise(what + " (an OVERWRITTEN buffer: accumulating onto its old contents fails)", got, ref, bound)
 
 
 # ---- chain runs ------------------------------------------------------------------------------------------------------
-def chain_geom(c):
-    return _lib.ConvGeom(c.N, c.H, c.W, c.C, c.K, c.R, c.R, c.stride, 1, 1, 1, 1, _lib.PAD_ZERO, 1, 0, c.P, c.Q)
-
-
 class ChainRun:
     def __init__(self, c, seed=0):
         self.c = c
@@ -379,8 +224,8 @@ class ChainRun:
         e = a.abs() * per_image(esc, N) + per_image(esh, N) + U * x.abs() if self.has_bn else torch.zeros_like(x)
         return x.reshape(self.a.shape), e.reshape(self.a.shape)
 
-    def check(self, outs, what):
-        return getattr(self, "_check_" + self.c.op)(outs, what)
+    def check(self, what):
+        return getattr(self, "_check_" + self.c.op)(self.outputs(), what)
 
     def _check_running(self, outs, what):
         """running statistics and num_batches_tracked; the worst |err|/bound"""
@@ -389,9 +234,9 @@ class ChainRun:
         mean, var, rstd, *_ = self.consts()
         rm, rv = running_ref(self.rm0.cuda(), self.rv0.cuda(), mean, var, self.count)
         unb = var * self.count / (self.count - 1)
-        worst = check(what + " running_mean", outs["running_mean"], rm,
+        worst = check_elementwise(what + " running_mean", outs["running_mean"], rm,
                       8 * U * (self.rm0.cuda().double().abs() + mean.abs().sum(0)) + 1e-30)
-        worst = max(worst, check(what + " running_var", outs["running_var"], rv,
+        worst = max(worst, check_elementwise(what + " running_var", outs["running_var"], rv,
                                  8 * U * (self.rv0.cuda().double().abs() + unb.abs().sum(0)) + 1e-30))
         assert outs["nbt"].item() == NBT0 + self.G, f"{what}: num_batches_tracked {outs['nbt'].item()}"
         return worst
@@ -412,7 +257,7 @@ class ChainRun:
             s = self.cs.double().view(c.N, 1, 1, c.K)
             y = y * s
             bound = bound * s.abs() + U * y.abs()
-        worst = check(what + " y", outs["y"], y, bound)
+        worst = check_elementwise(what + " y", outs["y"], y, bound)
         if c.out_stats:
             yk = outs["y"].double().view(self.G, -1, c.K)
             ref = torch.stack([yk.sum(1), (yk * yk).sum(1)], 1)
@@ -426,7 +271,7 @@ class ChainRun:
         shape = (c.N, c.H, c.W, c.C)
         ref = conv_dgrad(dz, w, shape, c.stride, 1)
         bound = U * (c.R * c.R * c.K + 4) * conv_dgrad(dz.abs(), w.abs(), shape, c.stride, 1)
-        worst = check(what + " g_out", outs["g_out"], ref, bound)
+        worst = check_elementwise(what + " g_out", outs["g_out"], ref, bound)
         if c.op == "dgrad" and c.sums:
             mean, var, rstd, *_ = self.consts()
             a = self.a.double()
@@ -454,7 +299,7 @@ class ChainRun:
             conv_wgrad(e, dz.abs(), shape, c.stride, 1)
         if self.unused_ws:
             assert torch.isnan(outs["ws"]).all(), f"{what}: a workspace the plan does not use was written"
-        return check(what + " dw", outs["dw"], ref, bound)
+        return check_elementwise(what + " dw", outs["dw"], ref, bound)
 
     def _check_dz(self, outs, what):
         c = self.c
@@ -472,10 +317,10 @@ class ChainRun:
         else:
             ref = G_ * cs * act_grad(c.act, a)
             bound = 2 * U * ref.abs()
-        worst = check(what + " dz", outs["dz"], ref, bound)
+        worst = check_elementwise(what + " dz", outs["dz"], ref, bound)
         if c.db:
             rows = N * c.H * c.W
-            worst = max(worst, check(what + " db", outs["db"], ref.sum((0, 1, 2)),
+            worst = max(worst, check_elementwise(what + " db", outs["db"], ref.sum((0, 1, 2)),
                                      bound.sum((0, 1, 2)) + U * (rows + 16) * ref.abs().sum((0, 1, 2))))
         return worst
 
@@ -484,7 +329,7 @@ class ChainRun:
         x, e = self.staged_x()
         out = x.permute(0, 2, 1) if c.nchw else x
         bnd = e.permute(0, 2, 1) if c.nchw else e
-        worst = check(what + " out", outs["out"], out, bnd)
+        worst = check_elementwise(what + " out", outs["out"], out, bnd)
         return max(worst, self._check_running(outs, what))
 
     def _check_tail_bwd(self, outs, what):
@@ -556,16 +401,17 @@ class TailRun:
         return rb
 
     def outputs(self):
-        return {k: v.clone() for k, v in self.arena.t.items() if self.arena.layout[k][3] != "in"}
+        return self.arena.outputs()
 
-    def check(self, outs, what):
+    def check(self, what):
+        outs = self.outputs()
         c = self.c
         C, K = c.C, c.K
         # forward
         out, pre, A, b = tail_fwd_ref(self.a, self.ss, self.w, self.bias, c.act_mid, c.act_out)
         bound = 2.0 ** -22 * (math.ceil(9 * C / 8) + 9 + 4) * A
         bound = bound + U * (pre.abs() + b.abs())
-        worst = check(what + " out", outs["out"], out, act_bound(c.act_out, pre, out, bound))
+        worst = check_elementwise(what + " out", outs["out"], out, act_bound(c.act_out, pre, out, bound))
         # backward: both branches of the activation's derivative where the pre-activation is within ulps of 0
         a64 = self.a.double()
         pre64 = a64 * self.ss[:C].double() + self.ss[C:].double()
@@ -586,8 +432,8 @@ class TailRun:
         bs1 = U * m * S(dz.abs()) + S(bdz) + S(flip)
         bs2 = U * m * S((dz * xh).abs()) + S(bdz * xh.abs() + dz.abs() * exh) + S(flip * xh.abs())
         if c.dgb:
-            worst = max(worst, check(what + " dgamma", outs["dgb"][:C], r["s2"], bs2 + U * r["s2"].abs()))
-            worst = max(worst, check(what + " dbeta", outs["dgb"][C:], r["s1"], bs1 + U * r["s1"].abs()))
+            worst = max(worst, check_elementwise(what + " dgamma", outs["dgb"][:C], r["s2"], bs2 + U * r["s2"].abs()))
+            worst = max(worst, check_elementwise(what + " dbeta", outs["dgb"][C:], r["s1"], bs1 + U * r["s1"].abs()))
         sc = self.ss[:C].double()
         m1, m2 = r["s1"] / total, r["s2"] / total
         bda = sc.abs() * (bdz + bs1 / total + exh * m2.abs() + xh.abs() * bs2 / total +
@@ -595,100 +441,34 @@ class TailRun:
         if c.rtf:
             bda = bda + 2.0 ** -11 * (r["da"].abs() + bda)
         alt = torch.where(near0, ra["da"], torch.full_like(r["da"], float("nan"))) if ra is not None else None
-        worst = max(worst, check(what + " da", outs["da"], r["da"], bda, alt))
+        worst = max(worst, check_elementwise(what + " da", outs["da"], r["da"], bda, alt=alt))
         if c.rtf:
             assert ((outs["da"].view(torch.int32) & 0x1FFF) == 0).all(), f"{what}: round_tf32 da not TF32-representable"
         shape = (K, C, 3, 3)
         y_flip = (ra["y"] - r["y"]).abs() * near0 if ra is not None else torch.zeros_like(r["y"])
         bdw = U * (m + 4) * conv_wgrad(r["y"].abs(), gk.abs(), shape, 1, 1) + \
             conv_wgrad(U * r["pre"].abs() + y_flip, gk.abs(), shape, 1, 1)
-        worst = max(worst, check(what + " dw", outs["dw"], r["dw"], bdw))
+        worst = max(worst, check_elementwise(what + " dw", outs["dw"], r["dw"], bdw))
         if c.db:
-            worst = max(worst, check(what + " db", outs["db"], r["db"], U * (m + 4) * S(gk.abs())))
+            worst = max(worst, check_elementwise(what + " db", outs["db"], r["db"], U * (m + 4) * S(gk.abs())))
         return worst
 
 
 # ---- the per-case test ---------------------------------------------------------------------------------------------
-def check_route(run, kernels, grid):
-    """the family's kernels of one call, in launch order, and the first one's grid on a 132-SM device"""
-    c = run.c
-    marker = torch.zeros(1, device="cuda")
-    names, seen = [], []
-    # the first launch of a profiler session can lose its kernel record (see test_gpu_norm_conformance.check_route):
-    # a marker goes first; a record lost anyway does not repeat, a route that differs from the table does
-    for _ in range(3):
-        run.prepare()
-        seen = [(n, g) for n, g in traced_kernels(lambda: (marker.zero_(), run.call(
-            torch.cuda.current_stream().cuda_stream))) if n.startswith(("nbk_", "tail_"))]
-        names = [n for n, _ in seen]
-        if names == list(kernels):
-            break
-    if not seen:
-        return "the profiler recorded no CUDA kernel activity on this machine"
-    assert names == list(kernels), f"{c.id}: trace {names}, table {list(kernels)}"
-    if grid is not None and torch.cuda.get_device_properties(0).multi_processor_count == ch.NUM_SMS:
-        assert tuple(seen[0][1]) == tuple(grid), f"{c.id}: {names[0]} grid {seen[0][1]}, table {grid}"
-    return None
-
-
 # fp64 sums and fp32 atomics (tail.cu's backward: sums -> da, dgamma_dbeta; dw, db), running statistics from them;
 # a chain wgrad's dw repeats only with the slab workspace
-ALWAYS_VARIES = {"out_stats", "sums", "db", "ws", "dgb", "running_mean", "running_var", "nbt"}
-MAY_VARY = {"dw", "da"}
-
-
-def run_case(run, kernels, grid, deterministic, bad_rc):
-    c = run.c
-    lib = run.lib
-    run.prepare()
-    before = run.outputs()
-    rc = run.call(torch.cuda.current_stream().cuda_stream)
-    torch.cuda.synchronize()
-    if c.error:
-        assert rc in bad_rc, f"{c.id}: expected a refusal, rc = {rc}"
-        run.arena.check_guards(c.id)
-        after = run.outputs()
-        for k, v in before.items():
-            same = (v.view(torch.uint8) == after[k].view(torch.uint8)).all()
-            assert same, f"{c.id}: refused call wrote {k}"
-        return
-    assert rc == 0, f"{c.id}: rc {rc}: {lib.b200gan_last_error().decode()}"
-    run.arena.check_guards(c.id)
-    eager = run.outputs()
-    worst = run.check(eager, c.id + " eager")
-
-    skip_reason = check_route(run, kernels, grid)
-
-    # CUDA graph on a side stream, replayed once
-    side = torch.cuda.Stream()
-    run.prepare()
-    torch.cuda.synchronize()
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph, stream=side):
-        rc = run.call(side.cuda_stream)
-    assert rc == 0, f"{c.id}: rc {rc} under capture: {lib.b200gan_last_error().decode()}"
-    run.prepare()
-    torch.cuda.synchronize()
-    graph.replay()
-    torch.cuda.synchronize()
-    run.arena.check_guards(c.id + " graph")
-    replay = run.outputs()
-    for k, v in replay.items():
-        if k in ALWAYS_VARIES or (k in MAY_VARY and not deterministic):
-            continue
-        same = v.view(torch.uint8) == eager[k].view(torch.uint8)
-        assert same.all(), f"{c.id}: graph replay differs from the eager call in {k} (marked deterministic)"
-    worst = max(worst, run.check(replay, c.id + " graph"))
-    print(f"\n{c.id}: worst |err|/bound {worst:.3g}, kernels {list(kernels)}")
-    if skip_reason:
-        pytest.skip(skip_reason)
+ALWAYS_VARIES = ("out_stats", "sums", "db", "ws", "dgb", "running_mean", "running_var", "nbt")
+MAY_VARY = ("dw", "da")
+FAMILY = ("nbk_", "tail_")
 
 
 @pytest.mark.parametrize("case", ch.CASES, ids=lambda c: c.id)
 def test_chain_case(case):
-    run_case(ChainRun(case), case.kernels, case.grid, case.deterministic, (-2,))
+    run_case(ChainRun(case), case.id, first_grid(case.kernels, case.grid), refuse=(-2,) if case.error else (),
+             varies=ALWAYS_VARIES + (() if case.deterministic else MAY_VARY), family=FAMILY, num_sms=ch.NUM_SMS)
 
 
 @pytest.mark.parametrize("case", tl.CASES, ids=lambda c: c.id)
 def test_tail_case(case):
-    run_case(TailRun(case), case.kernels, None, False, (-1, -2))
+    run_case(TailRun(case), case.id, first_grid(case.kernels, None), refuse=(-1, -2) if case.error else (),
+             varies=ALWAYS_VARIES + MAY_VARY, family=FAMILY)

@@ -1,8 +1,8 @@
 """The vanilla GAN discriminator (gan.py:64-80, bgan.py:66-80, aae.py:90-104) on the MLP critic kernels' Sigmoid mode:
 b200gan_mlp_disc_fwd / _bwd element by element against torch float64, then functional.MlpDiscriminatorFn end to end.
 
-Conformance: each case calls the C ABI on the guarded buffers of the convolution conformance test (Arena) and is
-checked with the references and bounds of tests/test_gpu_critic_conformance.py.  Bounds added here:
+Conformance: each case calls the C ABI on the guarded buffers of tests/conformance.py (Arena), runs its protocol and is
+checked with the critic's references and bounds (tests/critic_cases.py).  Bounds added here:
   y = sigmoid(z):  the fp64 logit z is within ez of the kernel's (the critic's row-dot bound); sigmoid' = y (1 - y)
                    changes by at most a factor exp(ez) over that interval; expf is within 2 ulp and 1 + e and the
                    division round once each: |y - sigmoid(z)| <= y (1 - y) ez exp(ez) + 4 u y.
@@ -24,10 +24,9 @@ import torch
 
 import critic_cases as cr
 from b200gan import _lib
+from conformance import Arena, check_elementwise, first_grid, not_vacuous, run_case
 from conftest import rel_err
-from test_gpu_conv_conformance import Arena, check_elementwise
-from test_gpu_critic_conformance import (U, check_mask, check_route, critic_bwd_ref, mask, rowdot_n)
-from test_gpu_stream_conformance import not_vacuous
+from critic_cases import U, check_mask, critic_bwd_ref, mask, rowdot_n
 
 pytestmark = pytest.mark.gpu
 F32 = torch.float32
@@ -161,7 +160,7 @@ class Run:
         self.arena.prepare(self.data)
 
     def outputs(self):
-        return {k: v.clone() for k, v in self.arena.t.items() if self.arena.layout[k][3] != "in"}
+        return self.arena.outputs()
 
     def call(self, st):
         p, d, L = self.arena.ptr, ctypes.byref(self.d), self.lib
@@ -212,47 +211,13 @@ class Run:
 @pytest.mark.parametrize("case", CASES, ids=lambda c: c.id)
 def test_disc_case(case):
     run = Run(case)
-    run.prepare()
-    before = run.outputs()
-    rc = run.call(torch.cuda.current_stream().cuda_stream)
-    torch.cuda.synchronize()
-    if case.error:
-        assert rc == -2, f"{case.id}: expected B200GAN_E_BAD_ARG, rc {rc}"
-        run.arena.check_guards(case.id)
-        after = run.outputs()
-        for k, v in before.items():
-            assert torch.equal(v.view(torch.int32), after[k].view(torch.int32)), f"{case.id}: refused call wrote {k}"
-        return
-    assert rc == 0, f"{case.id}: rc {rc}: {run.lib.b200gan_last_error().decode()}"
-    run.arena.check_guards(case.id)
     z = run.z64
     if case.logits == "near0":
         assert z.abs().max() < 0.01, case.id
     elif case.logits.startswith("sat"):
         assert z.abs().min() > 20 and (z > 0).all() == (case.logits == "sat_pos"), case.id
-    eager = run.outputs()
-    worst = run.check(case.id + " eager")
-
-    skip_reason = check_route(run)
-
-    side = torch.cuda.Stream()
-    run.prepare()
-    torch.cuda.synchronize()
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph, stream=side):
-        rc = run.call(side.cuda_stream)
-    assert rc == 0, f"{case.id}: rc {rc} under capture"
-    run.prepare()
-    torch.cuda.synchronize()
-    graph.replay()
-    torch.cuda.synchronize()
-    run.arena.check_guards(case.id + " graph")
-    for k, v in run.outputs().items():
-        assert torch.equal(v.view(torch.int32), eager[k].view(torch.int32)), f"{case.id}: graph replay differs in {k}"
-    worst = max(worst, run.check(case.id + " graph"))
-    print(f"\n{case.id}: worst |err|/bound {worst:.3g}, grid {case.grid}")
-    if skip_reason:
-        pytest.skip(skip_reason)
+    run_case(run, case.id, first_grid(case.kernels, case.grid), refuse=(-2,) if case.error else (),
+             family=tuple(cr.KERNEL.values()), num_sms=cr.NUM_SMS)
 
 
 # ---- the module path ------------------------------------------------------------------------------------------------

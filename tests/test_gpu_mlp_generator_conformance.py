@@ -1,7 +1,7 @@
 """Every case of tests/generator_cases.py (csrc/mlp_generator/mlp_generator.cu), element by element against fp64.
 
-Each case calls the C ABI on the guarded buffers of the convolution conformance test (Arena): outputs and workspaces
-started as NaN, sentinels around everything the library writes.  The running statistics are inputs the forward updates
+Each case calls the C ABI on the guarded buffers of tests/conformance.py (Arena) and runs its protocol: outputs and
+workspaces started as NaN, sentinels around everything the library writes.  The running statistics are inputs the forward updates
 in place; they are read back and checked against the fp64 update.
 
 The forward is checked layer by layer: each layer's reference starts from the kernel's own previous activations (the
@@ -9,11 +9,10 @@ saved region), so a bound covers one layer's rounding.  A forward without a save
 from the last hidden activation it leaves in its workspace and must repeat the saved-mode call bit for bit.  The
 backward reads a saved region formed from the fp64 forward and rounded to fp32, so its reference is exact in its
 inputs; bounds follow the conv suite: an fp32 chain of n products with s partials added outside it is within
-2^-23 (n + s + 4) A of fp64, A the same sum over |terms|, carried from layer to layer (mmr).
+2^-23 (n + s + 4) A of fp64, A the same sum over |terms|, carried from layer to layer (generator_cases.mmr).
 tests/test_cpu_mlp_generator.py holds the references to torch float64 autograd.
 """
 import ctypes
-import math
 import re
 
 import pytest
@@ -21,143 +20,10 @@ import torch
 
 import generator_cases as gc
 from b200gan import _lib
-from test_gpu_conv_conformance import Arena, check_elementwise, traced_kernels
-from test_gpu_critic_conformance import z
-from test_gpu_stream_conformance import not_vacuous
+from conformance import Arena, check_elementwise, first_grid, not_vacuous, run_case
+from generator_cases import EPS, F32, MOMENTUM, U, f32, gen_bwd_ref, gen_fwd_ref, make, saved_of, split_saved
 
 pytestmark = pytest.mark.gpu
-
-U = 2.0 ** -23
-EPS, MOMENTUM = 0.8, 0.1     # BatchNorm1d(o, 0.8) of wgan_gp.py:49 / gan.py:45, torch's default momentum
-F32 = torch.float32
-
-
-def f32(v):
-    return torch.tensor(v, dtype=F32).item()
-
-
-# ---- inputs and fp64 references (device-agnostic) ------------------------------------------------------------------
-def make(c, seed=0):
-    """the case's fp32 inputs on the CPU: z, W{l}, b{l}, and per norm layer gamma, beta, rm, rv, nbt; dout"""
-    g = torch.Generator().manual_seed(seed)
-    rn = lambda *s, scale=1.0: torch.randn(*s, generator=g) * scale  # noqa: E731
-    N, w = max(c.N, 1), c.widths
-    P = {"z": rn(N, w[0])}
-    for l in range(c.L):
-        P[f"W{l}"] = rn(w[l + 1], w[l], scale=1 / math.sqrt(w[l]))
-        P[f"b{l}"] = rn(w[l + 1], scale=0.2)
-        if c.has_norm[l]:
-            P[f"gamma{l}"] = 1 + rn(w[l + 1], scale=0.2)
-            P[f"beta{l}"] = rn(w[l + 1], scale=0.2)
-            P[f"rm{l}"] = rn(w[l + 1], scale=0.1)
-            P[f"rv{l}"] = 1 + torch.rand(w[l + 1], generator=g)
-            P[f"nbt{l}"] = torch.tensor([7], dtype=torch.int64)
-    P["dout"] = rn(N, w[-1])
-    return P
-
-
-def mask(a, slope):
-    return torch.where(a > 0, torch.ones_like(a), torch.full_like(a, slope))
-
-
-def gen_fwd_ref(P, c, acts=None):
-    """fp64 forward of case c from its (fp32) inputs P.  Per layer: x (the layer's input), h, and for a norm layer mean,
-    var, rstd, xhat, the updated running statistics; y, a; and out.  acts: the kernel's activations, each layer then
-    starts from the kernel's previous layer."""
-    D = {k: v.double() for k, v in P.items() if v.is_floating_point()}
-    slope, N = f32(c.slope), D["z"].shape[0]
-    x, layers = D["z"], []
-    for l in range(c.L):
-        r = {"x": x, "h": x @ D[f"W{l}"].t() + D[f"b{l}"]}
-        if l == c.L - 1:
-            r["out"] = torch.tanh(r["h"])
-        else:
-            y = r["h"]
-            if c.has_norm[l]:
-                mean = y.mean(0)
-                var = ((y - mean) ** 2).mean(0)
-                r.update(mean=mean, var=var, rstd=1 / torch.sqrt(var + f32(EPS)))
-                r["xhat"] = (y - mean) * r["rstd"]
-                y = r["xhat"] * D[f"gamma{l}"] + D[f"beta{l}"]
-                m = f32(MOMENTUM)
-                r["rm"] = (1 - m) * D[f"rm{l}"] + m * mean
-                r["rv"] = (1 - m) * D[f"rv{l}"] + m * var * N / (N - 1)
-            r["y"], r["a"] = y, y * mask(y, slope)
-            x = r["a"] if acts is None or acts[l] is None else acts[l].double()
-        layers.append(r)
-    return layers
-
-
-def saved_of(c, layers):
-    """the saved region (include/b200gan.h: a_l, then xhat and rstd of each norm layer) from a forward's layers"""
-    hid = [layers[l] for l in range(c.L - 1)]
-    parts = [r["a"] for r in hid] + [r["xhat"] for r, n in zip(hid, c.has_norm) if n] + \
-        [r["rstd"] for r, n in zip(hid, c.has_norm) if n]
-    return torch.cat([p.reshape(-1) for p in parts]) if parts else torch.zeros(0, dtype=torch.float64)
-
-
-def split_saved(c, saved, N):
-    """saved -> (acts, xhats, rstds), per hidden layer (None for layers without a norm)"""
-    w, o = c.widths, 0
-    acts, xh, rs = [], [None] * (c.L - 1), [None] * (c.L - 1)
-    for l in range(c.L - 1):
-        acts.append(saved[o:o + N * w[l + 1]].view(N, w[l + 1]))
-        o += N * w[l + 1]
-    for l in range(c.L - 1):
-        if c.has_norm[l]:
-            xh[l] = saved[o:o + N * w[l + 1]].view(N, w[l + 1])
-            o += N * w[l + 1]
-    for l in range(c.L - 1):
-        if c.has_norm[l]:
-            rs[l] = saved[o:o + w[l + 1]]
-            o += w[l + 1]
-    return acts, xh, rs
-
-
-def mmr(A, eA, B, n):
-    """A @ B in fp64 for an operand A off by eA and an exact B: the bound of the fp32 GEMM's own rounding, plus the
-    operand errors carried as independent ones (root-sum-square); and the mean magnitude of one term"""
-    S = A.abs() @ B.abs()
-    return A @ B, U * (n + 4) * S + torch.sqrt((eA * eA) @ (B * B)), S / max(A.shape[-1], 1)
-
-
-def rss(e, dim=0):
-    return torch.sqrt((e * e).sum(dim))
-
-
-def gen_bwd_ref(c, dout, out, z_, W, gamma, acts, xhat, rstd):
-    """fp64 backward for dout with bounds: name -> (value, bound[, mean magnitude of one term]) for dz, dW{l}, db{l},
-    dgamma{l}, dbeta{l}; every operand but the gradient itself is exact (the kernel reads the same fp32 values).  The
-    gradient's own error is carried from layer to layer as independent per-element errors (mmr, rss): the worst case of
-    correlated errors grows by the row sums of |W| per layer and is vacuous after five layers.  Each carried bound is
-    itself a worst case of its layer's rounding, far above the error a kernel makes."""
-    slope, N = f32(c.slope), dout.shape[0]
-    g = dout * (1 - out * out)
-    eg = U * (3 * g.abs() + 2 * dout.abs() * out * out)
-    r = {}
-    for l in range(c.L - 1, -1, -1):
-        ain = z_ if l == 0 else acts[l - 1]
-        r[f"dW{l}"] = mmr(g.t(), eg.t(), ain, N)
-        r[f"db{l}"] = (g.sum(0), U * (N + 4) * g.abs().sum(0) + rss(eg))
-        da, eda, _ = mmr(g, eg, W[l], W[l].shape[0])
-        if l == 0:
-            r["dz"] = (da, eda)
-            break
-        mk = mask(ain, slope)
-        dy, edy = da * mk, eda * mk.abs() + U * (da * mk).abs()
-        if c.has_norm[l - 1]:
-            xh, k = xhat[l - 1], gamma[l - 1] * rstd[l - 1]
-            s1, s2 = dy.sum(0), (dy * xh).sum(0)
-            es1 = U * (N + 4) * dy.abs().sum(0) + rss(edy)
-            es2 = U * (N + 4) * (dy * xh).abs().sum(0) + rss(edy * xh)
-            r[f"dbeta{l - 1}"], r[f"dgamma{l - 1}"] = (s1, es1), (s2, es2)
-            inner = dy - s1 / N - xh * s2 / N
-            g = k * inner
-            eg = k.abs() * (edy + es1 / N + xh.abs() * es2 / N
-                            + 6 * U * (dy.abs() + (s1 / N).abs() + (xh * s2 / N).abs())) + 2 * U * g.abs()
-        else:
-            g, eg = dy, edy
-    return r
 
 
 # ---- the case as buffers ---------------------------------------------------------------------------------------------
@@ -242,7 +108,7 @@ class Run:
 
     def check(self, what):
         c, t, N = self.c, self.arena.t, self.c.N
-        worst = 0.0
+        worst = self.check_against_kept(what) if c.op == "fwd" and not c.keep else 0.0
         if c.op == "bwd":
             D = {k: v.double() for k, v in self.data.items() if v.is_floating_point()}
             acts, xh, rs = split_saved(c, D["saved"], N)
@@ -307,76 +173,24 @@ class Run:
         return worst
 
 
-# ---- the per-case test -----------------------------------------------------------------------------------------------
-def check_route(run):
-    c = run.c
-    seen = []
-    for _ in range(3):
-        run.prepare()
-        seen = [(n, tuple(g)) for n, g in traced_kernels(lambda: run.call(torch.cuda.current_stream().cuda_stream))
-                if n in gc.KERNEL.values()]
-        if [n for n, _ in seen] == list(c.kernels):
-            break
-    if not seen:
-        return "the profiler recorded no CUDA kernel activity on this machine"
-    assert [n for n, _ in seen] == list(c.kernels), f"{c.id}: trace {seen}, table {c.kernels}"
-    if torch.cuda.get_device_properties(0).multi_processor_count == gc.NUM_SMS:
-        assert seen[0][1] == c.grid, f"{c.id}: grid {seen[0][1]}, table {c.grid}"
-    return None
-
-
-@pytest.mark.parametrize("case", gc.CASES, ids=lambda c: c.id)
-def test_generator_case(case):
-    run = Run(case)
-    lib = run.lib
-    run.prepare()
-    before = run.outputs()
-    rc = run.call(torch.cuda.current_stream().cuda_stream)
-    torch.cuda.synchronize()
-    if case.error:
-        assert rc == -2, f"{case.id}: expected B200GAN_E_BAD_ARG, rc {rc}"
-        run.arena.check_guards(case.id)
-        after = run.outputs()
-        for k, v in before.items():
-            assert torch.equal(v.view(torch.int32), after[k].view(torch.int32)), f"{case.id}: refused call wrote {k}"
-        return
-    assert rc == 0, f"{case.id}: rc {rc}: {lib.b200gan_last_error().decode()}"
-    run.arena.check_guards(case.id)
-    eager = run.outputs()
-    worst = run.check(case.id + " eager")
-
-    if case.op == "fwd" and not case.keep:
-        # the same call with a saved region computes the same out and running statistics, bit for bit
-        kept = Run(gc.Case(case.name, "fwd", case.N, case.widths, case.norms, case.slope))
+    def check_against_kept(self, what):
+        """the same call with a saved region computes the same out and running statistics, bit for bit"""
+        c = self.c
+        kept = Run(gc.Case(c.name, "fwd", c.N, c.widths, c.norms, c.slope))
         kept.prepare()
         assert kept.call(torch.cuda.current_stream().cuda_stream) == 0
         torch.cuda.synchronize()
-        worst = max(worst, kept.check(case.id + " kept"))
+        worst = kept.check(what + " kept")
+        mine = self.outputs()
         for k, v in kept.outputs().items():
-            if k in eager and k != "ws":
-                assert torch.equal(v.view(torch.int32), eager[k].view(torch.int32)), f"{case.id}: {k} differs " \
+            if k in mine and k != "ws":
+                assert torch.equal(v.view(torch.int32), mine[k].view(torch.int32)), f"{what}: {k} differs " \
                     "from the forward that keeps a saved region"
+        return worst
 
-    skip_reason = check_route(run)
 
-    side = torch.cuda.Stream()
-    run.prepare()
-    torch.cuda.synchronize()
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph, stream=side):
-        rc = run.call(side.cuda_stream)
-    assert rc == 0, f"{case.id}: rc {rc} under capture: {lib.b200gan_last_error().decode()}"
-    run.prepare()
-    torch.cuda.synchronize()
-    graph.replay()
-    torch.cuda.synchronize()
-    run.arena.check_guards(case.id + " graph")
-    for k, v in run.outputs().items():
-        if k == "ws":
-            continue
-        same = v.view(torch.int32) == eager[k].view(torch.int32)
-        assert same.all(), f"{case.id}: graph replay differs from the eager call in {k}"
-    worst = max(worst, run.check(case.id + " graph"))
-    print(f"\n{case.id}: worst |err|/bound {worst:.3g}, grid {case.grid}")
-    if skip_reason:
-        pytest.skip(skip_reason)
+# ---- the per-case test -----------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("case", gc.CASES, ids=lambda c: c.id)
+def test_generator_case(case):
+    run_case(Run(case), case.id, first_grid(case.kernels, case.grid), refuse=(-2,) if case.error else (),
+             varies=("ws",), family=tuple(gc.KERNEL.values()), num_sms=gc.NUM_SMS)

@@ -11,14 +11,12 @@
 Outputs land in NaN-filled buffers between NaN guard regions: every element must be written, nothing around it."""
 import ctypes
 import copy
-import json
-import os
-import tempfile
 
 import pytest
 import torch
 import torch.nn.functional as tf
 
+from conformance import check_route, traced_kernels
 from conftest import rel_err
 
 pytestmark = pytest.mark.gpu
@@ -52,34 +50,6 @@ def _guarded(shape, dtype=torch.float32, cl=True):
 
 def _guards_intact(buf):
     return bool(torch.isnan(buf[:GUARD]).all()) and bool(torch.isnan(buf[-GUARD:]).all())
-
-
-_WARM = []
-
-
-def traced_kernels(fn):
-    """names of the CUDA kernels `fn` launches, template arguments kept"""
-    from torch.profiler import ProfilerActivity, profile
-    if not _WARM:  # the first CUDA activity session of a process can come back empty
-        with profile(activities=[ProfilerActivity.CUDA]):
-            torch.ones(1, device="cuda").add_(1)
-            torch.cuda.synchronize()
-        _WARM.append(True)
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        torch.ones(1, device="cuda").add_(1)  # the first kernel record of a session can be lost: a sacrificial one
-        fn()
-        torch.cuda.synchronize()
-    with tempfile.TemporaryDirectory() as d:
-        path = os.path.join(d, "trace.json")
-        prof.export_chrome_trace(path)
-        with open(path) as fh:
-            trace = json.load(fh)
-    out = []
-    for ev in trace.get("traceEvents", []):
-        if ev.get("cat") == "kernel" and "b200gan::" in ev["name"]:
-            out.append(ev["name"].replace("void ", "").split("(", 1)[0].replace("b200gan::", ""))
-    return out
 
 
 # (id, N, C, K, H, W, up, act, slope): C = norm channels = conv input channels, K = conv output channels
@@ -208,13 +178,8 @@ def test_dgrad_norm_kernels_and_graph_replay(case):
         assert s.dgrad_norm(da, sums, stream) == 0
         assert s.from_sums(da, sums, dx, dgb, stream) == 0
 
-    names = []
-    for _ in range(3):  # a CUDA activity session now and then loses a kernel record; a wrong route repeats
-        names = traced_kernels(both)
-        if len(names) == 3:
-            break
-    if names:
-        assert names == [EXPECTED_DGRAD[c], "norm_bwd_apply_kernel<4>", "norm_bwd_params_kernel"], names
+    check_route(case[0], both, [(EXPECTED_DGRAD[c], None), ("norm_bwd_apply_kernel<4>", None),
+                                ("norm_bwd_params_kernel", None)])
     eager = (da.clone(), dx.clone(), dgb.clone())
     side = torch.cuda.Stream()
     torch.cuda.synchronize()
@@ -298,13 +263,12 @@ def test_tc_wgrad_bias_gradient_vs_fp64(case):
                                         ws.data_ptr(), ALGO_AUTO, ops._stream()) == 0
 
     names = []
-    for _ in range(3):
-        names = traced_kernels(call)
+    for _ in range(3):  # a profiler session now and then loses a kernel record; a wrong route repeats
+        names = [nm for nm, _ in traced_kernels(call)]
+        assert not any("colsum" in nm for nm in names), names
         if any(nm.startswith("wgrad_tc_kernel") for nm in names):
             break
-    if names:
-        assert not any("colsum" in nm for nm in names), names
-        assert any(nm.startswith("wgrad_tc_kernel") for nm in names), names
+    assert any(nm.startswith("wgrad_tc_kernel") for nm in names), names
     torch.cuda.synchronize()
     assert _guards_intact(bb) and not torch.isnan(db).any()
     d64 = dy.double()

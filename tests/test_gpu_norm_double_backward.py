@@ -1,8 +1,8 @@
 """Gradient penalties through training-mode BatchNorm2d / InstanceNorm2d (SURVEY.md 8f N2) on the GPU.
 
 C ABI: b200gan_norm_dbwd on every geometry of tests/norm_cases.py with none / LeakyReLU / ReLU, on guarded buffers
-(the Arena of the convolution conformance test), against the fp64 closed form of tests/test_cpu_norm_double_backward.py
-taking the mask from the kernel's own forward output (so an element next to a sign change cannot flip).  Bounds are
+(the Arena of tests/conformance.py), against the fp64 closed form of tests/norm_cases.py (held to torch float64 double
+backward by tests/test_cpu_norm_double_backward.py) taking the mask from the kernel's own forward output (so an element next to a sign change cannot flip).  Bounds are
 2^-16 relative to the magnitudes that enter each value, as in test_gpu_norm_conformance.py.  Also: every output asked for
 alone, the workspace handed back zeroed, Tanh / Sigmoid refused, a bit-identical CUDA-graph replay, and the kernel
 instances of every case, traced in one profiler session.
@@ -21,10 +21,9 @@ import torch
 
 import norm_cases as nc
 from b200gan import _lib
+from conformance import Arena, check_elementwise, check_route
 from conftest import rel_err
-from test_cpu_norm_double_backward import closed_form
-from test_gpu_conv_conformance import Arena, traced_kernels
-from test_gpu_norm_conformance import ACT_CODE, SLOPE, Run
+from norm_cases import ACT_CODE, SLOPE, Run, closed_form
 
 pytestmark = pytest.mark.gpu
 
@@ -43,7 +42,7 @@ class DRun:
     def __init__(self, case):
         self.fwd = Run(case, seed=1)
         self.fwd.prepare()
-        assert self.fwd.call() == 0
+        assert self.fwd.call(torch.cuda.current_stream().cuda_stream) == 0
         torch.cuda.synchronize()
         g, f = case.geom, self.fwd
         self.c, self.g, self.G, self.lib = case, g, f.G, f.lib
@@ -117,17 +116,6 @@ class DRun:
         return gdy, gx, gg, TOL * b_gdy, TOL * b_gx, None if gg_b is None else TOL * gg_b
 
 
-def check(what, got, ref, bound):
-    got = got.double().reshape(ref.shape)
-    assert not torch.isnan(got).any(), f"{what}: NaN (an element never written, or a guard read)"
-    err = (got - ref).abs()
-    bad = (err > bound).nonzero()
-    if bad.numel():
-        at = tuple(bad[0].tolist())
-        raise AssertionError(f"{what}: |err| {err[at].item():.3e} > bound {bound[at].item():.3e} at {at}; "
-                             f"got {got[at].item():.9g}, fp64 {ref[at].item():.9g}")
-
-
 @pytest.mark.parametrize("case", CASES, ids=lambda c: c.id)
 def test_norm_dbwd_case(case):
     run = DRun(case)
@@ -139,10 +127,10 @@ def test_norm_dbwd_case(case):
     run.arena.check_guards(case.id)
     assert (t["sums"] == 0).all(), f"{case.id}: the workspace is not handed back zeroed"
     gdy, gx, gg, b_gdy, b_gx, b_gg = run.reference()
-    check(f"{case.id} gdy", nchw(t["gdy"], g), gdy, b_gdy)
-    check(f"{case.id} gx", nchw(t["gx"], g), gx, b_gx)
+    check_elementwise(f"{case.id} gdy", nchw(t["gdy"], g), gdy, b_gdy)
+    check_elementwise(f"{case.id} gx", nchw(t["gx"], g), gx, b_gx)
     if g.affine:
-        check(f"{case.id} ggamma", t["gg"], gg, b_gg)
+        check_elementwise(f"{case.id} ggamma", t["gg"], gg, b_gg)
     full = {k: t[k].clone() for k in ("gx", "gdy", "gg") if k in t}
 
     # each output alone: bit-identical to the full call, the others never written
@@ -183,24 +171,10 @@ def test_norm_dbwd_traced_instances():
     """Every case's calls in ONE profiler session (few sessions per process keep the activity records complete): the
     kernel instances in launch order, and the (samples, channel slices) of each templated launch."""
     runs = [DRun(c) for c in CASES]
-    for r in runs:
-        r.prepare()
-    # the session's first launch can lose its kernel record (see test_gpu_norm_conformance.check_route): a marker
-    marker = torch.zeros(1, device="cuda")
-    want = [(c, n) for c in CASES for n in expected_instances(c)]
-    seen = []
-    for _ in range(3):  # a session that drops a record does not drop it again
-        for r in runs:
-            r.prepare()
-        seen = [(n, grid) for n, grid in traced_kernels(lambda: (marker.zero_(), [r.call() for r in runs]))
-                if n.startswith("norm_")]
-        if len(seen) == len(want):
-            break
-    assert [n for n, _ in seen] == [n for _, n in want], "trace and table differ"
-    for (c, n), (_, grid) in zip(want, seen):
-        if "<" in n:
-            g = c.geom
-            assert tuple(grid[1:]) == (g.N if g.per_sample else 1, g.slices), (c.id, n, grid)
+    launches = [(n, (None, c.geom.N if c.geom.per_sample else 1, c.geom.slices) if "<" in n else None)
+                for c in CASES for n in expected_instances(c)]
+    check_route("norm_dbwd", lambda: [r.call() for r in runs], launches, family=("norm_",),
+                prepare=lambda: [r.prepare() for r in runs])
 
 
 @pytest.mark.parametrize("act", ["tanh", "sigmoid"])

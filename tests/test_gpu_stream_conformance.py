@@ -1,8 +1,8 @@
 """Every case of tests/stream_cases.py (head.cu and index_ops.cu), element by element against torch float64.
 
-Each case calls the C ABI on the guarded buffers of the convolution conformance test (Arena): inputs between NaN
-guards, outputs started as NaN, sentinels around everything the library writes.  Adam's p, m and v are read and
-written in place: they get the "io" role of IoArena below (their data, and sentinel guards); its step buffer starts at
+Each case calls the C ABI on the guarded buffers of tests/conformance.py (Arena) and runs its protocol: inputs between
+NaN guards, outputs started as NaN, sentinels around everything the library writes.  Adam's p, m and v are read and
+written in place: they get the Arena's "io" role (their data, and sentinel guards); its step buffer starts at
 (step0, 0) and must come back as (step0 + 1, 0).
 
 Checks:
@@ -10,139 +10,27 @@ Checks:
     the epilogue backward for none / LeakyReLU / ReLU, restated in fp32 with the kernel's operation order;
   - everything else against fp64 with a bound from the arithmetic, 2^-23 (n + s + 4) A as in the conv suite: A the
     same sum over |terms|, n the length of the kernel's longest fp32 chain and s the partials added outside it;
-    tanh / sigmoid carried through with act_bound of the fused suite; Adam's bound counts its roundings per step;
-  - the traced kernels, launch count and grids of the table (a marker launch opens the profiler session);
-  - a CUDA-graph replay, bit for bit where the case is deterministic;
+    tanh / sigmoid carried through with chain_cases.act_bound; Adam's bound counts its roundings per step;
+  - the traced kernels, launch count and grids of the table;
+  - a CUDA-graph replay, bit for bit but for the epilogue's atomically summed db;
   - refusals: the error code, untouched outputs, intact guards.
 """
-import ctypes
 import math
 
 import pytest
 import torch
-import torch.nn.functional as F
 
 import stream_cases as sc
 from b200gan import _lib
-from test_gpu_conv_conformance import Arena, check_elementwise, tf32_rna, traced_kernels
-from test_gpu_fused_conformance import act_bound
+from chain_cases import act_bound
+from conformance import Arena, bits_equal, check_elementwise, not_vacuous, run_case, tf32_rna
+from stream_cases import (ADAM, F32, SLOPE, U, act32_exact, act64, adam_ref, bce_grad_ref, bce_ref, grad32_exact, pad_grad_ref,
+                          pad_ref, upsample_grad_ref, upsample_ref)
 
 pytestmark = pytest.mark.gpu
 
-U = 2.0 ** -23
-SLOPE = 0.2
 ACT_CODE = {"none": _lib.ACT_NONE, "lrelu": _lib.ACT_LRELU, "relu": _lib.ACT_RELU, "tanh": _lib.ACT_TANH,
             "sigmoid": _lib.ACT_SIGMOID}
-ADAM = dict(lr=2e-4, b1=0.5, b2=0.999, eps=1e-8)   # dcgan.py:134-135
-F32 = torch.float32
-
-
-# ---- fp64 references (device-agnostic: tests/test_cpu_kernel_coverage.py holds them to stock torch) -----------------
-def bce_ref(v, t):
-    """torch.nn.BCELoss(): mean of -(t log v + (1 - t) log(1 - v)), logs clamped at -100; and its terms"""
-    v, t = v.double(), t.double()
-    lp, lq = torch.log(v).clamp_min(-100), torch.log1p(-v).clamp_min(-100)
-    terms = (t - 1) * lq - t * lp
-    return terms.mean(), terms, lp, lq
-
-
-def bce_grad_ref(v, t, gout):
-    """d loss / d v = gout / n * (v - t) / max((1 - v) v, 1e-12) (the clamp of torch's binary_cross_entropy_backward)"""
-    v, t = v.double(), t.double()
-    eps = torch.tensor(1e-12, dtype=F32).item()
-    return gout / v.numel() * (v - t) / ((1 - v) * v).clamp_min(eps)
-
-
-def pad_ref(x_nhwc, pads, mode):
-    t, l, b, r = pads
-    y = F.pad(x_nhwc.permute(0, 3, 1, 2), (l, r, t, b), mode="reflect" if mode == "reflect" else "constant")
-    return y.permute(0, 2, 3, 1)
-
-
-def pad_grad_ref(dy_nhwc, xshape, pads, mode):
-    x = torch.zeros(xshape, dtype=dy_nhwc.dtype, device=dy_nhwc.device, requires_grad=True)
-    (g,) = torch.autograd.grad(pad_ref(x, pads, mode), x, dy_nhwc)
-    return g
-
-
-def upsample_ref(x_nhwc):
-    return x_nhwc.repeat_interleave(2, 1).repeat_interleave(2, 2)
-
-
-def upsample_grad_ref(dy_nhwc):
-    N, H2, W2, C = dy_nhwc.shape
-    return dy_nhwc.reshape(N, H2 // 2, 2, W2 // 2, 2, C).sum((2, 4))
-
-
-def adam_consts(step0, lr=ADAM["lr"], b1=ADAM["b1"], b2=ADAM["b2"], eps=ADAM["eps"]):
-    """the kernel's fp32 casts of the Python-double terms of _single_tensor_adam, as doubles"""
-    f = lambda v: torch.tensor(v, dtype=F32).item()
-    t = step0 + 1.0
-    return dict(nss=f(-(lr / (1.0 - b1 ** t))), bc2=f(math.sqrt(1.0 - b2 ** t)), b1=f(b1), omb1=f(1.0 - b1), b2=f(b2),
-                omb2=f(1.0 - b2), eps=f(eps))
-
-
-def adam_ref(p, g, m, v, step0, gscale=1.0):
-    """one Adam step in fp64 on the kernel's constants; returns p, m, v and their bounds (roundings per step:
-    m 2, v 3, the denominator 3 (sqrt, divide, add), the update 3 (divide, multiply, add))"""
-    k = adam_consts(step0)
-    p, g, m, v = p.double(), g.double() * gscale, m.double(), v.double()
-    m1 = k["b1"] * m + k["omb1"] * g
-    v1 = k["b2"] * v + k["omb2"] * g * g
-    sq = torch.sqrt(v1)
-    den = sq / k["bc2"] + k["eps"]
-    p1 = p + k["nss"] * (m1 / den)
-    em = 2 * U * (k["b1"] * m.abs() + k["omb1"] * g.abs())
-    ev = 3 * U * (k["b2"] * v.abs() + k["omb2"] * g * g)
-    eden = torch.where(sq > 0, ev / (2 * sq.clamp_min(1e-300)), ev.sqrt()) / k["bc2"] + 3 * U * den
-    ep = abs(k["nss"]) * (em / den + m1.abs() * eden / (den * den) + 2 * U * m1.abs() / den) + U * p1.abs()
-    return (p1, ep), (m1, em), (v1, ev)
-
-
-def act64(name, v):
-    return {"none": lambda: v, "lrelu": lambda: torch.where(v > 0, v, v * SLOPE), "relu": lambda: v.clamp_min(0),
-            "tanh": lambda: torch.tanh(v), "sigmoid": lambda: torch.sigmoid(v)}[name]()
-
-
-def act32_exact(name, x):
-    """none / LeakyReLU / ReLU in fp32, as apply_act evaluates them"""
-    return {"none": lambda: x, "lrelu": lambda: torch.where(x > 0, x, x * SLOPE),
-            "relu": lambda: x.clamp_min(0)}[name]()
-
-
-def grad32_exact(name, y):
-    """act_grad_from_out of none / LeakyReLU / ReLU in fp32"""
-    one = torch.ones_like(y)
-    return {"none": lambda: one, "lrelu": lambda: torch.where(y > 0, one, one * SLOPE),
-            "relu": lambda: (y > 0).to(y.dtype)}[name]()
-
-
-# ---- buffers -------------------------------------------------------------------------------------------------------
-class IoArena(Arena):
-    """Arena with an "io" role: a read-modify-write operand holds its data, between sentinel guards"""
-
-    def prepare(self, data):
-        super().prepare(data)
-        for name, (o, numel, dtype, role, nbytes) in self.layout.items():
-            if role == "io":
-                self.t[name].copy_(data[name].reshape(-1))
-
-
-def bits_equal(what, got, want):
-    got, want = got.reshape(-1).contiguous(), want.reshape(-1).contiguous().to(got.dtype)
-    same = got.view(torch.int32) == want.view(torch.int32)
-    if not same.all():
-        i = same.logical_not().nonzero()[0].item()
-        raise AssertionError(f"{what}: element {i}: {got[i].item()!r}, expected bit for bit {want[i].item()!r}")
-
-
-def not_vacuous(what, bound, terms):
-    """median bound below the median magnitude of one term of the sum"""
-    t = terms[terms > 0]
-    if t.numel() == 0:
-        return
-    med_b, med_t = bound.median().item(), t.median().item()
-    assert med_b < med_t, f"{what}: vacuous bound: median bound {med_b:.3e} >= median one-term contribution {med_t:.3e}"
 
 
 # ---- runs ------------------------------------------------------------------------------------------------------------
@@ -152,7 +40,7 @@ class Run:
         self.gen = torch.Generator().manual_seed(seed)
         self.off = {}                     # name -> leading floats in front of the operand (misaligned pointers)
         specs, self.data = getattr(self, "setup_" + c.op)(c.dims, c.opt)
-        self.arena = IoArena(specs)
+        self.arena = Arena(specs)
 
     # data helpers
     def randn(self, *s, scale=1.0):
@@ -181,7 +69,7 @@ class Run:
         self.arena.prepare(self.data)
 
     def outputs(self):
-        return {k: v.clone() for k, v in self.arena.t.items() if self.arena.layout[k][3] != "in"}
+        return self.arena.outputs()
 
     # ---- head.cu
     def setup_linear1(self, d, o):
@@ -495,72 +383,11 @@ class Run:
 
 
 # ---- the per-case test ---------------------------------------------------------------------------------------------
-FAMILY = {k for c in sc.CASES for k in c.kernels}
-
-
-def check_route(run):
-    """the case's kernels in launch order with their grids, from one profiler session opened by a marker launch"""
-    c = run.c
-    marker = torch.zeros(1, device="cuda")
-    seen = []
-    for _ in range(3):   # a lost record does not repeat; a route that differs from the table does
-        run.prepare()
-        seen = [(n, tuple(g)) for n, g in traced_kernels(lambda: (marker.zero_(), run.call(
-            torch.cuda.current_stream().cuda_stream))) if n in FAMILY]
-        if [n for n, _ in seen] == list(c.kernels):
-            break
-    if not seen and c.kernels:
-        return "the profiler recorded no CUDA kernel activity on this machine"
-    assert [n for n, _ in seen] == list(c.kernels), f"{c.id}: trace {seen}, table {c.launches}"
-    if torch.cuda.get_device_properties(0).multi_processor_count == sc.NUM_SMS:
-        assert seen == c.launches, f"{c.id}: trace {seen}, table {c.launches}"
-    return None
-
-
-VARIES = {"epilogue": {"db"}}
+FAMILY = tuple({k for c in sc.CASES for k in c.kernels})
+VARIES = {"epilogue": ("db",)}
 
 
 @pytest.mark.parametrize("case", sc.CASES, ids=lambda c: c.id)
 def test_stream_case(case):
-    run = Run(case)
-    lib = run.lib
-    run.prepare()
-    before = run.outputs()
-    rc = run.call(torch.cuda.current_stream().cuda_stream)
-    torch.cuda.synchronize()
-    if case.error:
-        assert rc == -2, f"{case.id}: expected B200GAN_E_BAD_ARG, rc {rc}"
-        run.arena.check_guards(case.id)
-        after = run.outputs()
-        for k, v in before.items():
-            assert torch.equal(v.view(torch.int32), after[k].view(torch.int32)), f"{case.id}: refused call wrote {k}"
-        return
-    assert rc == 0, f"{case.id}: rc {rc}: {lib.b200gan_last_error().decode()}"
-    run.arena.check_guards(case.id)
-    eager = run.outputs()
-    worst = run.check(case.id + " eager")
-
-    skip_reason = check_route(run)
-
-    side = torch.cuda.Stream()
-    run.prepare()
-    torch.cuda.synchronize()
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph, stream=side):
-        rc = run.call(side.cuda_stream)
-    assert rc == 0, f"{case.id}: rc {rc} under capture: {lib.b200gan_last_error().decode()}"
-    run.prepare()
-    torch.cuda.synchronize()
-    graph.replay()
-    torch.cuda.synchronize()
-    run.arena.check_guards(case.id + " graph")
-    replay = run.outputs()
-    for k, v in replay.items():
-        if k in VARIES.get(case.op, ()):
-            continue
-        same = v.view(torch.int32) == eager[k].view(torch.int32)
-        assert same.all(), f"{case.id}: graph replay differs from the eager call in {k}"
-    worst = max(worst, run.check(case.id + " graph"))
-    print(f"\n{case.id}: worst |err|/bound {worst:.3g}, launches {case.launches}")
-    if skip_reason:
-        pytest.skip(skip_reason)
+    run_case(Run(case), case.id, case.launches, refuse=(-2,) if case.error else (), varies=VARIES.get(case.op, ()),
+             family=FAMILY, num_sms=sc.NUM_SMS)

@@ -6,6 +6,7 @@ import pytest
 import torch
 
 from conftest import rel_err
+from tail_cases import mods
 
 pytestmark = pytest.mark.gpu
 
@@ -17,20 +18,6 @@ CASES = [  # N, C, K, H, W, mid activation, out activation
     (2, 128, 3, 17, 64, "lrelu", "tanh"),
     (1, 64, 2, 5, 128, "none", "sigmoid"),
 ]
-
-
-def _mods(ns, c, k, mid, out):
-    layers = [ns.Conv2d(8, c, 3, 1, 1), ns.BatchNorm2d(c, 0.8)]
-    if mid == "lrelu":
-        layers.append(ns.LeakyReLU(0.2, inplace=True))
-    elif mid == "relu":
-        layers.append(ns.ReLU(inplace=True))
-    layers.append(ns.Conv2d(c, k, 3, stride=1, padding=1))
-    if out == "tanh":
-        layers.append(ns.Tanh())
-    elif out == "sigmoid":
-        layers.append(ns.Sigmoid())
-    return ns.Sequential(*layers)
 
 
 @pytest.fixture(autouse=True)
@@ -45,8 +32,8 @@ def test_tail_matches_stock_torch(case):
     from b200gan import nn as bnn, zoo
     n, c, k, h, w, mid, out = case
     torch.manual_seed(3)
-    ref = _mods(zoo.namespace(stock=True), c, k, mid, out).cuda().train()
-    ours = _mods(zoo.namespace(), c, k, mid, out).cuda().train()
+    ref = mods(zoo.namespace(stock=True), c, k, mid, out).cuda().train()
+    ours = mods(zoo.namespace(), c, k, mid, out).cuda().train()
     with torch.no_grad():
         ref[1].weight.normal_(1.0, 0.2)
         ref[1].bias.normal_(0.0, 0.2)
@@ -73,8 +60,8 @@ def test_tail_falls_back_in_eval_mode_and_keeps_the_accumulators_clean():
     """ADVICE r1: conv -> BatchNorm2d(eval) must not leave partial sums in the shared statistics accumulator."""
     from b200gan import zoo
     torch.manual_seed(4)
-    ref = _mods(zoo.namespace(stock=True), 64, 1, "lrelu", "tanh").cuda()
-    ours = _mods(zoo.namespace(), 64, 1, "lrelu", "tanh").cuda()
+    ref = mods(zoo.namespace(stock=True), 64, 1, "lrelu", "tanh").cuda()
+    ours = mods(zoo.namespace(), 64, 1, "lrelu", "tanh").cuda()
     ours.load_state_dict(ref.state_dict())
     x = torch.randn(2, 8, 32, 32, device="cuda")
     ref.eval(); ours.eval()

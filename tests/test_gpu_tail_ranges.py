@@ -7,7 +7,7 @@ import pytest
 import torch
 
 from conftest import rel_err
-from test_gpu_tail import _mods
+from tail_cases import mods
 
 pytestmark = pytest.mark.gpu
 
@@ -32,8 +32,8 @@ def test_tail_ranges_match_stock_torch(case):
     from b200gan import zoo
     n, c, k, h, w, mid, out = case
     torch.manual_seed(5)
-    ref = _mods(zoo.namespace(stock=True), c, k, mid, out).cuda().train()
-    ours = _mods(zoo.namespace(), c, k, mid, out).cuda().train()
+    ref = mods(zoo.namespace(stock=True), c, k, mid, out).cuda().train()
+    ours = mods(zoo.namespace(), c, k, mid, out).cuda().train()
     with torch.no_grad():
         ref[1].weight.normal_(1.0, 0.2)
         ref[1].bias.normal_(0.0, 0.2)
