@@ -365,28 +365,58 @@ def ptxas_report(path):
 
 
 # ---- the registry ------------------------------------------------------------------------------------------------
+class Family:
+    """a registered case table: its cases, a case's kernel names, the C ABI entry points its runs call, and the modules
+    (the case table and its GPU conformance test) in which those calls are made"""
+
+    def __init__(self, cases, names, entry_points, modules):
+        self.cases, self.names, self.entry_points, self.modules = cases, names, tuple(entry_points), tuple(modules)
+
+
 def case_tables():
-    """family -> (its case table, a case's kernel names): every table whose kernels count as covered"""
+    """family -> Family: every table whose kernels and entry points count as covered"""
     import chain_cases
     import class_head_cases
     import conv_cases
     import critic_cases
     import generator_cases
     import norm_cases
+    import norm_conv_cases
     import pixel_loss_cases
     import stream_cases
     import tail_cases
     names = lambda c: c.kernels  # noqa: E731
+    b = "b200gan_"
     return {
-        "conv": (conv_cases.CASES, names),
-        "chain": (chain_cases.CASES, names),
-        "tail": (tail_cases.CASES, names),
-        "norm": (norm_cases.CASES, names),
-        "critic": (critic_cases.CASES, names),
-        "stream": (stream_cases.CASES, names),
-        "generator": (generator_cases.CASES, names),
-        "class head": (class_head_cases.CASES, names),
-        "pixel loss": (pixel_loss_cases.CASES, lambda c: [k for k, _ in c.kernels()]),
+        "conv": Family(conv_cases.CASES, names,
+                       [b + "conv2d_" + p for p in ("fprop", "dgrad", "wgrad", "wgrad_fused_bias")],
+                       ["conv_cases.py", "test_gpu_conv_conformance.py"]),
+        "chain": Family(chain_cases.CASES, names,
+                        [b + "nb_" + p for p in ("fprop", "dz", "wgrad", "dgrad", "tail_fwd", "tail_bwd")],
+                        ["chain_cases.py", "test_gpu_fused_conformance.py"]),
+        "tail": Family(tail_cases.CASES, names, [b + "tail_fprop", b + "tail_bwd"],
+                       ["tail_cases.py", "test_gpu_fused_conformance.py"]),
+        "norm": Family(norm_cases.CASES, names, [b + "norm_" + p for p in ("stats", "finalize", "apply", "bwd")],
+                       ["norm_cases.py", "test_gpu_norm_conformance.py"]),
+        "norm conv": Family(norm_conv_cases.CASES, names, norm_conv_cases.ENTRY_POINTS,
+                            ["norm_conv_cases.py", "test_gpu_norm_conv_conformance.py"]),
+        "critic": Family(critic_cases.CASES, names,
+                         [b + p for p in ("mlp_critic_fwd", "mlp_critic_bwd", "mlp_critic_dbwd", "critic_step_mlp")],
+                         ["critic_cases.py", "test_gpu_critic_conformance.py"]),
+        "stream": Family(stream_cases.CASES, names,
+                         [b + p for p in ("epilogue_bwd", "bias_grad", "nchw_to_nhwc", "nhwc_to_nchw", "upsample2x_fwd",
+                                          "upsample2x_bwd", "pad2d_fwd", "pad2d_bwd", "act_fwd", "linear1_fwd",
+                                          "linear1_bwd", "bce_fwd", "bce_bwd", "adam_multi")],
+                         ["stream_cases.py", "test_gpu_stream_conformance.py"]),
+        "generator": Family(generator_cases.CASES, names, [b + "mlp_gen_fwd", b + "mlp_gen_bwd"],
+                            ["generator_cases.py", "test_gpu_mlp_generator_conformance.py"]),
+        "class head": Family(class_head_cases.CASES, names,
+                             [b + p for p in ("class_head_fwd", "class_head_bwd", "cross_entropy_fwd",
+                                              "cross_entropy_bwd")],
+                             ["class_head_cases.py", "test_gpu_class_head_conformance.py"]),
+        "pixel loss": Family(pixel_loss_cases.CASES, lambda c: [k for k, _ in c.kernels()],
+                             [b + "pixel_loss_fwd", b + "pixel_loss_bwd"],
+                             ["pixel_loss_cases.py", "test_gpu_pixel_loss_conformance.py"]),
     }
 
 

@@ -11,9 +11,14 @@ not from a run.  Tile widths and split counts assume a 132-SM H100 SXM; tests/te
 grids only on such a device.
 
 tests/test_cpu_conv_case_table.py checks it against b200gan_conv2d_supported and against the kernels declared in the
-sources; tests/test_gpu_conv_conformance.py runs every case.
+sources; tests/test_gpu_conv_conformance.py runs every case.  The fp64 references, their bounds and the bias-gradient
+chain of the weight-gradient kernel sit at the end of this module, where the fused norm-conv suite shares them.
 """
+import math
 from dataclasses import dataclass, replace
+
+import torch
+import torch.nn.functional as F
 
 FPROP, DGRAD, WGRAD = 0, 1, 2
 PASS_NAMES = {FPROP: "fprop", DGRAD: "dgrad", WGRAD: "wgrad"}
@@ -50,6 +55,7 @@ class Case:
     deterministic: bool = True  # repeating the call gives the same bits (dy / dw / dx; never the fp64 statistics)
     s: int = 0                  # partial sums added outside one accumulation chain
     error: bool = False         # the call must be refused (B200GAN_E_BAD_ARG)
+    fused_bias: bool = False    # wgrad through b200gan_conv2d_wgrad_fused_bias (db summed inside wgrad_tc_kernel)
     why: str = ""
 
     @property
@@ -301,6 +307,42 @@ STAGED = [
 
 GEOMETRY_CASES = TC + TC_DGRAD + TC_WGRAD + SIMT + FEWK + STAGED
 
+
+# ---- the bias gradient summed inside the tensor-core weight gradient (b200gan_conv2d_wgrad_fused_bias) ---------------
+def _fused(c, why):
+    """c through the fused-bias entry point: a Conv2d on the tensor-core route launches no colsum_kernel; a
+    ConvTranspose2d and every other route still sum db with it"""
+    tc_conv2d = c.tc and not c.transposed
+    return replace(c, name=c.name + "_fb", fused_bias=True, why=why,
+                   kernels=tuple(k for k in c.kernels if not (tc_conv2d and k == "colsum_kernel")))
+
+
+def _wg(name, N, C, K, H, W, kernel, grid, s=0, **kw):
+    """a 3x3 tensor-core wgrad case; grid = (pixel splits, jobs, M-tiles x N-tiles) from wg_plan at 132 SMs"""
+    return _c(name, N, C, K, H, W, 3, 3, pads=P1, pas=WGRAD, kernels=(kernel,) + _WG_TILE, grid=grid, s=s,
+              deterministic=grid[0] == 1, **kw)
+
+
+_BY_NAME = {(c.name, c.pas): c for c in GEOMETRY_CASES}
+FUSED_BIAS = [_fused(c, f"fused db on {c.why}") for c in TC_WGRAD] + [
+    _fused(_wg("w_k256", 2, 32, 256, 8, 8, "wgrad_tc_kernel<32, 8>", (1, 9, 2)), "dy is A over two M-tiles: channels 128.. come from M-tile 1"),
+    _fused(_wg("w_k384", 2, 32, 384, 8, 8, "wgrad_tc_kernel<32, 8>", (1, 9, 3)), "dy is A over three M-tiles"),
+    _fused(_wg("w_c256_k64", 2, 256, 64, 8, 8, "wgrad_tc_kernel<64, 8>", (1, 9, 2)), "C = 256, K = 64: dy is B, x spans two M-tiles"),
+    _fused(_wg("w_dcgan_up2_k128", 128, 128, 128, 16, 16, "wgrad_tc_kernel<128, 6>", (8, 16, 1), s=32, up=2),
+           "DCGAN conv1 (dcgan.py:54-55): dy is A, four phase jobs x 8 pixel splits add to each channel"),
+    _fused(_wg("w_dcgan_up2_k64", 32, 128, 64, 32, 32, "wgrad_tc_kernel<64, 8>", (8, 16, 1), s=32, up=2),
+           "DCGAN conv2 (dcgan.py:58-59) at batch 32: dy is B (NB = 64); at batch 128 one image's share of dw lies "
+           "below the dw bound of a 512-stage split"),
+    _fused(_wg("w_k128_many_splits", 256, 64, 128, 16, 16, "wgrad_tc_kernel<64, 8>", (14, 9, 1), s=14), "dy is A, 14 pixel splits"),
+    _fused(_wg("w_k32_b_operand", 64, 128, 32, 20, 20, "wgrad_tc_kernel<32, 8>", (14, 9, 1), s=14),
+           "K = 32: dy is B (NB = 32); 20x20 maps clipped by 32x1 boxes"),
+    _fused(_wg("w_s2_k128", 64, 64, 128, 32, 32, "wgrad_tc_kernel<64, 8>", (14, 9, 1), s=14, stride=2),
+           "stride 2: x through the parity view, dy summed at the output grid"),
+] + [_fused(_BY_NAME[(n, WGRAD)], f"fused-bias entry point off the tensor-core route: {w}") for n, w in (
+    ("simt_wg_staged", "SIMT forced, the staged kernel"), ("simt_5x5", "5x5, conv_wgrad_kernel"),
+    ("fewk3", "few output channels"), ("nb4_s2", "few input channels, staged"))]
+GEOMETRY_CASES = GEOMETRY_CASES + FUSED_BIAS
+
 # ---- epilogue matrix: one case per option and one with all of them, for every fprop family ---------------------------
 # (family, base case, main kernels, tile images BNn (per-sample statistics fuse only at 1), fuses statistics at all)
 _FAMILIES = [
@@ -355,3 +397,188 @@ NARROW_BLOCK_KERNELS = ("nbk_fprop2_kernel", "nbk_dgrad2_kernel", "nbk_wgrad_ker
 
 def base_name(kernel):
     return kernel.split("<", 1)[0]
+
+
+# ---- the weight-gradient plan (a mirror of wg_plan in csrc/wgrad_tc.cu) -----------------------------------------------
+@dataclass(frozen=True)
+class WgPlan:
+    s_is_a: int      # 1: x is the A operand and dy (the dense operand D) is B
+    NB: int          # output channels of a CTA's B side
+    njobs: int       # filter taps, or 16 (phase, tap) jobs of the x2 upsample fold
+    mtiles: int
+    ntiles: int
+    Ho: int          # pixel grid of D the contraction runs over
+    Wo: int
+    bwl: int         # the 32-pixel box is 2^bwl x 2^bhl pixels of ipb images
+    bhl: int
+    ipb: int
+    tiles_w: int
+    tiles_h: int
+    tiles_total: int
+    tps: int         # tiles per pixel split
+    nsplits: int
+
+    @property
+    def grid(self):
+        return (self.nsplits, self.njobs, self.mtiles * self.ntiles)
+
+
+def _ilog2c(v):
+    return max(0, (v - 1).bit_length())
+
+
+def wg_plan(c, num_sms=NUM_SMS):
+    """the tensor-core weight gradient's plan of a geometry it accepts, as wg_plan computes it"""
+    up2 = c.up == 2
+    sch, dch = (c.K, c.C) if c.transposed else (c.C, c.K)
+    s_is_a = 0 if dch % 128 == 0 else 1
+    mch, nch = (sch, dch) if s_is_a else (dch, sch)
+    NB = 256 if nch % 256 == 0 else 128 if nch % 128 == 0 else 64 if nch % 64 == 0 else 32
+    njobs = 16 if up2 else c.R * c.S
+    Ho = c.H if up2 or c.transposed else c.P
+    Wo = c.W if up2 or c.transposed else c.Q
+    bwl = min(_ilog2c(Wo), 5)
+    bhl = min(_ilog2c(Ho), 5 - bwl)
+    tiles_w, tiles_h, ipb = -(-Wo // (1 << bwl)), -(-Ho // (1 << bhl)), 32 >> (bwl + bhl)
+    total = -(-c.N // ipb) * tiles_w * tiles_h
+    per_split = njobs * (mch // 128) * (nch // NB)
+    max_ns = min(max(total // 8, 1), 4 * num_sms)
+    ns, best = 1, -1
+    for s in range(1, max_ns + 1):
+        cost = -(-s * per_split // num_sms) * (-(-total // s) + 8)
+        if best < 0 or cost < best:
+            best, ns = cost, s
+    tps = -(-total // ns)
+    return WgPlan(s_is_a, NB, njobs, mch // 128, nch // NB, Ho, Wo, bwl, bhl, ipb, tiles_w, tiles_h, total, tps,
+                  -(-total // tps))
+
+
+# ---- fp64 references and their bounds ---------------------------------------------------------------------------------
+U = 2.0 ** -23
+EPS_UP2_FOLD = 2.0 ** -11 + 3 * 2.0 ** -24
+
+
+def geom(c):
+    from b200gan import _lib
+    t, l, b, r = c.pads
+    return _lib.ConvGeom(c.N, c.H, c.W, c.C, c.K, c.R, c.S, c.stride, t, l, b, r, c.pad_mode, c.up, int(c.transposed),
+                         c.P, c.Q)
+
+
+def wshape(c):
+    return (c.C, c.K, c.R, c.S) if c.transposed else (c.K, c.C, c.R, c.S)
+
+
+def conv_ref(c, x_nchw, w):
+    t, l, b, r = c.pads
+    if c.transposed:
+        return F.conv_transpose2d(x_nchw, w, stride=c.stride, padding=(t, l))
+    if c.up == 2:
+        x_nchw = x_nchw.repeat_interleave(2, 2).repeat_interleave(2, 3)
+    x_nchw = F.pad(x_nchw, (l, r, t, b), mode="reflect" if c.pad_mode == REFLECT else "constant")
+    return F.conv2d(x_nchw, w, stride=c.stride)
+
+
+def nchw(t_nhwc):
+    return t_nhwc.permute(0, 3, 1, 2)
+
+
+def operands(c, x, dy, w):
+    """x, dy, w in fp64 as the kernel's arithmetic sees them (wgmma truncates raw activations to TF32, the packed
+    weights are RNA-rounded); and eps_op, the operand rounding the reference does not reproduce"""
+    from conformance import tf32_rna, tf32_trunc
+    eps_op = 0.0
+    if c.tc:
+        x, dy = tf32_trunc(x), tf32_trunc(dy)
+        if c.pas != WGRAD:
+            if c.up == 2:
+                eps_op = EPS_UP2_FOLD  # the fold's fp32 sums and their RNA are not reproduced
+            else:
+                w = tf32_rna(w)
+    return x.double(), dy.double(), w.double(), eps_op
+
+
+def conv_pass_ref(c, x, dy, w):
+    """the pass's linear result in fp64 (NHWC for activations, parameter layout for dw)"""
+    if c.pas == FPROP:
+        return conv_ref(c, nchw(x), w).permute(0, 2, 3, 1)
+    if c.pas == DGRAD:
+        xv = torch.zeros(c.N, c.C, c.H, c.W, dtype=torch.float64, device="cuda", requires_grad=True)
+        y = conv_ref(c, xv, w)
+        (g,) = torch.autograd.grad(y, xv, nchw(dy))
+        return g.permute(0, 2, 3, 1)
+    wv = torch.zeros_like(w, requires_grad=True)
+    y = conv_ref(c, nchw(x), wv)
+    (g,) = torch.autograd.grad(y, wv, nchw(dy))
+    return g
+
+
+def contraction(c):
+    if c.pas == FPROP:
+        return c.R * c.S * c.C
+    if c.pas == DGRAD:
+        return c.R * c.S * c.K * c.up * c.up
+    return c.N * (c.H * c.W if c.transposed else c.P * c.Q)
+
+
+def conv_bound(c, A, eps_op, num_sms=NUM_SMS):
+    """wgmma: eps_op A + 2^-22 (ceil(n / 8) + s + 4) A;  fp32: 2^-23 (n + s + 4) A.  A tensor-core weight gradient
+    accumulates in one chain only the pixels of its split (at most 32 per tile), and the s splits are added after"""
+    n = contraction(c)
+    if c.tc and c.pas == WGRAD:
+        n = min(n, 32 * wg_plan(c, num_sms).tps)
+    if c.tc:
+        return eps_op * A + 2.0 ** -22 * (math.ceil(n / 8) + c.s + 4) * A
+    return U * (n + c.s + 4) * A
+
+
+def one_tap(c, w):
+    m = torch.zeros_like(w)
+    m[:, :, c.R // 2, c.S // 2] = 1
+    return w * m
+
+
+def fused_db_bound(c, dy, num_sms):
+    """The bound on db of b200gan_conv2d_wgrad_fused_bias on the tensor-core route, per channel, from the sums the
+    kernel actually forms.  Every fp32 addition rounds once, by at most 2^-24 of its result, and the result is
+    replaced here by its exact value (the difference is second order and covered by the last factor):
+      dy = A (K % 128 == 0): a thread sums, stage after stage of its split's 32-pixel boxes, the pairs of pixel rows
+                             8k + 2j, 8k + 2j + 1 (k < 4) that its fragment holds; two shuffles add the four threads j;
+      dy = B:                a thread adds pixel row j of every stage; five shuffles add the 32 threads;
+      then one fp32 atomic per CTA and channel onto zero, in any order: each result is at most the sum of the
+    CTAs' |partial|.  CTAs of a channel: pixel splits x the jobs that read dy (one; four phases of the upsample fold)."""
+    u = 2.0 ** -24
+    pl = wg_plan(c, num_sms)
+    ns, tps, BW, BH, ipb = pl.nsplits, pl.tps, 1 << pl.bwl, 1 << pl.bhl, pl.ipb
+    views = [dy[:, a::2, b::2] for a in (0, 1) for b in (0, 1)] if c.up == 2 else [dy]
+    chain = torch.zeros(c.K, dtype=torch.float64, device=dy.device)
+    parts = []
+    for d in views:
+        N, Ho, Wo, K = d.shape
+        nimg = -(-N // ipb) * ipb
+        t = torch.zeros(nimg, pl.tiles_h * BH, pl.tiles_w * BW, K, dtype=torch.float64, device=dy.device)
+        t[:N, :Ho, :Wo] = d.double()
+        t = t.view(nimg // ipb, ipb, pl.tiles_h, BH, pl.tiles_w, BW, K).permute(0, 2, 4, 1, 3, 5, 6)
+        t = t.reshape(pl.tiles_total, 32, K)  # box row = w + BW (h + BH image), TMA zero fill past the map and N
+        t = torch.cat([t, t.new_zeros(ns * tps - pl.tiles_total, 32, K)]).view(ns, tps, 32, K)
+        if not pl.s_is_a:
+            r = t.view(ns, tps, 4, 8, K)
+            pairs = r[:, :, :, 0::2] + r[:, :, :, 1::2]          # [split, stage, k, j, K]
+            acc = pairs.reshape(ns, tps * 4, 4, K).cumsum(1)
+            chain += pairs.abs().sum((0, 1, 2, 3)) + acc.abs().sum((0, 1, 2))
+            a = acc[:, -1]
+            s01, s23 = a[:, 0] + a[:, 1], a[:, 2] + a[:, 3]
+            p = s01 + s23
+            chain += (s01.abs() + s23.abs() + p.abs()).sum(0)
+        else:
+            acc = t.cumsum(1)                                     # [split, stage, lane, K]
+            chain += acc.abs().sum((0, 1, 2))
+            v = acc[:, -1]
+            for lvl, o in enumerate((16, 8, 4, 2, 1), 1):
+                v = v + v[:, torch.arange(32, device=dy.device) ^ o]
+                chain += v.abs().sum((0, 1)) / 2 ** lvl           # 2^lvl lanes hold each sum
+            p = v[:, 0]
+        parts.append(p)
+    P = torch.cat(parts)
+    depth = 4 * tps + 5 + P.shape[0]
+    return u * (chain + (P.shape[0] - 1) * P.abs().sum(0)) * (1 + 2 * depth * u)

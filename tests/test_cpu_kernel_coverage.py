@@ -2,9 +2,13 @@
 suites agree with stock torch float64.  Needs the built library (the case tables import it), not a GPU.
 
 A kernel is covered when a case table of the registry (conformance.case_tables) names it; the few kernels a dedicated
-test covers instead are listed in COVERED_BY_TEST with that test.  A new kernel without a case fails here.
+test covers instead are listed in COVERED_BY_TEST with that test.  A new kernel without a case fails here.  The same
+holds for the C ABI: every entry point of include/b200gan.h that launches work on a stream is named by one registered
+family and called in that family's case table or GPU conformance test, or listed in ENTRY_POINTS_COVERED_BY_TEST.  An
+entry point that is a run-time mode of an existing kernel (a fused epilogue, a from-sums pass) so needs cases of its own.
 """
 import os
+import re
 
 import pytest
 import torch
@@ -12,11 +16,21 @@ import torch.nn.functional as F
 
 import critic_cases as cr
 import stream_cases as sc
-from conformance import CSRC, case_tables, declared, declared_under_csrc, needs_nvcc, ptxas_report, table_kernels
+from conformance import CSRC, ROOT, case_tables, declared, declared_under_csrc, needs_nvcc, ptxas_report, \
+    table_kernels
 
 COVERED_BY_TEST = {
     "pack_multi_kernel": "tests/test_gpu_conv_conformance.py::test_pack_weights_multi_30_jobs (bit-exact, 30 jobs)",
 }
+
+ENTRY_POINTS_COVERED_BY_TEST = {
+    "b200gan_pack_weights": "tests/test_gpu_conv_conformance.py::test_pack_weights_bit_exact",
+    "b200gan_pack_weights_multi": "tests/test_gpu_conv_conformance.py::test_pack_weights_multi_30_jobs",
+    "b200gan_norm_dbwd": "tests/test_gpu_norm_double_backward.py::test_norm_dbwd_case",
+    "b200gan_mlp_disc_fwd": "tests/test_gpu_mlp_discriminator.py::test_disc_case",
+    "b200gan_mlp_disc_bwd": "tests/test_gpu_mlp_discriminator.py::test_disc_case",
+}
+HEADER = os.path.join(ROOT, "include", "b200gan.h")
 
 
 def test_every_kernel_has_a_case():
@@ -27,13 +41,51 @@ def test_every_kernel_has_a_case():
     for d in (e.name for e in os.scandir(CSRC) if e.is_dir()):
         assert any(f.startswith(d + os.sep) for f in kernels.values()), f"no kernel parsed under csrc/{d}"
     covered = set()
-    for cases, names in case_tables().values():
-        covered |= table_kernels(cases, names)
+    for fam in case_tables().values():
+        covered |= table_kernels(fam.cases, fam.names)
     missing = set(kernels) - covered - set(COVERED_BY_TEST)
     assert not missing, f"kernels without a conformance case: {sorted((kernels[k], k) for k in missing)}"
     stale = set(COVERED_BY_TEST) - set(kernels)
     assert not stale, f"COVERED_BY_TEST names kernels the sources do not declare: {sorted(stale)}"
     assert not set(COVERED_BY_TEST) & covered, "a kernel in COVERED_BY_TEST also has a case: drop it from the map"
+
+
+def stream_entry_points(header):
+    """the functions a C header declares with a `void *stream` parameter"""
+    src = re.sub(r"/\*.*?\*/", "", header, flags=re.S)
+    return {m.group(1) for m in re.finditer(r"\b(b200gan_\w+)\s*\(([^;{]*)\)\s*;", src)
+            if re.search(r"\bvoid\s*\*\s*stream\b", m.group(2))}
+
+
+def test_every_entry_point_has_a_case():
+    """every entry point that takes a stream is named by one registered family and called in that family's case table
+    or GPU conformance test, or listed in ENTRY_POINTS_COVERED_BY_TEST with the test that calls it"""
+    with open(HEADER) as fh:
+        entry = stream_entry_points(fh.read())
+    assert len(entry) > 40, f"parsed only {len(entry)} entry points from {HEADER}"
+    owner = {}
+    for name, fam in case_tables().items():
+        for e in fam.entry_points:
+            assert e not in owner, f"{e} is named by the families {owner[e]!r} and {name!r}"
+            owner[e] = name
+            texts = []
+            for m in fam.modules:
+                with open(os.path.join(ROOT, "tests", m)) as fh:
+                    texts.append(fh.read())
+            assert any(re.search(r"\b" + e + r"\b", t) for t in texts), \
+                f"family {name!r} names {e}, but none of {fam.modules} calls it"
+    stale = (set(owner) | set(ENTRY_POINTS_COVERED_BY_TEST)) - entry
+    assert not stale, f"entry points named in the registry or ENTRY_POINTS_COVERED_BY_TEST but not declared: {stale}"
+    both = set(owner) & set(ENTRY_POINTS_COVERED_BY_TEST)
+    assert not both, f"an entry point with a family is also in ENTRY_POINTS_COVERED_BY_TEST: drop it from the map: {both}"
+    for e, test in ENTRY_POINTS_COVERED_BY_TEST.items():
+        path, _, fn = test.partition("::")
+        with open(os.path.join(ROOT, path)) as fh:
+            text = fh.read()
+        assert re.search(r"\b" + e + r"\b", text) and re.search(r"\bdef " + fn + r"\(", text), \
+            f"{e}: {test} does not exist or does not call it"
+    missing = entry - set(owner) - set(ENTRY_POINTS_COVERED_BY_TEST)
+    assert not missing, f"entry points without a case: {sorted(missing)}"
 
 
 def test_critic_and_stream_tables_match_their_sources():

@@ -8,9 +8,10 @@ rounded to TF32 with RNA, raw activations truncated to TF32 by wgmma; SIMT kerne
 operation on absolute values, scales an error bound that follows from the arithmetic, not from a fit:
   wgmma   |y - ref| <= eps_op * A + 2^-22 * (ceil(n / 8) + s + 4) * A
   fp32    |y - ref| <= 2^-23 * (n + s + 4) * A
-with n the contraction length and s the partial sums added outside one accumulation chain; eps_op is the operand
-rounding the reference does not reproduce (the x2 upsample fold's fp32 tap sums before RNA).  The bound is carried
-through the epilogue with its Lipschitz constants.
+with n the contraction length (a tensor-core weight gradient: the pixels of one split) and s the partial sums added
+outside one accumulation chain; eps_op is the operand rounding the reference does not reproduce (the x2 upsample fold's
+fp32 tap sums before RNA).  The bound is carried through the epilogue with its Lipschitz constants.  The bias gradient that b200gan_conv2d_wgrad_fused_bias sums inside
+the tensor-core weight gradient is held to the bound of its actual summation chain (conv_cases.fused_db_bound).
 """
 import ctypes
 import math
@@ -18,31 +19,19 @@ import math
 import numpy as np
 import pytest
 import torch
-import torch.nn.functional as F
 
 import conv_cases as cc
 from b200gan import _lib
-from conformance import (STATS_FILL, Arena, check_elementwise, first_grid, not_vacuous, np_rna, run_case, tf32_rna,
-                         tf32_trunc)
+from conformance import STATS_FILL, Arena, check_elementwise, first_grid, not_vacuous, np_rna, run_case, tf32_rna, \
+    tf32_trunc
+from conv_cases import U, conv_bound, conv_pass_ref, fused_db_bound, geom, one_tap, operands, wshape
 
 pytestmark = pytest.mark.gpu
 
-U = 2.0 ** -23
-EPS_UP2_FOLD = 2.0 ** -11 + 3 * 2.0 ** -24
 SLOPE = 0.2
 
 
 # ---- the case as tensors -----------------------------------------------------------------------------------------
-def geom(c):
-    t, l, b, r = c.pads
-    return _lib.ConvGeom(c.N, c.H, c.W, c.C, c.K, c.R, c.S, c.stride, t, l, b, r, c.pad_mode, c.up, int(c.transposed),
-                         c.P, c.Q)
-
-
-def wshape(c):
-    return (c.C, c.K, c.R, c.S) if c.transposed else (c.K, c.C, c.R, c.S)
-
-
 def resolve_algo(c, lib, g):
     if c.pas == cc.WGRAD and c.algo == "AUTO":
         return _lib.ALGO_AUTO
@@ -138,8 +127,9 @@ class Run:
         if c.pas == cc.DGRAD:
             return lib.b200gan_conv2d_dgrad(ctypes.byref(self.g), a.ptr("dy"), a.ptr("w"), a.ptr("dx"), a.ptr("ws"),
                                             self.algo, stream_handle)
-        return lib.b200gan_conv2d_wgrad(ctypes.byref(self.g), a.ptr("x"), a.ptr("dy"), a.ptr("dw"), a.ptr("db"),
-                                        a.ptr("ws"), self.algo, stream_handle)
+        wgrad = lib.b200gan_conv2d_wgrad_fused_bias if c.fused_bias else lib.b200gan_conv2d_wgrad
+        return wgrad(ctypes.byref(self.g), a.ptr("x"), a.ptr("dy"), a.ptr("dw"), a.ptr("db"), a.ptr("ws"), self.algo,
+                     stream_handle)
 
     def outputs(self):
         return self.arena.outputs()
@@ -148,68 +138,7 @@ class Run:
         return check_outputs(self, self.outputs(), what)
 
 
-# ---- fp64 reference ------------------------------------------------------------------------------------------------
-def conv_ref(c, x_nchw, w):
-    t, l, b, r = c.pads
-    if c.transposed:
-        return F.conv_transpose2d(x_nchw, w, stride=c.stride, padding=(t, l))
-    if c.up == 2:
-        x_nchw = x_nchw.repeat_interleave(2, 2).repeat_interleave(2, 3)
-    x_nchw = F.pad(x_nchw, (l, r, t, b), mode="reflect" if c.pad_mode == cc.REFLECT else "constant")
-    return F.conv2d(x_nchw, w, stride=c.stride)
-
-
-def nchw(t_nhwc):
-    return t_nhwc.permute(0, 3, 1, 2)
-
-
-def operands(run):
-    """the operands in fp64, as the kernel's arithmetic sees them; and eps_op"""
-    c, inp = run.c, run.inp
-    tc = run.c.tc
-    x, dy, w = inp["x"], inp["dy"], inp["w"]
-    eps_op = 0.0
-    if tc:
-        x, dy = tf32_trunc(x), tf32_trunc(dy)
-        if c.pas != cc.WGRAD:
-            if c.up == 2:
-                eps_op = EPS_UP2_FOLD  # the fold's fp32 sums and their RNA are not reproduced
-            else:
-                w = tf32_rna(w)
-    return x.double(), dy.double(), w.double(), eps_op
-
-
-def conv_pass_ref(c, x, dy, w):
-    """the pass's linear result in fp64 (NHWC for activations, parameter layout for dw)"""
-    if c.pas == cc.FPROP:
-        return conv_ref(c, nchw(x), w).permute(0, 2, 3, 1)
-    if c.pas == cc.DGRAD:
-        xv = torch.zeros(c.N, c.C, c.H, c.W, dtype=torch.float64, device="cuda", requires_grad=True)
-        y = conv_ref(c, xv, w)
-        (g,) = torch.autograd.grad(y, xv, nchw(dy))
-        return g.permute(0, 2, 3, 1)
-    wv = torch.zeros_like(w, requires_grad=True)
-    y = conv_ref(c, nchw(x), wv)
-    (g,) = torch.autograd.grad(y, wv, nchw(dy))
-    return g
-
-
-def contraction(c):
-    if c.pas == cc.FPROP:
-        return c.R * c.S * c.C
-    if c.pas == cc.DGRAD:
-        return c.R * c.S * c.K * c.up * c.up
-    return c.N * (c.H * c.W if c.transposed else c.P * c.Q)
-
-
-def conv_bound(run, A, eps_op):
-    c = run.c
-    n = contraction(c)
-    if c.tc:
-        return eps_op * A + 2.0 ** -22 * (math.ceil(n / 8) + c.s + 4) * A
-    return U * (n + c.s + 4) * A
-
-
+# ---- fp64 reference: conv_cases holds the linear part and its bound; the epilogue is here ------------------------
 def apply_act(name, v):
     if name == "lrelu":
         return torch.where(v > 0, v, v * SLOPE)
@@ -254,10 +183,10 @@ def epilogue_ref(run, conv, bound):
 def check_outputs(run, outs, what):
     """every output of the call against the fp64 reference; returns the worst |err|/bound"""
     c = run.c
-    x, dy, w, eps_op = operands(run)
+    x, dy, w, eps_op = operands(c, run.inp["x"], run.inp["dy"], run.inp["w"])
     ref = conv_pass_ref(c, x, dy, w)
     A = conv_pass_ref(c, x.abs(), dy.abs(), w.abs())
-    bound = conv_bound(run, A, eps_op)
+    bound = conv_bound(c, A, eps_op, torch.cuda.get_device_properties(0).multi_processor_count)
     worst = 0.0
     if c.pas == cc.FPROP:
         y_ref, b = epilogue_ref(run, ref, bound)
@@ -275,17 +204,15 @@ def check_outputs(run, outs, what):
         worst = check_elementwise(what, outs["dw"], ref, bound, "(param index)")
         db_ref = run.inp["dy"].double().sum((0, 1, 2))
         db_A = run.inp["dy"].double().abs().sum((0, 1, 2))
-        n = c.N * c.P * c.Q
-        check_elementwise(what + " db", outs["db"], db_ref, U * (n + 1100) * db_A, "(k,)")
+        if c.fused_bias and c.tc and not c.transposed:
+            db_bound = fused_db_bound(c, run.inp["dy"], torch.cuda.get_device_properties(0).multi_processor_count)
+            not_vacuous(what + " db", db_bound, run.inp["dy"].double().abs().reshape(-1))
+        else:
+            db_bound = U * (c.N * c.P * c.Q + 1100) * db_A
+        worst = max(worst, check_elementwise(what + " db", outs["db"], db_ref, db_bound, "(k,)"))
         if c.N > 1:
             not_vacuous(what, bound, conv_pass_ref(replace_n(c), x[:1], dy[:1], w).abs())
     return worst
-
-
-def one_tap(c, w):
-    m = torch.zeros_like(w)
-    m[:, :, c.R // 2, c.S // 2] = 1
-    return w * m
 
 
 def replace_n(c):
