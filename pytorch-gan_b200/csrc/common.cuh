@@ -71,6 +71,17 @@ __device__ __forceinline__ float round_tf32(float v) {
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(v));
   return __uint_as_float(r);
 }
+// BatchNorm / InstanceNorm statistics: norm_stats_kernel and the conv_tc.cu epilogues sum x and x^2 from zero in fp32
+// (the plain sums), and x - p and (x - p)^2 around a pivot p from the data.  The plain sums round relative to
+// mean^2 + var: where a block's |mean| <= 4 std they are about as accurate as the pivoted ones and are the ones added,
+// so that data near zero gets the same bits as from plain sums alone; beyond, the pivoted sums are.  (The chain's
+// epilogue in narrow_block.cu always adds its pivoted sums.)  s1, s2: the block's [sum x, sum x^2] formed from its
+// pivoted sums in fp64; n its count.
+__device__ __forceinline__ bool stats_plain_ok(double s1, double s2, double n) {
+  if (n <= 0.0) return true;
+  const double m = s1 / n, var = s2 / n - m * m;
+  return m * m <= 16.0 * var;
+}
 // reflection of index i into [0, n) (torch ReflectionPad2d: edge pixel not repeated)
 __device__ __forceinline__ int reflect_idx(int i, int n) {
   if (i < 0) i = -i;

@@ -173,6 +173,71 @@ __device__ __forceinline__ void st_row32(uint8_t *chunk, int m, const float (&v)
     *reinterpret_cast<float4 *>(row + ((j ^ (m & 7)) << 4)) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
 }
 
+// BatchNorm / InstanceNorm statistics of 32 channels of one pixel per lane, over the warp's 32 pixels: the plain fp32
+// column sums of x and x^2 (added to plain[]), and the warp's [sum x, sum x^2] in fp64 (added to s[]).  Where every
+// channel of the warp has its mean within 4 standard deviations of zero (stats_plain_ok), s[] takes the plain sums;
+// otherwise (far: sticky over calls) it takes fp32 column sums of x - pivot and (x - pivot)^2, which round relative to
+// the spread rather than to the mean, brought back in fp64.  The plain sums tell the cases apart: where they are
+// inaccurate, |mean| / std exceeds 1 / sqrt(K u), far above 4.  v is the lane's row m of `chunk` as staged; the
+// pivots are the warp's first pixel of the tile, row 32 q of `piv_chunk` (rows that are multiples of 8 are not
+// swizzled), written by lane 0 of the warp.  When that pixel is outside the output, so is every pixel of the warp.
+__device__ __forceinline__ void stats_sums32(float (&v)[32], bool valid, const uint8_t *chunk, int m,
+                                             const uint8_t *piv_chunk, int q, int lane, float (&plain)[2],
+                                             double (&s)[2], bool &far) {
+  float s2[32];
+#pragma unroll
+  for (int j = 0; j < 32; ++j) {
+    v[j] = valid ? v[j] : 0.f;
+    s2[j] = v[j] * v[j];
+  }
+  const float a = warp_colsum32(v, lane), b = warp_colsum32(s2, lane);
+  plain[0] += a;
+  plain[1] += b;
+  const int n = __popc(__ballot_sync(0xffffffffu, valid));
+  far = __any_sync(0xffffffffu, far || !stats_plain_ok(a, b, n));
+  if (!far) {
+    s[0] += a;
+    s[1] += b;
+    return;
+  }
+  __syncwarp();
+  ld_row32(chunk, m, v);
+  ld_row32(piv_chunk, 32 * q, s2);
+  const float piv = reinterpret_cast<const float *>(piv_chunk + 32 * q * 128)[lane];
+#pragma unroll
+  for (int j = 0; j < 32; ++j) {
+    v[j] = valid ? v[j] - s2[j] : 0.f;
+    s2[j] = v[j] * v[j];
+  }
+  const double d = warp_colsum32(v, lane), e = warp_colsum32(s2, lane), pd = piv;
+  s[0] += fma((double)n, pd, d);
+  s[1] += fma((double)n * pd, pd, fma(2.0 * pd, d, e));
+}
+// the warp's four doubles of one channel: [sum x, sum x^2] in fp64, the plain fp32 sums as a float pair in the bytes of
+// dst[2], and whether the warp took the pivoted sums
+__device__ __forceinline__ void stats_store(double *dst, const float (&plain)[2], const double (&s)[2], bool far) {
+  dst[0] = s[0];
+  dst[1] = s[1];
+  reinterpret_cast<float2 *>(dst)[2] = make_float2(plain[0], plain[1]);
+  dst[3] = far ? 1.0 : 0.0;
+}
+// [sum x, sum x^2] of one channel of the tile from its four warps' doubles at r, r + step, ...: the plain sums added in
+// fp32 warp by warp when no warp took the pivoted sums, else the fp64 ones
+__device__ __forceinline__ void stats_tile(const double *r, int step, double &s1, double &s2) {
+  double d = 0.0, e = 0.0, far = 0.0;
+  float a = 0.f, b = 0.f;
+#pragma unroll
+  for (int qq = 0; qq < 4; ++qq, r += step) {
+    const float2 ab = reinterpret_cast<const float2 *>(r)[2];
+    a += ab.x;
+    b += ab.y;
+    d += r[0];
+    e += r[1];
+    far += r[3];
+  }
+  s1 = far == 0.0 ? (double)a : d;
+  s2 = far == 0.0 ? (double)b : e;
+}
 // bias, activation, Dropout2d scale and TF32 rounding of 32 output channels of one pixel.  Every option is tested ONCE
 // per chunk, never per element: a switch inside the unrolled element loop becomes 32 indirect branches.
 __device__ __forceinline__ void epilogue_chunk(float (&v)[32], const float *bias, int narrow_k, int act, float slope,
@@ -261,7 +326,7 @@ struct TcSmem {
   static constexpr int RING = STAGES * STAGE_BYTES;
   static constexpr int STAGING = (BN / 32) * TC_A_BYTES;
   static constexpr int MAIN = RING > STAGING ? RING : STAGING;
-  static constexpr int TOTAL = MAIN + 1024 + 256 + 4 * BN * 2 * 4;  // + alignment slack, barriers, statistics
+  static constexpr int TOTAL = MAIN + 1024 + 256 + 4 * BN * 4 * 8;  // + alignment slack, barriers, statistics
 };
 
 template <int BN, int STAGES>
@@ -273,7 +338,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t *full = reinterpret_cast<uint64_t *>(smem + L::MAIN);
   uint64_t *empty = full + STAGES;
-  float *red = reinterpret_cast<float *>(smem + L::MAIN + 256);  // [4][BN][2]
+  double *red = reinterpret_cast<double *>(smem + L::MAIN + 256);  // [4][BN][4]: each warp's sums (stats_store)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int ph = blockIdx.z / p.ksplit, ks = blockIdx.z % p.ksplit;
@@ -391,23 +456,23 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         st_row32(chunk, m, v);
       }
       if (p.stats) {
-        float s2[32];
+        double *dst = red + (q * BN + c + lane) * 4;
         // not in the 256-wide instance, where it would spill (the host never asks for it there)
-        if (BN < 256 && p.nb_x) {
+        if (BN < 256 && p.nb_x) {   // the norm-backward sums: plain fp32 column sums only, a count of 0
+          float s2[32];
           const int ch = ntile * BN + c;
           norm_bwd_terms(v, s2, valid ? p.nb_x + ((int64_t)(on * p.Ho + oh) * p.Wo + ow) * p.ldk + ch : nullptr,
                          p.nb_mean_rstd + ch, p.nb_scale_shift + ch, p.ldk, p.nb_act, p.nb_slope);
+          const float cs1 = warp_colsum32(v, lane);
+          const float plain[2] = {cs1, warp_colsum32(s2, lane)};
+          stats_store(dst, plain, {0.0, 0.0}, false);
         } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            v[j] = valid ? v[j] : 0.f;
-            s2[j] = v[j] * v[j];
-          }
+          float plain[2] = {0.f, 0.f};
+          double sum[2] = {0.0, 0.0};
+          bool far = false;
+          stats_sums32(v, valid, chunk, m, chunk, q, lane, plain, sum, far);
+          stats_store(dst, plain, sum, far);
         }
-        float cs1 = warp_colsum32(v, lane);
-        float cs2 = warp_colsum32(s2, lane);
-        red[(q * BN + c + lane) * 2 + 0] = cs1;
-        red[(q * BN + c + lane) * 2 + 1] = cs2;
       }
     }
     fence_proxy_async();  // generic-proxy smem writes -> visible to the async (TMA) proxy
@@ -426,15 +491,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     }
     if (p.stats) {
       for (int e = ct; e < BN; e += 256) {
-        float a = 0.f, b = 0.f;
-#pragma unroll
-        for (int qq = 0; qq < 4; ++qq) {
-          a += red[(qq * BN + e) * 2 + 0];
-          b += red[(qq * BN + e) * 2 + 1];
-        }
+        double a, b;
+        stats_tile(red + e * 4, BN * 4, a, b);
         const int gidx = (p.stats_per_sample ? n0 * p.ldk : 0) + ntile * BN + e;
-        atomicAdd(p.stats + gidx, (double)a);
-        atomicAdd(p.stats + p.stats_groups + gidx, (double)b);
+        atomicAdd(p.stats + gidx, a);
+        atomicAdd(p.stats + p.stats_groups + gidx, b);
       }
     }
   }
@@ -568,7 +629,7 @@ conv_tc_up2_allphase_kernel(const __grid_constant__ CUtensorMap tmA, const __gri
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t *full = reinterpret_cast<uint64_t *>(smem + MP_MAIN);
   uint64_t *empty = full + MP_STAGES;
-  float *red = reinterpret_cast<float *>(smem + MP_MAIN + 256);  // [4][BN][2]
+  double *red = reinterpret_cast<double *>(smem + MP_MAIN + 256);  // [4][BN][4]: each warp's sums (stats_store)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int ntile = blockIdx.y;
@@ -656,7 +717,11 @@ conv_tc_up2_allphase_kernel(const __grid_constant__ CUtensorMap tmA, const __gri
     const bool valid = (ow < p.Wo) && (oh < p.Ho) && (on < p.N);
     const float *cs = p.chan_scale && valid ? p.chan_scale + (int64_t)on * p.ldk + ntile * BN + c : nullptr;
     const float *bias = p.bias ? p.bias + ntile * BN + c : nullptr;
-    float st1 = 0.f, st2 = 0.f;
+    // statistics (stats_sums32) over the four phases, around the pivots of phase 0 where needed, from its staged chunk
+    float plain[2] = {0.f, 0.f};
+    double sum[2] = {0.0, 0.0};
+    bool far = false;
+    const uint8_t *piv_chunk = smem + half * TC_A_BYTES;
     if (ct == 0) TC_TRACE(40);
 #pragma unroll 1
     for (int j = 0; j < 4; ++j) {
@@ -666,16 +731,7 @@ conv_tc_up2_allphase_kernel(const __grid_constant__ CUtensorMap tmA, const __gri
       ld_row32(chunk, m, v);
       epilogue_chunk(v, bias, 0, p.act, p.slope, cs, p.rtf);
       st_row32(chunk, m, v);
-      if (p.stats) {
-        float s2[32];
-#pragma unroll
-        for (int e = 0; e < 32; ++e) {
-          v[e] = valid ? v[e] : 0.f;
-          s2[e] = v[e] * v[e];
-        }
-        st1 += warp_colsum32(v, lane);
-        st2 += warp_colsum32(s2, lane);
-      }
+      if (p.stats) stats_sums32(v, valid, chunk, m, piv_chunk, q, lane, plain, sum, far);
       fence_proxy_async();
       consumers_sync();
       if (ct == 0) {
@@ -691,19 +747,14 @@ conv_tc_up2_allphase_kernel(const __grid_constant__ CUtensorMap tmA, const __gri
       TC_TRACE(41);
     }
     if (p.stats) {
-      red[(q * BN + c + lane) * 2 + 0] = st1;
-      red[(q * BN + c + lane) * 2 + 1] = st2;
+      stats_store(red + (q * BN + c + lane) * 4, plain, sum, far);
       consumers_sync();
       if (ct < BN) {
-        float a = 0.f, b = 0.f;
-#pragma unroll
-        for (int qq = 0; qq < 4; ++qq) {
-          a += red[(qq * BN + ct) * 2 + 0];
-          b += red[(qq * BN + ct) * 2 + 1];
-        }
+        double a, b;
+        stats_tile(red + ct * 4, BN * 4, a, b);
         const int gidx = (p.stats_per_sample ? n0 * p.ldk : 0) + ntile * BN + ct;
-        atomicAdd(p.stats + gidx, (double)a);
-        atomicAdd(p.stats + p.stats_groups + gidx, (double)b);
+        atomicAdd(p.stats + gidx, a);
+        atomicAdd(p.stats + p.stats_groups + gidx, b);
       }
     }
   }
@@ -1008,7 +1059,7 @@ static int run_up2_allphase(const float *x, int N, int H, int W, int C, const fl
     uint32_t bbox[2] = {TC_BK, (uint32_t)MP_BN};
     if (int e = make_tmap_f32(&tmB, packed, 2, dims, strides, bbox)) return e;
   }
-  constexpr int SMEM = MP_MAIN + 1024 + 256 + 4 * MP_BN * 2 * 4;
+  constexpr int SMEM = MP_MAIN + 1024 + 256 + 4 * MP_BN * 4 * 8;
   static std::atomic<uint64_t> attr_done{0};
   if (int e = ensure_dynamic_smem(conv_tc_up2_allphase_kernel, SMEM, attr_done)) return e;
   dim3 grid((unsigned)(p.tiles_w * p.tiles_h * ceil_div(N, BNn)), (unsigned)(K / MP_BN), 1);

@@ -164,9 +164,11 @@ struct NbFprop2 {
 // shared memory.  Thread = PT pixels x KT output channels in registers: lanes of a warp are consecutive pixels (pixel i
 // of a thread is lp + i * TPX), the weights are read as broadcasts -- one LDS.128 of weights feeds 4 * PT FMAs, one of
 // activations 4 * KT (the first version had PT = 1: 3.8 FMAs per shared-memory load, and stalled on them).
-// dynamic smem: w [R*S*C][KB] | patch [TN][PR][PC][CP] | sc, sh [C] | red [8][2*KT]
+// dynamic smem: w [R*S*C][KB] | patch [TN][PR][PC][CP] | sc, sh [C] | red [8][2*KT] (fp64)
+// <4, 4> (DCGAN layers 2 and 3) is held to three blocks per SM, which its shared memory allows at most: at the 64
+// registers ptxas picks for it otherwise, the statistics' pivot spills.  0: no minimum (the other instances).
 template <int KT, int PT>
-__global__ void __launch_bounds__(256)
+__global__ void __launch_bounds__(256, KT == 4 && PT == 4 ? 3 : 0)
 nbk_fprop2_kernel(const __grid_constant__ NbFprop2 p) {
   extern __shared__ __align__(16) float nsm[];
   const NbTile &t = p.t;
@@ -175,7 +177,7 @@ nbk_fprop2_kernel(const __grid_constant__ NbFprop2 p) {
   float *x_s = w_s + (size_t)taps * p.C * t.KB;
   float *sc_s = x_s + (((size_t)t.TN * p.PR * p.PC * p.CP + 3) & ~(size_t)3);
   float *sh_s = sc_s + ((p.C + 3) & ~3);
-  float *red = sh_s + ((p.C + 3) & ~3);
+  double *red = reinterpret_cast<double *>(sh_s + ((p.C + 3) & ~3));
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const bool has_in = p.in_bn.stats != nullptr;
   // the tile's images belong to ONE statistics group (the planner keeps TN a divisor of the group size)
@@ -287,12 +289,25 @@ nbk_fprop2_kernel(const __grid_constant__ NbFprop2 p) {
     }
   }
   const int k0 = kbase + kgi * KT;
+  // The statistics are summed around a pivot per channel (see norm.cu), so that the fp32 sums of v - pivot and
+  // (v - pivot)^2 round relative to the spread of the channel rather than to its mean: the pivot is pixel 0's value of
+  // the warp's first lane whose pixel 0 is inside the output.  A lane whose pixel 0 is outside has every pixel outside
+  // (pixel i is TPX pixels on, a multiple of the tile's columns: the same column, a later row or image); a warp without
+  // such a lane adds nothing.
   float s1[KT], s2[KT];
+  float *piv = reinterpret_cast<float *>(red + warp * 2 * KT);  // the warp's pivots until its sums take the slot
+  int cnt = 0;   // this thread's pixels inside the output
 #pragma unroll
   for (int j = 0; j < KT; ++j) s1[j] = s2[j] = 0.f;
 #pragma unroll
   for (int i = 0; i < PT; ++i) {
     const bool valid = yoff[i] >= 0;
+    cnt += valid;
+    int src = 0;
+    if (i == 0) {
+      const unsigned holders = __ballot_sync(0xffffffffu, valid);
+      src = holders ? __ffs(holders) - 1 : 0;
+    }
 #pragma unroll
     for (int j = 0; j < KT; ++j) {
       float v = acc[i][j];
@@ -302,9 +317,18 @@ nbk_fprop2_kernel(const __grid_constant__ NbFprop2 p) {
       if (p.rtf) v = round_tf32(v);
       v = valid ? v : 0.f;
       acc[i][j] = v;
-      s1[j] += v;
-      s2[j] = fmaf(v, v, s2[j]);
+      float pj;
+      if (i == 0) {
+        pj = __shfl_sync(0xffffffffu, v, src);
+        if (lane == 0) piv[j] = pj;
+      } else {
+        pj = piv[j];
+      }
+      const float d = valid ? v - pj : 0.f;
+      s1[j] += d;
+      s2[j] = fmaf(d, d, s2[j]);
     }
+    if (i == 0) __syncwarp();
     if (valid) {
       float *yo = p.y + yoff[i] + k0;
 #pragma unroll
@@ -314,20 +338,27 @@ nbk_fprop2_kernel(const __grid_constant__ NbFprop2 p) {
     }
   }
   if (p.out_stats) {
+    // each warp hands [sum v, sum v^2] of its pixels over in fp64, in the slot that held its pivots
+    float pw[KT];
+#pragma unroll
+    for (int j = 0; j < KT; ++j) pw[j] = piv[j];
+    const int n = __reduce_add_sync(0xffffffffu, cnt);   // the warp's pixels inside the output
+    __syncwarp();
 #pragma unroll
     for (int j = 0; j < KT; ++j) {
       const float a1 = warp_sum(s1[j]), a2 = warp_sum(s2[j]);
       if (lane == 0) {
-        red[warp * 2 * KT + j] = a1;
-        red[warp * 2 * KT + KT + j] = a2;
+        const double pd = pw[j], ad = a1;
+        red[warp * 2 * KT + j] = fma((double)n, pd, ad);
+        red[warp * 2 * KT + KT + j] = fma((double)n * pd, pd, fma(2.0 * pd, ad, (double)a2));
       }
     }
     __syncthreads();
     if (tid < t.KG * 2 * KT) {   // the TPX / 32 warps of a channel group are consecutive
       const int g = tid / (2 * KT), idx = tid % (2 * KT), wpg = TPX >> 5;
-      float tsum = 0.f;
+      double tsum = 0.0;
       for (int wi = 0; wi < wpg; ++wi) tsum += red[(g * wpg + wi) * 2 * KT + idx];
-      atomicAdd(p.out_stats + (size_t)grp * 2 * p.K + (idx < KT ? 0 : p.K) + kbase + g * KT + (idx % KT), (double)tsum);
+      atomicAdd(p.out_stats + (size_t)grp * 2 * p.K + (idx < KT ? 0 : p.K) + kbase + g * KT + (idx % KT), tsum);
     }
   }
 }
@@ -929,7 +960,7 @@ static NbPlan nb_plan(int nout, int64_t wrow, int cin, int N, int Ho, int Wo, in
         t.tiles_r = ceil_div(Ho, t.TR);
         t.tiles_q = ceil_div(Wo, t.TQ);
         const size_t floats = (size_t)((wrow * KB + 3) & ~(int64_t)3) + ((patch(t.TN, t.TR, t.TQ) + 3) & ~(size_t)3) +
-                              2 * (size_t)((cin + 3) & ~3) + 8 * 2 * 16;
+                              2 * (size_t)((cin + 3) & ~3) + 8 * 2 * 16 * (nclasses_is_dgrad ? 1 : 2);  // red: fp64 in fprop
         const size_t smem = floats * sizeof(float);
         if (smem > NB_SMEM_MAX) continue;
         const int64_t blocks = (int64_t)ceil_div(N, t.TN) * t.tiles_r * t.tiles_q * (nout / KB) * nclasses;

@@ -5,8 +5,16 @@
 // cyclegan/models.py:29,33,51,61,76,108 (affine=False, no running stats, eps 1e-5).
 // Statistics are kept per "group": g = c (BatchNorm) or n*C + c (InstanceNorm).  Normalisation
 // uses the biased variance; running_var is updated with the unbiased one (torch semantics).
-// All kernels are HBM-bound streaming passes with fp64 accumulation only at the final atomic, so
-// that E[x^2]-E[x]^2 does not cancel catastrophically.  Each pass has one kernel for every C: the
+// All kernels are HBM-bound streaming passes with fp64 accumulation only at the final atomic.  The
+// statistics are [sum x, sum x^2] per group, and the variance E[x^2]-E[x]^2 is formed from them in
+// fp64.  fp32 partial sums taken from zero round relative to mean^2 + var, and the subtraction loses
+// the variance in proportion to (mean / std)^2: a channel far from zero, or constant, would get an
+// rstd wrong by O(1).  So every producer of those sums (norm_stats_kernel here, the conv_tc.cu and
+// narrow_block.cu epilogues) sums x - p and (x - p)^2 around a pivot p taken from the group's own
+// data and adds n p + sum(x - p) and sum(x - p)^2 + 2 p sum(x - p) + n p^2 in fp64; norm_stats and
+// the conv epilogues add their plain sums instead where a block's mean is near zero
+// (stats_plain_ok, common.cuh).
+// Each pass has one kernel for every C: the
 // apply and backward kernels are templated on the vector width (float4 along C, or scalar when C
 // is not a multiple of 4 or an operand is not 16-byte aligned), and the backward always recomputes
 // a LeakyReLU / ReLU mask from x when scale_shift is given.
@@ -21,34 +29,47 @@ namespace b200gan {
 __global__ void __launch_bounds__(256)
 norm_stats_kernel(const float *__restrict__ x, double *__restrict__ stats, int C, int64_t rows,
                   int64_t rows_per_block, int G, int per_sample) {
-  __shared__ float s1[8][33], s2[8][33];
+  __shared__ float s1[8][33], s2[8][33], s3[8][33], s4[8][33];
   const int c = blockIdx.x * 32 + threadIdx.x;
   const int64_t base_row = per_sample ? (int64_t)blockIdx.z * rows : 0;
   int64_t r0 = (int64_t)blockIdx.y * rows_per_block;
   int64_t r1 = r0 + rows_per_block;
   if (r1 > rows) r1 = rows;
-  float a = 0.f, b = 0.f;
+  // plain sums a = sum x, b = sum x^2, and around the column's first row of the block, p: d = sum (x - p),
+  // e = sum (x - p)^2, whose rounding is relative to the spread of the group rather than to its mean (stats_plain_ok)
+  float a = 0.f, b = 0.f, d = 0.f, e = 0.f, p = 0.f;
   if (c < C) {
     const float *xp = x + (base_row + r0) * C + c;
+    p = __ldg(xp);
     for (int64_t r = r0 + threadIdx.y; r < r1; r += 8) {
-      float v = __ldg(xp + (r - r0) * C);
+      const float v = __ldg(xp + (r - r0) * C), w = v - p;
       a += v;
       b = fmaf(v, v, b);
+      d += w;
+      e = fmaf(w, w, e);
     }
   }
   s1[threadIdx.y][threadIdx.x] = a;
   s2[threadIdx.y][threadIdx.x] = b;
+  s3[threadIdx.y][threadIdx.x] = d;
+  s4[threadIdx.y][threadIdx.x] = e;
   __syncthreads();
   if (threadIdx.y == 0 && c < C) {
-    double ta = 0.0, tb = 0.0;
+    double ta = 0.0, tb = 0.0, td = 0.0, te = 0.0;
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       ta += (double)s1[i][threadIdx.x];
       tb += (double)s2[i][threadIdx.x];
+      td += (double)s3[i][threadIdx.x];
+      te += (double)s4[i][threadIdx.x];
     }
+    // the pivoted sums back to [sum x, sum x^2] in fp64: n p + d and e + 2 p d + n p^2 over the block's n rows
+    const double n = (double)(r1 - r0), pd = (double)p;
+    const double pa = fma(n, pd, td), pb = fma(n * pd, pd, fma(2.0 * pd, td, te));
+    const bool plain = stats_plain_ok(pa, pb, n);
     int g = per_sample ? blockIdx.z * C + c : c;
-    atomicAdd(stats + g, ta);
-    atomicAdd(stats + G + g, tb);
+    atomicAdd(stats + g, plain ? ta : pa);
+    atomicAdd(stats + G + g, plain ? tb : pb);
   }
 }
 

@@ -383,6 +383,7 @@ def case_tables():
     import norm_cases
     import norm_conv_cases
     import pixel_loss_cases
+    import stats_cases
     import stream_cases
     import tail_cases
     names = lambda c: c.kernels  # noqa: E731
@@ -417,6 +418,8 @@ def case_tables():
         "pixel loss": Family(pixel_loss_cases.CASES, lambda c: [k for k, _ in c.kernels()],
                              [b + "pixel_loss_fwd", b + "pixel_loss_bwd"],
                              ["pixel_loss_cases.py", "test_gpu_pixel_loss_conformance.py"]),
+        # the statistics every normalisation producer hands on: its entry points belong to norm, conv and chain
+        "statistics": Family(stats_cases.CASES, names, [], ["stats_cases.py", "test_gpu_norm_statistics.py"]),
     }
 
 

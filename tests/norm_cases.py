@@ -14,7 +14,7 @@ from dataclasses import dataclass
 import torch
 
 from b200gan import _lib
-from conformance import Arena
+from conformance import Arena, check_elementwise
 
 ACTS = ("none", "lrelu", "relu", "tanh", "sigmoid")
 KERNELS = {"norm_stats_kernel", "norm_finalize_kernel", "norm_apply_kernel", "norm_bwd_reduce_kernel",
@@ -180,3 +180,78 @@ def closed_form(x, dy, gamma, beta, u, ugamma, ubeta, eps, act, per_sample, ap=N
     if gamma is not None:
         ggamma = (r * (Q - A * U - B * T)).sum(0).view(c)
     return gdy, gx, ggamma
+
+
+# ---- element-wise checks of a run (tests/test_gpu_norm_conformance.py, tests/test_gpu_norm_statistics.py) ----------
+TOL = 2.0 ** -16
+U = 2.0 ** -23
+LIPSCHITZ = {"none": 1.0, "lrelu": 1.0, "relu": 1.0, "tanh": 1.0, "sigmoid": 0.25}
+
+
+def act_fwd(name, v):
+    return {"none": lambda: v, "lrelu": lambda: torch.where(v > 0, v, v * SLOPE), "relu": lambda: v.clamp_min(0),
+            "tanh": lambda: torch.tanh(v), "sigmoid": lambda: torch.sigmoid(v)}[name]()
+
+
+def act_grad(name, y):
+    """the derivative the library applies, from the kernel's output y"""
+    return {"none": lambda: torch.ones_like(y), "lrelu": lambda: torch.where(y > 0, 1.0, SLOPE),
+            "relu": lambda: (y > 0).double(), "tanh": lambda: 1 - y * y, "sigmoid": lambda: y * (1 - y)}[name]()
+
+
+def check_outputs(run, what):
+    """every output of a Run against fp64 (from run.x and run.dy); the worst |err|/bound.  Bounds are 2^-16 relative to
+    the magnitudes that enter each value; the statistics themselves are held to their summation chains by
+    tests/test_gpu_norm_statistics.py"""
+    c, g, t = run.c, run.c.geom, run.arena.t
+    x, dy = run.x.double(), run.dy.double()
+    dims = (1,) if g.per_sample else (0, 1)
+    count = g.H * g.W * (1 if g.per_sample else g.N)
+    mean = x.mean(dims, keepdim=True)
+    var = ((x - mean) ** 2).mean(dims, keepdim=True)
+    rstd = 1 / torch.sqrt(var + run.eps)
+    ga = run.gamma.double() if g.affine else torch.ones(g.C, dtype=torch.float64, device="cuda")
+    be = run.beta.double() if g.affine else torch.zeros(g.C, dtype=torch.float64, device="cuda")
+
+    # forward
+    xhat = (x - mean) * rstd
+    pre = xhat * ga + be
+    y_ref = act_fwd(c.act, pre)
+    b = LIPSCHITZ[c.act] * TOL * ((x.abs() + mean.abs()) * rstd * ga.abs() + be.abs()) + 4 * U * y_ref.abs()
+    if c.rtf:
+        b = b + 2.0 ** -11 * (y_ref.abs() + b)
+    y = t["y"].view(g.N, g.H * g.W, g.C)
+    worst = check_elementwise(f"{what} y", y, y_ref, b)
+    if c.rtf:
+        assert ((t["y"].view(torch.int32) & 0x1FFF) == 0).all(), f"{what}: round_tf32 y not TF32-representable"
+    assert (t["stats"] == 0).all(), f"{what}: the statistics accumulator is not handed back zeroed"
+    if not g.per_sample:
+        m, v = mean.view(-1), var.view(-1) * count / max(count - 1, 1)
+        rm = (1 - MOMENTUM) * run.rm0.double() + MOMENTUM * m
+        rv = (1 - MOMENTUM) * run.rv0.double() + MOMENTUM * v
+        worst = max(worst, check_elementwise(f"{what} running_mean", t["running_mean"], rm,
+                                             TOL * (run.rm0.double().abs() + x.abs().mean(dims).view(-1))))
+        worst = max(worst, check_elementwise(f"{what} running_var", t["running_var"], rv,
+                                             TOL * (run.rv0.double().abs() + v.abs())))
+        assert t["nbt"].item() == NBT0 + 1, f"{what}: num_batches_tracked {t['nbt'].item()}"
+
+    # backward, through the derivative of the kernel's own output
+    dz = dy * act_grad(c.act, y.double())
+    m1, m2 = dz.mean(dims, keepdim=True), (dz * xhat).mean(dims, keepdim=True)
+    dx_ref = ga * rstd * (dz - m1 - xhat * m2)
+    a1, a2 = dz.abs().mean(dims, keepdim=True), (dz * xhat).abs().mean(dims, keepdim=True)
+    b = TOL * ga.abs() * rstd * (dz.abs() + a1 + xhat.abs() * a2)
+    if c.rtf:
+        b = b + 2.0 ** -11 * (dx_ref.abs() + b)
+    dx = t["dx"].view(g.N, g.H * g.W, g.C)
+    worst = max(worst, check_elementwise(f"{what} dx", dx, dx_ref, b))
+    if c.rtf:
+        assert ((t["dx"].view(torch.int32) & 0x1FFF) == 0).all(), f"{what}: round_tf32 dx not TF32-representable"
+    if g.affine:
+        dgamma, dbeta = (dz * xhat).sum(dims).reshape(-1), dz.sum(dims).reshape(-1)
+        worst = max(worst, check_elementwise(f"{what} dgamma", t["dgb"][:run.G], dgamma,
+                                             TOL * (dz * xhat).abs().sum(dims).reshape(-1)))
+        worst = max(worst, check_elementwise(f"{what} dbeta", t["dgb"][run.G:], dbeta,
+                                             TOL * dz.abs().sum(dims).reshape(-1)))
+    assert (t["sums"] == 0).all(), f"{what}: the backward's sums workspace is not handed back zeroed"
+    return worst

@@ -240,8 +240,9 @@ def _cdiv(a, b):
     return -(-a // b)
 
 
-def nb_plan(nout, wrow, cin, N, Ho, Wo, ncls, allow_pt, groups, patch, sms=ch.NUM_SMS):
-    """nb_plan of narrow_block.cu without its tuning hook: (KT, PT, KG, TN, TR, TQ) or None"""
+def nb_plan(nout, wrow, cin, N, Ho, Wo, ncls, allow_pt, groups, patch, sms=ch.NUM_SMS, red=256):
+    """nb_plan of narrow_block.cu without its tuning hook: (KT, PT, KG, TN, TR, TQ) or None; red: the floats of the
+    cross-warp sums (the forward keeps them in fp64)"""
     kts = [16, 8, 4] if nout % 16 == 0 else [8, 4] if nout % 8 == 0 else [4] if nout % 4 == 0 else \
         [nout] if nout in (3, 6) else [1]
     best, best_cost = None, 1e30
@@ -257,7 +258,7 @@ def nb_plan(nout, wrow, cin, N, Ho, Wo, ncls, allow_pt, groups, patch, sms=ch.NU
                 TN = TP // (TQ * TR)
                 if (TN > 1 and TN // 2 >= N) or (groups > 1 and (N // groups) % TN):
                     continue
-                floats = ((wrow * KB + 3) & ~3) + ((patch(TN, TR, TQ) + 3) & ~3) + 2 * ((cin + 3) & ~3) + 256
+                floats = ((wrow * KB + 3) & ~3) + ((patch(TN, TR, TQ) + 3) & ~3) + 2 * ((cin + 3) & ~3) + red
                 if floats * 4 > 200 * 1024:
                     continue
                 blocks = _cdiv(N, TN) * _cdiv(Ho, TR) * _cdiv(Wo, TQ) * (nout // KB) * ncls
@@ -274,7 +275,7 @@ def plan_fprop(N, C, K, H, W, R, stride, pad=1, groups=1):
     P, Q = (H + 2 * pad - R) // stride + 1, (W + 2 * pad - R) // stride + 1
     CP = C + 4 if C % 4 == 0 else C
     b = nb_plan(K, R * R * C, C, N, P, Q, 1, R * R * C >= 16, groups,
-                lambda TN, TR, TQ: TN * ((TR - 1) * stride + R) * ((TQ - 1) * stride + R) * CP)
+                lambda TN, TR, TQ: TN * ((TR - 1) * stride + R) * ((TQ - 1) * stride + R) * CP, red=512)
     if b is None:
         return None
     KT, PT, KG, TN, TR, TQ = b
