@@ -9,6 +9,7 @@ become single fused nodes; anything unknown is executed leaf by leaf.
 
 There is no CPU / cuDNN fallback for the conv and norm modules: CPU tensors raise.
 """
+import dataclasses
 import warnings
 
 import torch
@@ -132,32 +133,39 @@ def _conv_cache(conv):
     return cache
 
 
-def _run_conv(conv, x, up=1, extra_pads=(0, 0, 0, 0), pad_mode=PAD_ZERO, act=ACT_NONE, slope=0.0, chan_scale=None,
-              stats=None, rtf_out=False, rtf_dz=False):
+def _conv_spec(conv, up=1, extra_pads=(0, 0, 0, 0), pad_mode=PAD_ZERO, act=ACT_NONE, slope=0.0, stats=None,
+               rtf_out=False, rtf_dz=False):
+    """The ConvSpec of `conv` behind an optional Upsample x`up` and padding layer: their pads add to the conv's own"""
     if not _conv_ok(conv):
         raise NotImplementedError(f"b200gan: unsupported convolution configuration: {conv}")
-    transposed = isinstance(conv, _T["ConvTranspose2d"])
-    pad = int(conv.padding[0])
-    if pad_mode == PAD_REFLECT and pad != 0:
+    return ConvSpec(stride=int(conv.stride[0]), pads=tuple(e + int(conv.padding[0]) for e in extra_pads),
+                    pad_mode=pad_mode, up=up, transposed=isinstance(conv, _T["ConvTranspose2d"]), act=act, slope=slope,
+                    stats=stats, rtf_out=rtf_out, rtf_dz=rtf_dz)
+
+
+def _run_conv(conv, x, spec, chan_scale=None):
+    if spec.pad_mode == PAD_REFLECT and int(conv.padding[0]) != 0:
         raise NotImplementedError("b200gan: reflection padding in front of a zero-padded conv")
-    if pad_mode == PAD_REFLECT and up == 1 and _tc_like(conv, 1):
+    if spec.pad_mode == PAD_REFLECT and spec.up == 1 and _tc_like(conv, 1):
         # tensor-core path wants zero padding (TMA out-of-bounds fill): materialise the mirrored border once
         # (cyclegan/models.py:27-28: ReflectionPad2d(1) -> Conv2d(256, 256, 3)) and run the conv un-padded
-        x = F.PadFn.apply(x, tuple(extra_pads), PAD_REFLECT, True)  # RN-round: operands of a TF32 MMA
-        extra_pads, pad_mode = (0, 0, 0, 0), PAD_ZERO
-    pads = tuple(e + pad for e in extra_pads)
-    spec = ConvSpec(stride=int(conv.stride[0]), pads=pads, pad_mode=pad_mode, up=up, transposed=transposed, act=act,
-                    slope=slope, stats=stats, rtf_out=rtf_out, rtf_dz=rtf_dz)
+        x = F.PadFn.apply(x, spec.pads, PAD_REFLECT, True)  # RN-round: operands of a TF32 MMA
+        spec = dataclasses.replace(spec, pads=(0, 0, 0, 0), pad_mode=PAD_ZERO)
     return F.conv_block(x, conv.weight, conv.bias, chan_scale, spec, _conv_cache(conv))
+
+
+def _cumulative_average(norm):
+    """True for a norm that keeps running statistics with momentum=None: their cumulative average no kernel computes"""
+    return norm.track_running_stats and norm.running_mean is not None and norm.momentum is None
 
 
 def _running_stats(norm):
     """(running_mean, running_var, num_batches_tracked, momentum) that a training-mode BatchNorm2d updates; Nones and
     0.0 if it keeps no running statistics"""
+    if _cumulative_average(norm):
+        raise NotImplementedError("b200gan: BatchNorm2d(momentum=None)")
     if not (norm.track_running_stats and norm.running_mean is not None):
         return None, None, None, 0.0
-    if norm.momentum is None:
-        raise NotImplementedError("b200gan: BatchNorm2d(momentum=None)")
     return norm.running_mean, norm.running_var, norm.num_batches_tracked, float(norm.momentum)
 
 
@@ -180,7 +188,7 @@ def _run_norm(norm, x, act=ACT_NONE, slope=0.0, stats=None, rtf_out=False, rtf_d
         raise ValueError(f"expected 4D input (got {x.dim()}D input)")
     if per_sample and x.shape[2] * x.shape[3] == 1 and norm.training:
         raise ValueError(f"Expected more than 1 spatial element when training, got input size {tuple(x.shape)}")
-    use_batch_stats = per_sample or norm.training or norm.running_mean is None
+    use_batch_stats = _uses_batch_stats(norm)
     if use_batch_stats and not per_sample:
         _no_groups("a stand-alone BatchNorm2d")
     if use_batch_stats:
@@ -205,14 +213,14 @@ def _gpu4d(x):
 # ---- leaf modules ----------------------------------------------------------------------------------
 class Conv2d(_T["Conv2d"]):
     def forward(self, x):
-        return _run_conv(self, x)
+        return _run_conv(self, x, _conv_spec(self))
 
 
 class ConvTranspose2d(_T["ConvTranspose2d"]):
     def forward(self, x, output_size=None):
         if output_size is not None:
             raise NotImplementedError("b200gan: ConvTranspose2d(output_size=...)")
-        return _run_conv(self, x)
+        return _run_conv(self, x, _conv_spec(self))
 
 
 class BatchNorm2d(_T["BatchNorm2d"]):
@@ -427,13 +435,15 @@ class CrossEntropyLoss(_T["CrossEntropyLoss"]):
 
 
 # ---- fusion planner ------------------------------------------------------------------------------------
+# A plan is a list of steps, each with run(x, stats, nchw_out) -> (output, the statistics it fused for the norm after it,
+# or None).  A fused step's run returns None when its input does not qualify; _run_step then runs the step's `fallback`,
+# the plan of its parts.
 class _ConvStep:
-    def __init__(self, conv, up, extra_pads, pad_mode, act, slope, dropout2d, stats):
+    def __init__(self, conv, up, extra_pads, pad_mode, act, slope, dropout2d, stats, next_norm):
         self.conv, self.up, self.extra_pads, self.pad_mode = conv, up, extra_pads, pad_mode
-        self.act, self.slope, self.dropout2d, self.stats = act, slope, dropout2d, stats
+        self.act, self.slope, self.dropout2d, self.stats, self.next_norm = act, slope, dropout2d, stats, next_norm
         self.rtf_out = False
         self.rtf_dz = False
-        self.next_norm = None
 
     def tc_like(self, full=False):
         if self.pad_mode == PAD_REFLECT and self.up != 1:
@@ -445,6 +455,18 @@ class _ConvStep:
         BatchNorm2d never consumes -- and so never re-zeroes -- the shared accumulator)"""
         return self.stats if (self.next_norm is not None and _uses_batch_stats(self.next_norm)) else None
 
+    def spec(self, stats=None):
+        return _conv_spec(self.conv, self.up, self.extra_pads, self.pad_mode, self.act, self.slope, stats, self.rtf_out,
+                          self.rtf_dz)
+
+    def run(self, x, stats, nchw_out):
+        scale = _step_dropout2d_scale(self, x.shape[0], x.device)
+        if scale is not None:
+            _no_groups("a Dropout2d outside a fused chain")
+        want = self.fused_stats()
+        out = _run_conv(self.conv, x, self.spec(want), scale)
+        return out if want is not None else (out, None)
+
 
 class _NormStep:
     def __init__(self, norm, act, slope, takes_stats):
@@ -452,18 +474,25 @@ class _NormStep:
         self.rtf_out = False
         self.rtf_dx = False
 
+    def run(self, x, stats, nchw_out):
+        return _run_norm(self.norm, x, self.act, self.slope, stats, self.rtf_out, self.rtf_dx), None
+
 
 class _LeafStep:
     def __init__(self, mod):
         self.mod = mod
 
+    def run(self, x, stats, nchw_out):
+        return self.mod(x), None
 
-class _TailStep:
-    """BatchNorm2d [-> LeakyReLU/ReLU] -> Conv2d(C, K<=3, 3, 1, 1) [-> act]: the fused Generator tail (dcgan.py:60-63).
-    Keeps the two steps it replaces for the cases the fused kernels do not take (eval mode, odd sizes)."""
 
-    def __init__(self, norm_step, conv_step):
-        self.norm_step, self.conv_step = norm_step, conv_step
+def _run_step(step, x, stats, nchw_out=False):
+    res = step.run(x, stats, nchw_out)
+    if res is not None:
+        return res
+    for part in step.fallback:
+        x, stats = _run_step(part, x, stats)
+    return x, stats
 
 
 def _no_hooks(m):
@@ -475,26 +504,77 @@ def _plain(m, name):
     return type(m) in (_T[name], REPLACEMENTS[name]) and _no_hooks(m)
 
 
-def _norm_conv_fused(ns, cs, x_shape):
-    """True if a norm step and the conv step after it run as functional.NormConvFn at this input shape: BatchNorm2d
-    [-> LeakyReLU/ReLU] with batch statistics (training mode) [-> Upsample x2] -> Conv2d, stride 1, zero padding, no
-    hooks, and a geometry whose data gradient can carry the norm's sums (dcgan.py:53-55, 56-59).  No side effects."""
-    if not (isinstance(ns, _NormStep) and isinstance(cs, _ConvStep)):
-        return False
-    norm, conv = ns.norm, cs.conv
-    if not isinstance(norm, _T["BatchNorm2d"]) or ns.act not in (ACT_NONE, ACT_LRELU, ACT_RELU):
-        return False
-    if isinstance(conv, _T["ConvTranspose2d"]) or cs.pad_mode != PAD_ZERO or tuple(conv.stride) != (1, 1):
-        return False
-    if not (_no_hooks(norm) and _no_hooks(conv) and norm.training and ops.bn_groups.active <= 1):
-        return False
-    if norm.track_running_stats and norm.momentum is None:
-        return False
-    if not (len(x_shape) == 4 and x_shape[1] == norm.num_features == conv.in_channels):
-        return False
-    pads = tuple(e + int(conv.padding[0]) for e in cs.extra_pads)
-    g, _ = ops.make_geom(tuple(x_shape), tuple(conv.weight.shape), 1, pads, PAD_ZERO, cs.up)
-    return ops.conv_dgrad_norm_supported(g)
+class _NormConvStep:
+    """BatchNorm2d [-> LeakyReLU/ReLU] [-> Upsample x2] -> Conv2d, stride 1, zero padding (dcgan.py:53-55, 56-59) as
+    functional.NormConvFn, whose backward takes the norm's sums from the conv's data-gradient epilogue: when the norm
+    normalises with batch statistics (training mode, no ops.bn_groups), neither module has hooks, and the geometry's
+    data gradient can carry the norm's sums."""
+
+    def __init__(self, norm_step, conv_step):
+        self.norm_step, self.conv_step = norm_step, conv_step
+        self.fallback = [norm_step, conv_step]
+
+    def run(self, x, stats, nchw_out):
+        ns, cs = self.norm_step, self.conv_step
+        norm, conv = ns.norm, cs.conv
+        if not (_no_hooks(norm) and _no_hooks(conv) and norm.training and ops.bn_groups.active <= 1):
+            return None
+        if not (x.dim() == 4 and x.shape[1] == norm.num_features == conv.in_channels):
+            return None
+        want = cs.fused_stats()
+        cspec = cs.spec(want)
+        g, _ = ops.make_geom(tuple(x.shape), tuple(conv.weight.shape), 1, cspec.pads, PAD_ZERO, cspec.up)
+        if not ops.conv_dgrad_norm_supported(g):
+            return None
+        nspec, rm, rv, nbt = _batch_norm_spec(norm, False, ns.act, ns.slope, ns.rtf_out, ns.rtf_dx)
+        scale = _step_dropout2d_scale(cs, x.shape[0], x.device)
+        out = F.NormConvFn.apply(x, norm.weight, norm.bias, stats, rm, rv, nbt, conv.weight, conv.bias, scale, nspec,
+                                 cspec, _conv_cache(conv))
+        return out if want is not None else (out, None)
+
+
+def _pair_candidate(ns, cs):
+    return (isinstance(ns, _NormStep) and isinstance(cs, _ConvStep) and isinstance(ns.norm, _T["BatchNorm2d"])
+            and ns.act in (ACT_NONE, ACT_LRELU, ACT_RELU) and not isinstance(cs.conv, _T["ConvTranspose2d"])
+            and cs.pad_mode == PAD_ZERO and tuple(cs.conv.stride) == (1, 1))
+
+
+def _fuse_two(steps, candidate, fused):
+    """steps with every adjacent (a, b) that `candidate` accepts replaced by fused(a, b), left to right"""
+    out, k = [], 0
+    while k < len(steps):
+        if k + 1 < len(steps) and candidate(steps[k], steps[k + 1]):
+            out.append(fused(steps[k], steps[k + 1]))
+            k += 2
+        else:
+            out.append(steps[k])
+            k += 1
+    return out
+
+
+def _fuse_pairs(steps):
+    return _fuse_two(steps, _pair_candidate, _NormConvStep)
+
+
+class _TailStep:
+    """BatchNorm2d [-> LeakyReLU/ReLU] -> Conv2d(C, K<=3, 3, 1, 1) [-> act]: the fused Generator tail (dcgan.py:60-63).
+    Falls back to its norm and conv for the cases the fused kernels do not take (eval mode, odd sizes)."""
+
+    def __init__(self, norm_step, conv_step):
+        self.norm_step, self.conv_step = norm_step, conv_step
+        self.fallback = _fuse_pairs([norm_step, conv_step])
+
+    def run(self, x, stats, nchw_out):
+        ns, cs = self.norm_step, self.conv_step
+        norm, conv = ns.norm, cs.conv
+        _no_groups("the fused generator tail")
+        if not (norm.training and x.shape[1] == conv.in_channels == norm.num_features
+                and ops.tail_supported(tuple(x.shape), conv.out_channels, ns.act, ns.slope, cs.act)):
+            return None
+        rm, rv, nbt, momentum = _running_stats(norm)
+        spec = F.TailSpec(eps=float(norm.eps), momentum=momentum, act_mid=ns.act, slope=ns.slope, act_out=cs.act,
+                          rtf_dx=ns.rtf_dx)
+        return F.TailFn.apply(x, stats, norm.weight, norm.bias, rm, rv, nbt, conv.weight, conv.bias, spec), None
 
 
 def _chain_plan(chain, shape):
@@ -509,12 +589,9 @@ def _chain_plan(chain, shape):
         macs = float(oshape[0]) * oshape[2] * oshape[3] * conv.out_channels * conv.in_channels * g.R * g.S
         if macs > _ChainStep.MAX_MACS or not ops.nb_supported(g) or oshape[2] * oshape[3] < 1:
             return None
-        if ns is not None:
-            norm = ns.norm
-            if not (norm.training and norm.num_features == conv.out_channels):
-                return None
-            if norm.track_running_stats and norm.momentum is None:
-                return None
+        if ns is not None and not (ns.norm.training and ns.norm.num_features == conv.out_channels
+                                   and not _cumulative_average(ns.norm)):
+            return None
         plan.append((cs, ns, oshape))
         shape = oshape
     return plan
@@ -526,7 +603,7 @@ def groups_eligible(seq, x_shape, groups):
     if not isinstance(seq, Sequential) or not ops.Config.fuse_narrow_chain or x_shape[0] % groups != 0:
         return False
     steps = seq._plan()
-    if not steps or not all(isinstance(st, _ChainStep) for st in steps):
+    if not steps or not all(isinstance(st, _ChainStep) and st.after is None for st in steps):
         return False
     shape = tuple(x_shape)
     with ops.bn_groups(groups):
@@ -540,18 +617,63 @@ def groups_eligible(seq, x_shape, groups):
 
 class _ChainStep:
     """A run of narrow [Conv2d -> act -> Dropout2d] (+ BatchNorm2d) blocks (dcgan.py:77-88) executed as the fused chain
-    of csrc/narrow_block.cu when the runtime shapes qualify; `steps` are the ordinary steps it stands for."""
+    of csrc/narrow_block.cu when the runtime shapes qualify; `steps` are the ordinary steps it stands for.  `after`: the
+    conv step behind a chain that ends in a norm, when the two would pair (_NormConvStep) if the chain fell back."""
 
     MAX_MACS = 6.0e8   # per layer: above this the tensor-core path is the better choice
 
-    def __init__(self, steps):
-        self.steps = steps
-        self.layers = []  # (conv step, norm step or None)
-        i = 0
-        while i < len(steps):
-            ns = steps[i + 1] if i + 1 < len(steps) and isinstance(steps[i + 1], _NormStep) else None
-            self.layers.append((steps[i], ns))
-            i += 2 if ns is not None else 1
+    def __init__(self, steps, after=None):
+        self.steps, self.after = steps, after
+        self.fallback = _fuse_pairs(steps + ([after] if after is not None else []))
+        self.layers = [(cs, ns if isinstance(ns, _NormStep) else None)  # (conv step, norm step or None)
+                       for cs, ns in zip(steps, steps[1:] + [None]) if isinstance(cs, _ConvStep)]
+
+    def run(self, x, stats, nchw_out):
+        shape = tuple(x.shape)
+        plan = _chain_plan(self, shape) if ops.Config.fuse_narrow_chain else None
+        if plan is None:
+            _no_groups("a conv chain that does not qualify for the fused kernels")
+            return None
+        groups = ops.bn_groups.active
+        if groups > 1 and shape[0] % groups != 0:
+            raise RuntimeError("b200gan: ops.bn_groups: the batch does not split evenly into the groups")
+        # Dropout2d masks.  One pass: drawn layer by layer as F.dropout2d does.  G statistics groups = G forward passes of
+        # the reference: pass 0 draws all its layers' masks, then pass 1, ... -- drawn up front in that order.
+        scales = [None] * len(plan)
+        for gq in range(groups):
+            for li, (cs, ns, oshape) in enumerate(plan):
+                part = _step_dropout2d_scale(cs, x.shape[0] // groups, x.device)
+                if part is not None:
+                    scales[li] = part if scales[li] is None else torch.cat([scales[li], part])
+        edge, prev_norm = None, None
+        chain = F.ChainPass()
+        for li, (cs, ns, oshape) in enumerate(plan):
+            conv = cs.conv
+            gam = bet = rm = rv = nbt = None
+            momentum = 0.0
+            if prev_norm is not None:
+                gam, bet = prev_norm.weight, prev_norm.bias
+                rm, rv, nbt, momentum = _running_stats(prev_norm)
+            spec = F.NbSpec(stride=int(conv.stride[0]), pad=int(conv.padding[0]), act=cs.act, slope=cs.slope,
+                            momentum=momentum, want_stats=ns is not None, groups=groups)
+            out_box = []
+            res = F.NbConvFn.apply(x, conv.weight, conv.bias, scales[li], gam, bet, rm, rv, nbt, edge, out_box, spec,
+                                   _conv_cache(conv), chain)
+            if ns is not None:
+                x, stats = res
+                norm = ns.norm
+                edge = ops.BnEdge(stats, None if norm.weight is None else norm.weight.detach(),
+                                  None if norm.bias is None else norm.bias.detach(), norm.eps,
+                                  oshape[0] // groups * oshape[2] * oshape[3], groups)
+                out_box.append(edge)
+                prev_norm = norm
+            else:
+                x, edge, prev_norm = res, None, None
+        if edge is not None:
+            rm, rv, nbt, momentum = _running_stats(prev_norm)
+            x = F.NbTailFn.apply(x, prev_norm.weight, prev_norm.bias, rm, rv, nbt, edge, momentum,
+                                 bool(nchw_out and self.after is None), chain)
+        return (x, None) if self.after is None else _run_step(self.after, x, None)
 
 
 def _chain_conv_candidate(cs):
@@ -586,8 +708,9 @@ def _fuse_chains(steps):
                 convs -= 1
                 break
         if convs >= 2:
-            out.append(_ChainStep(steps[i:j]))
-            i = j
+            after = steps[j] if j < n and _pair_candidate(steps[j - 1], steps[j]) else None
+            out.append(_ChainStep(steps[i:j], after))
+            i = j + (after is not None)
         else:
             out.append(steps[i])
             i += 1
@@ -599,21 +722,21 @@ def _uses_batch_stats(norm):
 
 
 def _tail_candidate(ns, cs):
-    if not (isinstance(ns, _NormStep) and isinstance(cs, _ConvStep)):
+    if not _pair_candidate(ns, cs) or cs.up != 1 or cs.extra_pads != (0, 0, 0, 0):
         return False
-    norm, conv = ns.norm, cs.conv
-    if not isinstance(norm, _T["BatchNorm2d"]) or ns.act not in (ACT_NONE, ACT_LRELU, ACT_RELU):
-        return False
-    if isinstance(conv, _T["ConvTranspose2d"]) or cs.up != 1 or cs.extra_pads != (0, 0, 0, 0) or cs.pad_mode != PAD_ZERO:
-        return False
-    if cs.dropout2d is not None or cs.stats is not None:
-        return False
-    return (tuple(conv.kernel_size) == (3, 3) and tuple(conv.stride) == (1, 1) and tuple(conv.padding) == (1, 1)
-            and conv.out_channels <= 3 and conv.in_channels in (32, 64, 128))
+    conv = cs.conv
+    return (cs.dropout2d is None and cs.stats is None and tuple(conv.kernel_size) == (3, 3)
+            and tuple(conv.padding) == (1, 1) and conv.out_channels <= 3 and conv.in_channels in (32, 64, 128))
 
 
 def _is_norm(m):
     return isinstance(m, (_T["BatchNorm2d"], _T["InstanceNorm2d"]))
+
+
+def _act_after(mods, j):
+    """(act, slope, index after it) of the activation module at mods[j], or (ACT_NONE, 0.0, j) if there is none"""
+    act = _act_of(mods[j]) if j < len(mods) else None
+    return (ACT_NONE, 0.0, j) if act is None else (*act, j + 1)
 
 
 def _build_plan(mods):
@@ -627,38 +750,23 @@ def _build_plan(mods):
             mode = PAD_REFLECT if isinstance(mods[j], _T["ReflectionPad2d"]) else PAD_ZERO
             j += 1
         conv = mods[j] if j < n else None
-        is_conv = isinstance(conv, (_T["Conv2d"], _T["ConvTranspose2d"])) and _conv_ok(conv)
-        if is_conv and isinstance(conv, _T["ConvTranspose2d"]) and (up != 1 or j != i):
-            is_conv = False
-        if is_conv and mode == PAD_REFLECT and int(conv.padding[0]) != 0:
-            is_conv = False
-        if is_conv:
-            j += 1
-            act, slope, d2 = ACT_NONE, 0.0, None
-            if j < n and _act_of(mods[j]) is not None:
-                act, slope = _act_of(mods[j])
-                j += 1
+        if (isinstance(conv, (_T["Conv2d"], _T["ConvTranspose2d"])) and _conv_ok(conv)
+                and not (isinstance(conv, _T["ConvTranspose2d"]) and (up != 1 or j != i))
+                and not (mode == PAD_REFLECT and int(conv.padding[0]) != 0)):
+            act, slope, j = _act_after(mods, j + 1)
+            d2 = None
             if j < n and isinstance(mods[j], _T["Dropout2d"]):
-                d2 = mods[j]
-                j += 1
-            stats = None
-            if j < n and _is_norm(mods[j]):
-                stats = isinstance(mods[j], _T["InstanceNorm2d"])
-            steps.append(_ConvStep(conv, up, extra, mode, act, slope, d2, stats))
-            steps[-1].next_norm = mods[j] if stats is not None else None
+                d2, j = mods[j], j + 1
+            norm = mods[j] if j < n and _is_norm(mods[j]) else None
+            stats = None if norm is None else isinstance(norm, _T["InstanceNorm2d"])
+            steps.append(_ConvStep(conv, up, extra, mode, act, slope, d2, stats, norm))
             i = j
             continue
         m = mods[i]
         if _is_norm(m):
-            j = i + 1
-            act, slope = ACT_NONE, 0.0
-            if j < n and _act_of(mods[j]) is not None:
-                act, slope = _act_of(mods[j])
-                j += 1
-            prev = steps[-1] if steps else None
-            takes = isinstance(prev, _ConvStep) and prev.stats is not None
+            act, slope, i = _act_after(mods, i + 1)
+            takes = bool(steps) and isinstance(steps[-1], _ConvStep) and steps[-1].stats is not None
             steps.append(_NormStep(m, act, slope, takes))
-            i = j
             continue
         steps.append(_LeafStep(m))
         i += 1
@@ -677,17 +785,8 @@ def _build_plan(mods):
             if (k + 1 < len(steps) and isinstance(steps[k + 1], _NormStep) and s.act == ACT_NONE
                     and s.dropout2d is None):
                 steps[k + 1].rtf_dx = True
-    steps = _fuse_chains(steps)
-    # the Generator tail: norm + narrow 3x3 conv as one fused node
-    fused, k = [], 0
-    while k < len(steps):
-        if k + 1 < len(steps) and _tail_candidate(steps[k], steps[k + 1]):
-            fused.append(_TailStep(steps[k], steps[k + 1]))
-            k += 2
-        else:
-            fused.append(steps[k])
-            k += 1
-    return fused
+    # precedence: chain > generator tail > norm-conv pair
+    return _fuse_pairs(_fuse_two(_fuse_chains(steps), _tail_candidate, _TailStep))
 
 
 def mlp_critic_layers(mods, in_features):
@@ -775,56 +874,6 @@ class Sequential(_T["Sequential"]):
             self.__dict__["_b200_plan"] = cached
         return cached[1]
 
-    def _run_chain(self, chain, x, nchw_out):
-        """Execute a _ChainStep through the fused kernels, or return None if the runtime shapes do not qualify."""
-        if not ops.Config.fuse_narrow_chain:
-            return None
-        shape = tuple(x.shape)
-        plan = _chain_plan(chain, shape)
-        if plan is None:
-            return None
-        groups = ops.bn_groups.active
-        if groups > 1 and shape[0] % groups != 0:
-            raise RuntimeError("b200gan: ops.bn_groups: the batch does not split evenly into the groups")
-        # Dropout2d masks.  One pass: drawn layer by layer as F.dropout2d does.  G statistics groups = G forward passes of
-        # the reference: pass 0 draws all its layers' masks, then pass 1, ... -- drawn up front in that order.
-        scales = [None] * len(plan)
-        for gq in range(groups):
-            for li, (cs, ns, oshape) in enumerate(plan):
-                part = _step_dropout2d_scale(cs, x.shape[0] // groups, x.device)
-                if part is not None:
-                    scales[li] = part if scales[li] is None else torch.cat([scales[li], part])
-        edge, prev_norm = None, None
-        chain = F.ChainPass()
-        for li, (cs, ns, oshape) in enumerate(plan):
-            conv = cs.conv
-            scale = scales[li]
-            gam = bet = rm = rv = nbt = None
-            momentum = 0.0
-            if prev_norm is not None:
-                gam, bet = prev_norm.weight, prev_norm.bias
-                rm, rv, nbt, momentum = _running_stats(prev_norm)
-            spec = F.NbSpec(stride=int(conv.stride[0]), pad=int(conv.padding[0]), act=cs.act, slope=cs.slope,
-                            momentum=momentum, want_stats=ns is not None, groups=groups)
-            out_box = []
-            res = F.NbConvFn.apply(x, conv.weight, conv.bias, scale, gam, bet, rm, rv, nbt, edge, out_box, spec,
-                                   _conv_cache(conv), chain)
-            if ns is not None:
-                x, stats = res
-                norm = ns.norm
-                edge = ops.BnEdge(stats, None if norm.weight is None else norm.weight.detach(),
-                                  None if norm.bias is None else norm.bias.detach(), norm.eps,
-                                  oshape[0] // groups * oshape[2] * oshape[3], groups)
-                out_box.append(edge)
-                prev_norm = norm
-            else:
-                x, edge, prev_norm = res, None, None
-        if edge is not None:
-            rm, rv, nbt, momentum = _running_stats(prev_norm)
-            x = F.NbTailFn.apply(x, prev_norm.weight, prev_norm.bias, rm, rv, nbt, edge, momentum, bool(nchw_out),
-                                 chain)
-        return x
-
     def _forward_2d(self, x):
         """Matrix input: the whole MLP critic (wgan_gp.py:72-78), the whole vanilla GAN discriminator (gan.py:64-80), the
         MLP generator, or Linear(K, 1) + activation (the adv_layer of a discriminator, dcgan.py:92) as one node."""
@@ -871,70 +920,12 @@ class Sequential(_T["Sequential"]):
         # torch.cat (pix2pix/models.py:50) without a layout round trip per block.
         want_contiguous = x.is_contiguous()
         stats = None
-        queue = list(steps)
-        while queue:
-            s = queue.pop(0)
-            if isinstance(s, _ChainStep):
-                at_end = not queue
-                res = self._run_chain(s, x, want_contiguous and at_end)
-                if res is None:
-                    _no_groups("a conv chain that does not qualify for the fused kernels")
-                    queue[0:0] = s.steps
-                else:
-                    x, stats = res, None
-                    if at_end and want_contiguous and x.is_contiguous():
-                        return x
-                continue
-            if isinstance(s, _TailStep):
-                ns, cs = s.norm_step, s.conv_step
-                norm, conv = ns.norm, cs.conv
-                _no_groups("the fused generator tail")
-                if (norm.training and x.shape[1] == conv.in_channels and x.shape[1] == norm.num_features
-                        and ops.tail_supported(tuple(x.shape), conv.out_channels, ns.act, ns.slope, cs.act)):
-                    rm, rv, nbt, momentum = _running_stats(norm)
-                    spec = F.TailSpec(eps=float(norm.eps), momentum=momentum, act_mid=ns.act, slope=ns.slope,
-                                      act_out=cs.act, rtf_dx=ns.rtf_dx)
-                    x = F.TailFn.apply(x, stats if ns.takes_stats else None, norm.weight, norm.bias, rm, rv, nbt,
-                                       conv.weight, conv.bias, spec)
-                    stats = None
-                else:
-                    queue[0:0] = [ns, cs]
-                continue
-            if queue and _norm_conv_fused(s, queue[0], tuple(x.shape)):
-                # one node whose backward takes the norm's sums from the conv's data-gradient epilogue
-                ns, cs = s, queue.pop(0)
-                scale = _step_dropout2d_scale(cs, x.shape[0], x.device)
-                want = cs.fused_stats()
-                norm, conv = ns.norm, cs.conv
-                nspec, rm, rv, nbt = _batch_norm_spec(norm, False, ns.act, ns.slope, ns.rtf_out, ns.rtf_dx)
-                cspec = ConvSpec(stride=1, pads=tuple(e + int(conv.padding[0]) for e in cs.extra_pads), up=cs.up,
-                                 act=cs.act, slope=cs.slope, stats=want, rtf_out=cs.rtf_out, rtf_dz=cs.rtf_dz)
-                out = F.NormConvFn.apply(x, norm.weight, norm.bias, stats if ns.takes_stats else None, rm, rv, nbt,
-                                         conv.weight, conv.bias, scale, nspec, cspec, _conv_cache(conv))
-                x, stats = out if want is not None else (out, None)
-                continue
-            if isinstance(s, _ConvStep):
-                cs = _step_dropout2d_scale(s, x.shape[0], x.device)
-                if cs is not None:
-                    _no_groups("a Dropout2d outside a fused chain")
-                want = s.fused_stats()
-                out = _run_conv(s.conv, x, s.up, s.extra_pads, s.pad_mode, s.act, s.slope, cs, want, s.rtf_out,
-                                s.rtf_dz)
-                if want is not None:
-                    x, stats = out
-                else:
-                    x, stats = out, None
-            elif isinstance(s, _NormStep):
-                x = _run_norm(s.norm, x, s.act, s.slope, stats if s.takes_stats else None, s.rtf_out, s.rtf_dx)
-                stats = None
-            else:
-                x = s.mod(x)
-                stats = None
+        for k, step in enumerate(steps):
+            x, stats = _run_step(step, x, stats, want_contiguous and k + 1 == len(steps))
         if (want_contiguous and torch.is_tensor(x) and x.dim() == 4 and not x.is_contiguous()
                 and x.shape[2] * x.shape[3] <= ops.Config.contiguous_hw_limit):
             x = F.ToContiguousFn.apply(x)
         return x
-
 
 REPLACEMENTS = {
     "Conv2d": Conv2d, "ConvTranspose2d": ConvTranspose2d, "BatchNorm2d": BatchNorm2d,

@@ -1,4 +1,4 @@
-"""Host-side logic of the fused narrow conv chain WITHOUT a GPU: the planner (nn._ChainStep / Sequential._run_chain) and the
+"""Host-side logic of the fused narrow conv chain WITHOUT a GPU: the planner (nn._ChainStep and its run) and the
 autograd protocol of functional.NbConvFn / NbTailFn -- virtual gradients w.r.t. the never-materialised BatchNorm outputs,
 the `sums` hand-over between neighbouring layers, dgamma / dbeta routing, frozen weights, two passes accumulating -- are
 run on CPU with the six C entry points (b200gan_nb_*) replaced by torch restatements of what each kernel computes

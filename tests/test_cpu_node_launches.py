@@ -3,10 +3,14 @@ arguments -- forward, first-order backward and backward under create_graph=True 
 Every `ops` launch wrapper is replaced by a recorder that logs "name(key arguments)" and returns zeros of the right shape
 and layout; the support queries are stubbed so that each route is taken on purpose, in both directions.  What the kernels
 compute is checked by the GPU tests; this pins the wiring: the same launches, no more and no fewer."""
+import functools
+import json
+import pathlib
+
 import pytest
 import torch
 
-from b200gan import _lib
+from b200gan import _lib, zoo
 
 CL = torch.channels_last
 ALGO = {_lib.ALGO_AUTO: "auto", _lib.ALGO_SIMT: "simt", _lib.ALGO_TC: "tc"}
@@ -703,3 +707,123 @@ def test_norm_conv_pair_through_sequential(rec, supported, next_norm):
     else:
         assert rec.take() == first + conv_bwd + ["conv_dgrad(tc)", "bias_grad(act=lrelu,scale)", "conv_wgrad(auto)",
                                                  "norm_backward(bn,act=relu,affine,params,ss)"]
+
+
+# ---- whole networks through nn.Sequential: every planned step, fused and fallen back ---------------------------------
+# The launch log of a forward and a backward through each network below, compared with tests/golden/
+# sequential_launch_logs.json.  The networks are run in training and eval mode, on NCHW and channels_last input, with
+# the four support queries all answering yes and all answering no; the small hand-built Sequentials, which pin the
+# order in which fused steps fall back, also with only `nb` or only `tail` answering no.
+GOLDEN_LOGS = pathlib.Path(__file__).parent / "golden" / "sequential_launch_logs.json"
+SUPPORT = {"all": (True, True, True, True), "none": (False, False, False, False),
+           "no_nb": (True, True, True, False), "no_tail": (True, True, False, True)}   # (tc, dgn, tail, nb)
+
+
+def _dragan_critic(ns, rec):
+    """the body of tests/scripts/mini_dragan's Critic: three strided conv blocks, the last two with a BatchNorm2d"""
+    layers = []
+    for i, (cin, cout) in enumerate(((1, 16), (16, 32), (32, 64))):
+        layers += [ns.Conv2d(cin, cout, 3, 2, 1), ns.LeakyReLU(0.2, inplace=True), ns.Dropout2d(0.25)]
+        if i:
+            layers.append(ns.BatchNorm2d(cout, 0.8))
+    return ns.Sequential(*layers)
+
+
+def _n1_decoder(ns, rec):
+    """tests/test_gpu_n1.py's ConvTranspose2d -> BatchNorm2d -> ReLU decoder, at narrower widths"""
+    def up(i, o):
+        return [ns.ConvTranspose2d(i, o, 4, 2, 1), ns.BatchNorm2d(o, 0.8), ns.ReLU()]
+
+    def down(i, o):
+        return [ns.Conv2d(i, o, 4, 2, 1), ns.BatchNorm2d(o, 0.8), ns.LeakyReLU(0.2)]
+    return ns.Sequential(*down(64, 128), *down(128, 256), ns.Conv2d(256, 512, 1), *up(512, 256), *up(256, 128),
+                         ns.Conv2d(128, 32, 3, 1, 1), ns.Tanh())
+
+
+def _hooked(rec, m):
+    m.register_forward_hook(lambda mod, inp, out: rec.log.append(f"hook({type(mod).__name__})"))
+    return m
+
+
+NETS = {  # name: (builder(ns, rec), input shape, hand-built)
+    "dcgan_g": (lambda ns, rec: zoo.DCGANGenerator(16, nn=ns).conv_blocks, (2, 128, 4, 4), False),
+    "dcgan_d": (lambda ns, rec: zoo.DCGANDiscriminator(16, nn=ns).model, (2, 1, 16, 16), False),
+    "dragan_critic": (_dragan_critic, (2, 1, 16, 16), False),
+    "pix2pix_down": (lambda ns, rec: zoo.UNetDown(64, 128, dropout=0.5, nn=ns).model, (2, 64, 8, 8), False),
+    "pix2pix_up": (lambda ns, rec: zoo.UNetUp(128, 64, dropout=0.5, nn=ns).model, (2, 128, 4, 4), False),
+    "pix2pix_final": (lambda ns, rec: ns.Sequential(ns.Upsample(scale_factor=2), ns.ZeroPad2d((1, 0, 1, 0)),
+                                                    ns.Conv2d(128, 3, 4, padding=1), ns.Tanh()), (2, 128, 8, 8), False),
+    "cyclegan_g": (lambda ns, rec: zoo.GeneratorResNet((3, 16, 16), 1, nn=ns).model, (2, 3, 16, 16), False),
+    "n1_decoder": (_n1_decoder, (2, 64, 16, 16), False),
+    # a chain of three convs whose parts hold a BatchNorm2d -> stride-1 Conv2d pair
+    "chain_with_pair": (lambda ns, rec: ns.Sequential(
+        ns.Conv2d(4, 16, 3, 2, 1), ns.LeakyReLU(0.2), ns.Conv2d(16, 32, 3, 2, 1), ns.LeakyReLU(0.2),
+        ns.BatchNorm2d(32), ns.Conv2d(32, 32, 3, 1, 1), ns.LeakyReLU(0.2), ns.BatchNorm2d(32)), (2, 4, 16, 16), True),
+    # a BatchNorm2d directly in front of a chain whose first conv has stride 1
+    "norm_before_chain": (lambda ns, rec: ns.Sequential(
+        ns.BatchNorm2d(4), ns.Conv2d(4, 16, 3, 1, 1), ns.LeakyReLU(0.2), ns.Conv2d(16, 32, 3, 2, 1),
+        ns.LeakyReLU(0.2), ns.BatchNorm2d(32)), (2, 4, 16, 16), True),
+    # a chain ending in a BatchNorm2d, followed by an Upsample -> Conv2d the chain cannot take
+    "chain_then_conv": (lambda ns, rec: ns.Sequential(
+        ns.Conv2d(4, 16, 3, 2, 1), ns.LeakyReLU(0.2), ns.Conv2d(16, 32, 3, 2, 1), ns.LeakyReLU(0.2),
+        ns.BatchNorm2d(32), ns.Upsample(scale_factor=2), ns.Conv2d(32, 32, 3, 1, 1)), (2, 4, 16, 16), True),
+    "tail": (lambda ns, rec: ns.Sequential(
+        ns.Conv2d(64, 64, 3, 1, 1), ns.BatchNorm2d(64, 0.8), ns.LeakyReLU(0.2), ns.Conv2d(64, 3, 3, 1, 1),
+        ns.Tanh()), (2, 64, 8, 8), True),
+    "hooked_pair_norm": (lambda ns, rec: ns.Sequential(
+        _hooked(rec, ns.BatchNorm2d(32)), ns.ReLU(), ns.Conv2d(32, 32, 3, 1, 1)), (2, 32, 8, 8), True),
+    "hooked_pair_conv": (lambda ns, rec: ns.Sequential(
+        ns.BatchNorm2d(32), ns.ReLU(), _hooked(rec, ns.Conv2d(32, 32, 3, 1, 1))), (2, 32, 8, 8), True),
+    "hooked_before_pair": (lambda ns, rec: ns.Sequential(
+        _hooked(rec, ns.Conv2d(32, 32, 3, 1, 1)), ns.BatchNorm2d(32), ns.ReLU(), ns.Conv2d(32, 32, 3, 1, 1)),
+        (2, 32, 8, 8), True),
+}
+SEQUENTIAL_CASES = [f"{name}-{mode}-{layout}-{sup}" for name, (_, _, hand) in NETS.items()
+                    for mode in ("train", "eval") for layout in ("nchw", "cl")
+                    for sup in (SUPPORT if hand else ("all", "none"))]
+SEQUENTIAL_CASES += [f"{name}-train-cl-{sup}-groups2" for name in ("dcgan_d", "dragan_critic", "tail")
+                     for sup in ("all", "none")]
+SEQUENTIAL_CASES += [f"{name}-train-cl-{sup}-create_graph" for name in ("dcgan_d", "dragan_critic")
+                     for sup in ("all", "no_nb")]
+
+
+def sequential_log(rec, case):
+    """{"fwd": launches, "bwd": launches, "out": shape and layout}; a raised error ends its phase's list"""
+    from b200gan import ops
+    name, mode, layout, sup, *extra = case.split("-")
+    build, shape, _ = NETS[name]
+    rec.tc, rec.dgn, rec.tail, rec.nb = SUPPORT[sup]
+    torch.manual_seed(0)
+    seq = build(zoo.namespace(), rec).train(mode == "train")
+    x = torch.zeros(shape)
+    x = (x if layout == "nchw" else x.contiguous(memory_format=CL)).requires_grad_(True)
+    inputs = [x] + [q for q in seq.parameters() if q.requires_grad]
+    log = {}
+    with ops.bn_groups(2 if "groups2" in extra else 1):
+        try:
+            y = seq(x)
+        except (RuntimeError, NotImplementedError, ValueError) as e:
+            return {"fwd": rec.take() + [f"raise {type(e).__name__}: {e}"]}
+        log["fwd"] = rec.take()
+        log["out"] = [list(y.shape), "nchw" if y.is_contiguous() else "cl"]
+        try:
+            torch.autograd.grad(y, inputs, torch.zeros_like(y), allow_unused=True,
+                                create_graph="create_graph" in extra)
+            log["bwd"] = rec.take()
+        except (RuntimeError, NotImplementedError) as e:
+            log["bwd"] = rec.take() + [f"raise {type(e).__name__}: {e}"]
+    return log
+
+
+@functools.lru_cache(maxsize=None)
+def _golden_logs():
+    return json.loads(GOLDEN_LOGS.read_text())
+
+
+def test_every_sequential_case_has_a_golden_log():
+    assert sorted(_golden_logs()) == sorted(SEQUENTIAL_CASES)
+
+
+@pytest.mark.parametrize("case", SEQUENTIAL_CASES)
+def test_sequential_launch_log(rec, case):
+    assert sequential_log(rec, case) == _golden_logs()[case]

@@ -147,24 +147,30 @@ def test_patch_rebinds_and_restores_torch_nn():
     assert tnn.Conv2d is stock
 
 
-def test_fusion_plan_for_dcgan():
+def test_fusion_plan_for_dcgan_pairs_norms_with_convs():
     from b200gan import nn as bnn, zoo
     g, d = zoo.DCGANGenerator(64), zoo.DCGANDiscriminator(64)
-    kinds = [type(s).__name__ for s in bnn._build_plan(list(g.conv_blocks))]
-    # BatchNorm2d(64, .8) + LeakyReLU + Conv2d(64, 1, 3, 1, 1) + Tanh (dcgan.py:60-63) is the fused tail node
-    assert kinds == ["_NormStep", "_ConvStep", "_NormStep", "_ConvStep", "_TailStep"]
     steps = bnn._build_plan(list(g.conv_blocks))
-    tail = steps[4]
-    assert steps[1].up == 2 and steps[3].up == 2 and tail.conv_step.up == 1
-    assert steps[1].stats is False and steps[3].stats is False and steps[3].next_norm is g.conv_blocks[7]
+    # two BatchNorm2d -> Upsample -> Conv2d pairs (dcgan.py:53-59), then BatchNorm2d(64, .8) + LeakyReLU +
+    # Conv2d(64, 1, 3, 1, 1) + Tanh (dcgan.py:60-63) as the fused tail node
+    assert [type(s).__name__ for s in steps] == ["_NormConvStep", "_NormConvStep", "_TailStep"]
+    pairs, tail = steps[:2], steps[2]
+    assert [[type(s).__name__ for s in p.fallback] for p in pairs] == [["_NormStep", "_ConvStep"]] * 2
+    assert pairs[0].conv_step.up == 2 and pairs[1].conv_step.up == 2 and tail.conv_step.up == 1
+    assert pairs[0].conv_step.stats is False and pairs[1].conv_step.stats is False
+    assert pairs[1].conv_step.next_norm is g.conv_blocks[7]
     assert tail.norm_step.takes_stats and tail.norm_step.act == 1 and tail.norm_step.rtf_dx
     assert tail.conv_step.stats is None and tail.conv_step.act == 3
+    # when the fused tail does not take its input, its norm and conv fall back as one more pair
+    assert [type(s).__name__ for s in tail.fallback] == ["_NormConvStep"]
+    assert (tail.fallback[0].norm_step, tail.fallback[0].conv_step) == (tail.norm_step, tail.conv_step)
     # the four discriminator blocks (dcgan.py:77-88) form one fused chain; its constituent steps stay available
     plan = bnn._build_plan(list(d.model))
     assert [type(s).__name__ for s in plan] == ["_ChainStep"]
     dsteps = plan[0].steps
     assert [type(s).__name__ for s in dsteps] == ["_ConvStep", "_ConvStep", "_NormStep", "_ConvStep", "_NormStep",
                                                   "_ConvStep", "_NormStep"]
+    assert plan[0].fallback == dsteps and plan[0].after is None   # no norm there is followed by a stride-1 conv
     assert all(s.dropout2d is not None for s in dsteps if isinstance(s, bnn._ConvStep))
     assert dsteps[0].stats is None and dsteps[1].stats is False
     assert [(type(a).__name__, type(b).__name__) for a, b in plan[0].layers] == [

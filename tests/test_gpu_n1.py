@@ -27,15 +27,19 @@ def _decoder(ns):
                          ns.Conv2d(128, 32, 3, 1, 1), ns.Tanh())
 
 
-def test_plan_fuses_conv_transpose_batchnorm_relu():
+def test_plan_fuses_conv_transpose_batchnorm_relu_and_pairs_norm_conv():
     from b200gan import nn as bnn, zoo
     m = _decoder(zoo.namespace())
-    kinds = [(type(s).__name__, getattr(s, "stats", None)) for s in m._plan()]
+    plan = m._plan()
+    # a BatchNorm2d in front of a stride-1 Conv2d pairs with it (functional.NormConvFn); the others stay single steps
+    assert [type(s).__name__ for s in plan] == ["_ConvStep", "_NormStep", "_ConvStep", "_NormConvStep", "_ConvStep",
+                                                "_NormStep", "_ConvStep", "_NormConvStep"]
+    steps = [p for s in plan for p in (s.fallback if isinstance(s, bnn._NormConvStep) else [s])]
+    kinds = [(type(s).__name__, getattr(s, "stats", None)) for s in steps]
     # every (transposed) conv in front of a BatchNorm carries the fused statistics; the norm steps take them
     assert kinds == [("_ConvStep", False), ("_NormStep", None), ("_ConvStep", False), ("_NormStep", None),
                      ("_ConvStep", None), ("_ConvStep", False), ("_NormStep", None), ("_ConvStep", False),
                      ("_NormStep", None), ("_ConvStep", None)]
-    steps = m._plan()
     assert all(s.takes_stats for s in steps if isinstance(s, bnn._NormStep))
     assert steps[5].conv.__class__.__name__ == "ConvTranspose2d" and steps[6].act == 2   # ReLU fused into the norm
 
