@@ -153,6 +153,10 @@ int b200gan_conv2d_wgrad(const b200gan_conv_geom *g, const float *x, const float
  * values it already holds, instead of by a separate pass over dy (the other routes and ConvTranspose2d: as above). */
 int b200gan_conv2d_wgrad_fused_bias(const b200gan_conv_geom *g, const float *x, const float *dy, float *dw,
                                     float *db, float *workspace, int algo, void *stream);
+/* 1 if the tensor-core weight gradient of g runs phase-major, else 0: a Conv2d after Upsample x2 whose input x has a
+ * multiple of 128 channels (and dy does not) on maps at least 8 pixels wide.  Each CTA then computes the four taps of
+ * one output phase from one transpose of dy and one halo box of x. */
+int b200gan_conv2d_wgrad_phase_major(const b200gan_conv_geom *g);
 
 /* dz = dy * act'(y) * chan_scale  -- backward of the fused fprop epilogue, from the saved
  * output y (LeakyReLU/ReLU sign and Tanh/Sigmoid derivative are functions of y).

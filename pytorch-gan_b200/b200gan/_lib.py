@@ -101,6 +101,7 @@ SIGNATURES = {
     "b200gan_conv2d_wgrad_workspace_floats": (c_sz, [_P(ConvGeom), c_i32]),
     "b200gan_conv2d_wgrad": (c_i32, [_P(ConvGeom), c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_vp]),
     "b200gan_conv2d_wgrad_fused_bias": (c_i32, [_P(ConvGeom), c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_vp]),
+    "b200gan_conv2d_wgrad_phase_major": (c_i32, [_P(ConvGeom)]),
     "b200gan_epilogue_bwd": (c_i32, [c_vp, c_vp, c_vp, c_i32, c_f32, c_i64, c_i32, c_i64, c_i32, c_vp, c_vp]),
     "b200gan_bias_grad": (c_i32, [c_vp, c_vp, c_vp, c_i32, c_f32, c_i64, c_i32, c_i64, c_vp, c_vp]),
     "b200gan_norm_stats": (c_i32, [_P(NormDesc), c_vp, c_vp, c_vp]),

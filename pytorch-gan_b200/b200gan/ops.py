@@ -186,6 +186,11 @@ def conv_wgrad(g, x, dy, weight_shape, need_bias, algo):
     return dw, db
 
 
+def conv_wgrad_phase_major(g):
+    """whether the tensor-core weight gradient of g computes the four taps of an upsample phase per CTA"""
+    return bool(_lib.load().b200gan_conv2d_wgrad_phase_major(ctypes.byref(g)))
+
+
 def epilogue_bwd(dy, y, chan_scale, act, slope, round_tf32=False):
     n, k, p, q = dy.shape
     dz = torch.empty_like(dy, memory_format=CL)

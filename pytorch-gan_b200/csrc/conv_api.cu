@@ -44,6 +44,7 @@ struct TcNormBwd;
 int tc_dgrad(const b200gan_conv_geom *g, const float *dy, const float *packed, float *dx, const TcNormBwd *nb,
              cudaStream_t st);
 size_t tc_wgrad_workspace_floats(const b200gan_conv_geom *g);
+int tc_wgrad_phase_major(const b200gan_conv_geom *g);
 int tc_wgrad(const b200gan_conv_geom *g, const float *x, const float *dy, float *dw, float *db, float *ws,
              cudaStream_t st);
 
@@ -505,6 +506,11 @@ static int conv2d_wgrad(const b200gan_conv_geom *g, const float *x, const float 
   if (rc) return rc;
   if (db) return simt_colsum(dy, db, (int64_t)g->N * g->P * g->Q, g->K, st);
   return B200GAN_OK;
+}
+
+extern "C" int b200gan_conv2d_wgrad_phase_major(const b200gan_conv_geom *g) {
+  if (!g || validate_geom(g) || !tc_supported(g, 2)) return 0;
+  return tc_wgrad_phase_major(g);
 }
 
 extern "C" int b200gan_conv2d_wgrad(const b200gan_conv_geom *g, const float *x, const float *dy, float *dw,

@@ -18,6 +18,12 @@
 // registers, stages the tile in shared memory and adds it into the job's [M'][N'] matrix with a TMA reduce-store
 // (cp.reduce.async.bulk.tensor ... .add: the fp32 additions happen at L2); wgrad_reduce_kernel then folds the
 // jobs into the parameter layout [K][C][R][S].
+//
+// Phase-major mode (the upsample fold with x as A, boxes at least 8 pixels wide): the four taps of one output phase read
+// the same dy quarter, and their x windows are the 2x2 shifts of one halo box.  A CTA then runs all four taps of its
+// phase (blockIdx.y = 4 phase + q) over quarter q of its split's tiles: dy is loaded and transposed once per stage for
+// four MMAs, and x arrives as one (BW+1) x (BH+1) halo box instead of four 32-pixel boxes.  Same grid, same partial
+// matrices, same reduce.
 #include "tc_common.cuh"
 #include <stdlib.h>
 
@@ -27,6 +33,10 @@ constexpr int WG_THREADS = 384;  // producer warpgroup + two consumer warpgroups
 constexpr int WG_MAX_JOBS = 52;
 constexpr int WG_PIX = 32;       // pixels (GEMM-K) per pipeline stage
 constexpr int WG_CHUNK_BYTES = WG_PIX * 128;  // one 32-channel chunk of one stage
+constexpr int WG_PH_STAGES = 4;  // ring stages of the phase-major mode
+// one 32-channel chunk of an x halo box: (BW+1) (BH+1) rows per image, at most 72 (8 x 1 pixels x 4 images), in 1024-byte
+// units (128-byte swizzle atoms)
+constexpr int WG_HALO_BYTES = 9216;
 
 // One job = one filter tap (or one (phase, tap) pair of the upsample fold).  "S" is the operand that is shifted by
 // the tap (x for Conv2d, dy for ConvTranspose2d), "D" the one that is read at the loop pixel.
@@ -46,6 +56,7 @@ struct WgParams {
   int32_t imgs_per_box;           // 32 / (BW * BH)
   int32_t tiles_total, tiles_per_split;
   int32_t s_is_a;                 // 1: A = shifted operand S, B = D; 0: A = D, B = S
+  int32_t phase_major;            // 1: the four taps of a phase per CTA, x as a halo box (tmX has the halo box)
   int32_t mtiles, ntiles;         // tiles of the (M', N') output
   int32_t ldn;                    // N' total (row length of a partial matrix)
   int32_t mtotal;                 // M' total
@@ -65,7 +76,19 @@ struct WgSmem {
   static constexpr int MAIN = RING + 2 * T_BYTES > STAGING ? RING + 2 * T_BYTES : STAGING;
   static constexpr int TOTAL = MAIN + 1024 + 256;
   static_assert(TOTAL <= 232448, "wgrad_tc_kernel: shared memory");
+  // phase-major mode (NB <= 64): WG_PH_STAGES stages of four x halo chunks + dy inside the ring, in front of the same
+  // two B buffers; the epilogue stages the four taps' tiles in the retired ring
+  static constexpr int PH_A_BYTES = 4 * WG_HALO_BYTES;
+  static constexpr int PH_STAGE_BYTES = PH_A_BYTES + B_BYTES;
+  static_assert(NB > 64 || (WG_PH_STAGES * PH_STAGE_BYTES <= RING && 4 * STAGING <= RING),
+                "wgrad_tc_kernel: phase-major ring");
 };
+
+__device__ __forceinline__ uint32_t wg_lds32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr));
+  return v;
+}
 
 __device__ __forceinline__ void wg_consumers_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
@@ -73,6 +96,29 @@ __device__ __forceinline__ void wg_consumers_sync() { asm volatile("bar.sync 1, 
 // Thread (l%4) of an A fragment then reads pixels 2(l%4) and 2(l%4) + 1, whose rows have distinct 128-byte swizzle
 // phases for the four values of l%4: the 32 lanes of one fragment load hit 32 different banks.
 __device__ __forceinline__ int wg_kpos(int p) { return (p & ~7) | ((p & 7) >> 1) | ((p & 1) << 2); }
+
+// B = the stage's NB channels of 32 pixel rows (MN-major, 128B swizzle) -> K-major tile tb (NB channel rows of 32
+// pixels); thread (tp, tq) moves pixel row tp, channels tq * 4 + [0, 4) of every chunk, and with db adds them to dsb
+template <int NB>
+__device__ __forceinline__ void wg_transpose_b(const uint8_t *src, uint8_t *tb, int tp, int tq, int tk, bool db,
+                                               float *dsb) {
+#pragma unroll
+  for (int c = 0; c < NB / 32; ++c) {
+    const float4 v = *reinterpret_cast<const float4 *>(src + c * WG_CHUNK_BYTES + tp * 128 + ((tq ^ (tp & 7)) << 4));
+    const float e[4] = {v.x, v.y, v.z, v.w};
+    if constexpr (NB <= 64) {
+      if (db) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) dsb[4 * c + i] += e[i];
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int r = c * 32 + tq * 4 + i;
+      *reinterpret_cast<float *>(tb + r * 128 + (((tk >> 2) ^ (r & 7)) << 4) + (tk & 3) * 4) = e[i];
+    }
+  }
+}
 
 template <int NB, int STAGES>
 __global__ void __launch_bounds__(WG_THREADS, 1)
@@ -85,12 +131,19 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
   uint64_t *empty = full + STAGES;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int split = blockIdx.x, job = blockIdx.y;
+  const bool phm = NB <= 64 && p.phase_major;
+  const int split = blockIdx.x;
+  const int job = phm ? blockIdx.y & ~3 : blockIdx.y;  // phase-major: the phase's tap-(0, 0) job, 4 phase
   const int mt = blockIdx.z / p.ntiles, nt = blockIdx.z % p.ntiles;
-  const int t_begin = split * p.tiles_per_split;
+  int t_begin = split * p.tiles_per_split;
   int t_end = t_begin + p.tiles_per_split;
   if (t_end > p.tiles_total) t_end = p.tiles_total;
-  const int iters = t_end - t_begin;
+  if (phm) {  // quarter blockIdx.y % 4 of the split's tiles; the last ones may be short or empty
+    const int qn = (t_end - t_begin + 3) >> 2;
+    t_begin += (blockIdx.y & 3) * qn;
+    if (t_end > t_begin + qn) t_end = t_begin + qn;
+  }
+  const int iters = t_end > t_begin ? t_end - t_begin : 0;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmX);
@@ -113,6 +166,12 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
       const int a_dw = p.s_is_a ? jb.s_dw : 0, a_dh = p.s_is_a ? jb.s_dh : 0;
       const int b_dc = p.s_is_a ? jb.d_dc : jb.s_dc, b_da = p.s_is_a ? jb.d_da : jb.s_da;
       const int b_dw = p.s_is_a ? 0 : jb.s_dw, b_dh = p.s_is_a ? 0 : jb.s_dh;
+      // phase-major: A = the x halo box {32, BW+1, 1, BH+1, ipb} at the tap-(0, 0) shift, chunks WG_HALO_BYTES apart
+      const int nst = phm ? WG_PH_STAGES : STAGES;
+      const int a_pitch = phm ? WG_HALO_BYTES : WG_CHUNK_BYTES;
+      const int stage_bytes = phm ? L::PH_STAGE_BYTES : L::STAGE_BYTES;
+      const uint32_t tx = phm ? 4 * 128 * ((1 << p.bw_log2) + 1) * ((1 << p.bh_log2) + 1) * p.imgs_per_box + L::B_BYTES
+                              : L::STAGE_BYTES;
       int stage = 0;
       uint32_t phase = 0;
       for (int it = 0; it < iters; ++it) {
@@ -123,18 +182,18 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
         const int n = (t / p.tiles_h) * p.imgs_per_box;  // a box spans several images when H*W < WG_PIX
         const int w0 = tw << p.bw_log2, h0 = th << p.bh_log2;
         mbar_wait(&empty[stage], phase ^ 1);
-        uint8_t *sa = smem + stage * L::STAGE_BYTES;
-        uint8_t *sb = sa + L::A_BYTES;
-        mbar_arrive_expect_tx(&full[stage], L::STAGE_BYTES);
+        uint8_t *sa = smem + stage * stage_bytes;
+        uint8_t *sb = sa + 4 * a_pitch;
+        mbar_arrive_expect_tx(&full[stage], tx);
 #pragma unroll
         for (int c = 0; c < 4; ++c)
-          tma_load_5d(sa + c * WG_CHUNK_BYTES, mapA, &full[stage], a_dc + (mt * 4 + c) * 32, w0 + a_dw, a_da,
+          tma_load_5d(sa + c * a_pitch, mapA, &full[stage], a_dc + (mt * 4 + c) * 32, w0 + a_dw, a_da,
                       h0 + a_dh, n);
 #pragma unroll
         for (int c = 0; c < NB / 32; ++c)
           tma_load_5d(sb + c * WG_CHUNK_BYTES, mapB, &full[stage], b_dc + (nt * (NB / 32) + c) * 32, w0 + b_dw, b_da,
                       h0 + b_dh, n);
-        if (++stage == STAGES) {
+        if (++stage == nst) {
           stage = 0;
           phase ^= 1;
         }
@@ -168,8 +227,110 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
     float dsb[NB <= 64 ? NB / 8 : 1];
 #pragma unroll
     for (int i = 0; i < (NB <= 64 ? NB / 8 : 1); ++i) dsb[i] = 0.f;
+    auto flush_dsb = [&]() {  // lane = pixel row tp of the stage
+      if constexpr (NB <= 64) {
+        if (dbB) {
+#pragma unroll
+          for (int i = 0; i < NB / 8; ++i) {
+            float s = dsb[i];
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+            if (lane == 0) atomicAdd(p.db + nt * NB + (i >> 2) * 32 + tq * 4 + (i & 3), s);
+          }
+        }
+      }
+    };
     int stage = 0;
     uint32_t phase = 0;
+    if constexpr (NB <= 64) {
+      if (phm) {
+        // Phase-major: tap t = (dr, ds) = (t >> 1, t & 1) of the phase reads x at pixel (h + dr, w + ds) of the halo
+        // box, whose row for box pixel (image i, row h, column w) is (i (BH+1) + h) (BW+1) + w.  BW >= 8, so the 8
+        // pixels of a k slice lie in one box row and take consecutive halo rows.  hoff[k][j]: this thread's A
+        // fragment element (channel ac, halo row hrow(8k) + ap + j) of tap (0, 0) at j = 0 (a0) and 1 (a2); channel
+        // ac + 8 sits at hoff ^ 32 (its 16-byte unit is (ac / 4) ^ 2), and tap (dr, ds) at hoff[k][j + dr + ds] +
+        // dr BW 128 (BW is a multiple of 8: + BW rows keep the swizzle phase).  Rows hrow + ap + {0, 2, 4, 6} of the
+        // four lanes l % 4 have distinct swizzle phases for any hrow, so a fragment load hits 32 different banks.
+        uint32_t hoff[WG_PIX / 8][4];
+#pragma unroll
+        for (int k = 0; k < WG_PIX / 8; ++k) {
+          const int q = 8 * k, r = q >> p.bw_log2, img = r >> p.bh_log2;
+          const int row0 = q + r + img * ((1 << p.bw_log2) + 1) + ap;
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            const int row = row0 + j;
+            hoff[k][j] = (uint32_t)((2 * half + (wq >> 1)) * WG_HALO_BYTES + row * 128 + (((ac >> 2) ^ (row & 7)) << 4) +
+                                    (ac & 3) * 4);
+          }
+        }
+        const int bw_bytes = 128 << p.bw_log2;
+        float acc4[4][NB / 2];  // the first MMA of each tap overwrites it (scale_d = 0)
+        uint32_t fa[2][16];
+        // dy of stage `it` -> K-major B buffer it & 1, once for the four taps
+        auto transpose = [&](int it) {
+          mbar_wait(&full[stage], phase);
+          wg_consumers_sync();  // both warpgroups' MMAs of iteration it-2 (which read this buffer) have retired
+          wg_transpose_b<NB>(smem + stage * L::PH_STAGE_BYTES + L::PH_A_BYTES, smem + L::RING + (it & 1) * L::T_BYTES,
+                             tp, tq, tk, dbB, dsb);
+          fence_proxy_async();  // generic-proxy smem writes -> visible to wgmma
+          wg_consumers_sync();
+        };
+        // the four taps of stage `it`: tap t's fragments load into set t & 1 while tap t-1's MMAs run
+        auto taps = [&](int it) {
+          const uint32_t xs = smem_u32(smem) + stage * L::PH_STAGE_BYTES;
+          const uint32_t sb = smem_u32(smem + L::RING + (it & 1) * L::T_BYTES);
+#pragma unroll
+          for (int t = 0; t < 4; ++t) {
+            const int j0 = (t >> 1) + (t & 1);
+            const uint32_t xt = xs + (t >> 1) * bw_bytes;
+            uint32_t *f = fa[t & 1];
+            wgmma_wait<1>();  // tap t-2, the last reader of this fragment set, has retired
+#pragma unroll
+            for (int k = 0; k < WG_PIX / 8; ++k) {
+              f[4 * k + 0] = wg_lds32(xt + hoff[k][j0]);
+              f[4 * k + 1] = wg_lds32(xt + (hoff[k][j0] ^ 32));
+              f[4 * k + 2] = wg_lds32(xt + hoff[k][j0 + 1]);
+              f[4 * k + 3] = wg_lds32(xt + (hoff[k][j0 + 1] ^ 32));
+            }
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < WG_PIX / 8; ++k)
+              wgmma_tf32_rs<NB>(acc4[t], f + 4 * k, gmma_desc_sw128(sb + k * 32), (it > 0 || k > 0) ? 1u : 0u);
+            wgmma_commit();
+          }
+          mbar_arrive(&empty[stage]);
+          if (++stage == WG_PH_STAGES) {
+            stage = 0;
+            phase ^= 1;
+          }
+        };
+        transpose(0);
+#pragma unroll 1
+        for (int it = 0; it < iters; ++it) {
+          taps(it);
+          if (it + 1 < iters) transpose(it + 1);
+        }
+        wgmma_wait<0>();
+#pragma unroll
+        for (int t = 0; t < 4; ++t) wgmma_fence_regs<NB / 2>(acc4[t]);
+        flush_dsb();
+        wg_consumers_sync();  // every MMA has retired: the ring is free for the four staging tiles
+#pragma unroll
+        for (int t = 0; t < 4; ++t) store_acc_sw128<NB>(smem + t * L::STAGING, acc4[t], half * 64);
+        fence_proxy_async();
+        wg_consumers_sync();
+        if (ct == 0) {
+#pragma unroll 1
+          for (int t = 0; t < 4; ++t) {
+            const int row0 = (job + t) * p.mtotal + mt * 128;  // job 4 phase + t = (phase, tap t)
+            for (int c = 0; c < NB; c += 32)
+              tma_reduce_add_2d(&tmP, smem + t * L::STAGING + (c >> 5) * 16384, nt * NB + c, row0);
+          }
+          tma_store_commit_and_wait_read();
+        }
+        return;
+      }
+    }
     // stage `it` -> A fragments fa and the K-major B tile of buffer it & 1; the ring slot is released afterwards
     auto prepare = [&](int it, uint32_t(&fa)[16]) {
       uint8_t *tb = smem + L::RING + (it & 1) * L::T_BYTES;  // B^T: NB rows x 128 B
@@ -187,23 +348,7 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
           dsa1 += __uint_as_float(fa[4 * k + 1]) + __uint_as_float(fa[4 * k + 3]);
         }
       }
-#pragma unroll
-      for (int c = 0; c < NB / 32; ++c) {
-        const float4 v = *reinterpret_cast<const float4 *>(src + L::A_BYTES + c * WG_CHUNK_BYTES + tp * 128 +
-                                                           ((tq ^ (tp & 7)) << 4));
-        const float e[4] = {v.x, v.y, v.z, v.w};
-        if constexpr (NB <= 64) {
-          if (dbB) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) dsb[4 * c + i] += e[i];
-          }
-        }
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int r = c * 32 + tq * 4 + i;
-          *reinterpret_cast<float *>(tb + r * 128 + (((tk >> 2) ^ (r & 7)) << 4) + (tk & 3) * 4) = e[i];
-        }
-      }
+      wg_transpose_b<NB>(src + L::A_BYTES, tb, tp, tq, tk, dbB, dsb);
       mbar_arrive(&empty[stage]);
       fence_proxy_async();  // generic-proxy smem writes -> visible to wgmma
       wg_consumers_sync();
@@ -248,17 +393,7 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
         atomicAdd(p.db + ch + 8, dsa1);
       }
     }
-    if constexpr (NB <= 64) {
-      if (dbB) {  // lane = pixel row tp of the stage
-#pragma unroll
-        for (int i = 0; i < NB / 8; ++i) {
-          float s = dsb[i];
-#pragma unroll
-          for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-          if (lane == 0) atomicAdd(p.db + nt * NB + (i >> 2) * 32 + tq * 4 + (i & 3), s);
-        }
-      }
-    }
+    flush_dsb();
     wg_consumers_sync();  // every MMA has retired: ring and operand buffers are free for the staging tile
     // registers -> 128B-swizzled staging tile -> TMA reduce-add of the partial tile into partial[job][m'][n']
     store_acc_sw128<NB>(smem, acc, half * 64);
@@ -377,6 +512,7 @@ struct WgPlan {
   int s_is_a, NB, mtiles, ntiles, mtotal, ldn, njobs, bwl, bhl, tiles_w, tiles_h, tiles_total, nsplits, tps, Ho, Wo;
   int sch, dch;  // channels of the shifted / dense operand
   int ipb;
+  int phase_major;  // the x2 upsample fold with x as A and boxes at least 8 pixels wide: four taps per CTA
 };
 
 static bool wg_plan(const b200gan_conv_geom *g, WgPlan &pl) {
@@ -442,12 +578,20 @@ static bool wg_plan(const b200gan_conv_geom *g, WgPlan &pl) {
   }
   pl.tps = ceil_div(pl.tiles_total, ns);
   pl.nsplits = ceil_div(pl.tiles_total, pl.tps);
+  // x as A (then B = dy has NB <= 64) and an 8-pixel k slice inside one box row: the four taps of a phase share one dy
+  // transpose and one x halo box (same grid: quarter q of a split's tiles in place of tap q)
+  pl.phase_major = up2 && pl.s_is_a && pl.bwl >= 3;
   return true;
 }
 
 int tc_wgrad_supported(const b200gan_conv_geom *g) {
   WgPlan pl;
   return wg_plan(g, pl) ? 1 : 0;
+}
+
+int tc_wgrad_phase_major(const b200gan_conv_geom *g) {
+  WgPlan pl;
+  return wg_plan(g, pl) && pl.phase_major ? 1 : 0;
 }
 
 size_t tc_wgrad_workspace_floats(const b200gan_conv_geom *g) {
@@ -507,7 +651,7 @@ int tc_wgrad(const b200gan_conv_geom *g, const float *x, const float *dy, float 
   p.bw_log2 = pl.bwl; p.bh_log2 = pl.bhl;
   p.tiles_w = pl.tiles_w; p.tiles_h = pl.tiles_h; p.N = g->N; p.imgs_per_box = pl.ipb;
   p.tiles_total = pl.tiles_total; p.tiles_per_split = pl.tps;
-  p.s_is_a = pl.s_is_a; p.mtiles = pl.mtiles; p.ntiles = pl.ntiles; p.ldn = pl.ldn; p.mtotal = pl.mtotal;
+  p.s_is_a = pl.s_is_a; p.phase_major = pl.phase_major; p.mtiles = pl.mtiles; p.ntiles = pl.ntiles; p.ldn = pl.ldn; p.mtotal = pl.mtotal;
   p.partial = ws;
   p.db = db;
 
@@ -526,7 +670,9 @@ int tc_wgrad(const b200gan_conv_geom *g, const float *x, const float *dy, float 
       dims[0] = 2 * Cs; dims[1] = Ws / 2; dims[2] = 2; dims[3] = Hs / 2; dims[4] = g->N;
       strides[0] = 2 * Cs * 4; strides[1] = Ws * Cs * 4; strides[2] = 2 * Ws * Cs * 4; strides[3] = Hs * Ws * Cs * 4;
     }
-    if (int e = make_tmap_f32(&tmX, sptr, 5, dims, strides, box)) return e;
+    // phase-major: the halo box of a stage's x windows, one pixel wider and taller than the dy box
+    const uint32_t hbox[5] = {32, (uint32_t)(1 << pl.bwl) + 1, 1, (uint32_t)(1 << pl.bhl) + 1, (uint32_t)pl.ipb};
+    if (int e = make_tmap_f32(&tmX, sptr, 5, dims, strides, pl.phase_major ? hbox : box)) return e;
   }
   {
     uint64_t dims[5], strides[4];
